@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""bench.py -- headline benchmark of the B200 DEFLATE engine (contract: see the task statement).
+"""bench.py -- headline benchmark of the DEFLATE engine on one or more H100s.
 
 metric  : deflate level-6 GiB/s of raw input on silesia-small.tar (BASELINE.json), zlib wrapper, windowBits 15,
           one deflate(Z_FINISH)-equivalent call per stream -- configs[1].
@@ -8,8 +8,11 @@ step    : every rank compresses one copy of silesia-small.tar (15,736,320 B).  N
 value   : device-timed (CUDA events), input and output resident in HBM.
 e2e     : the same job through the zlib C ABI (compress2) with pinned HOST buffers, copies inside the timed region.
 roofline: k_match (the dominant kernel): algorithmic bytes = the raw input each full launch must read once.
---impl reference : the reference's CPU implementation of the path (the oracle restatement -- zlib-rs itself cannot
-          be built here, see DESIGN.md) on the host cores, same workload.
+--impl reference : the reference's CPU implementation of the path (oracle/, its restatement in C, see DESIGN.md) on the
+          host cores, same workload.
+--dump-outputs DIR : after the timed steps, writes the compressed stream of the last timed step as DIR/deflate_out.npy
+          (float32, one element per byte), so that two builds can be compared output for output.
+The bench writes nothing into the source tree: the host-native oracle build goes to a temporary directory.
 """
 import argparse
 import ctypes
@@ -26,6 +29,8 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 GIB = float(1 << 30)
+HBM_PEAK_GBS = 3350.0  # H100 SXM data sheet, HBM3
+HBM_PEAK_SOURCE = "H100 SXM data sheet: 3.35 TB/s HBM3"
 METRIC = "deflate_level6_raw_input_throughput_silesia_small_tar"
 
 
@@ -40,21 +45,23 @@ _oracle = {}
 
 
 def oracle_compress_fn():
-    """The CPU arm: oracle/ (C restatement of zlib-rs) compiled for THIS host's instruction set; falls back to the portable build
-    the tests use.  Returns (compress(data, level) -> (rc, bytes), flags description)."""
+    """The CPU arm: oracle/ (C restatement of zlib-rs) compiled for THIS host's instruction set into a temporary directory; falls
+    back to the portable build the tests use.  Returns (compress(data, level) -> (rc, bytes), flags description)."""
     if "fn" in _oracle:
         return _oracle["fn"], _oracle["flags"]
-    import hashlib
+    import shutil
+    import tempfile
     import oracle_lib as O
     fn, flags = O.compress, ORACLE_FLAGS["portable"]
     try:
-        model = [l for l in open("/proc/cpuinfo") if l.startswith(("model name", "flags"))][:2]
-        tag = hashlib.sha1("".join(model).encode()).hexdigest()[:10]
-        so = os.path.join(ROOT, "oracle", "_build", "libzoracle_native_%s.so" % tag)
-        if not os.path.exists(so):
-            subprocess.check_call(["make", "-C", os.path.join(ROOT, "oracle"), "native", "NATIVE_TAG=" + tag], stdout=subprocess.DEVNULL,
+        tmp = tempfile.mkdtemp(prefix="zb_bench_")
+        try:
+            so = os.path.join(tmp, "libzoracle_native.so")
+            subprocess.check_call(["make", "-C", os.path.join(ROOT, "oracle"), "native", "NATIVE_SO=" + so], stdout=subprocess.DEVNULL,
                                   stderr=subprocess.DEVNULL)
-        L = ctypes.CDLL(so)
+            L = ctypes.CDLL(so)
+        finally:
+            shutil.rmtree(tmp, ignore_errors=True)  # the loaded library stays mapped
         sz = ctypes.c_size_t
         L.zo_compress_ex.argtypes = [ctypes.c_char_p, ctypes.POINTER(sz), ctypes.c_char_p, sz] + [ctypes.c_int] * 5
 
@@ -188,7 +195,11 @@ def main():
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the compressed stream of the last timed step to DIR/deflate_out.npy (float32)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         return run_reference(args)
 
@@ -211,7 +222,7 @@ def main():
     W = max(args.warmup, 3)
     K = args.steps
 
-    # rotating inputs (10 copies = 157 MB > 126 MB L2) so the raw bytes come from HBM every step
+    # rotating inputs (10 copies = 157 MB > 50 MB L2) so the raw bytes come from HBM every step
     ROT = 10
     host = torch.frombuffer(bytearray(tar), dtype=torch.uint8)
     ins = []
@@ -279,6 +290,11 @@ def main():
         ms, res = step(W + i, True)
         dev_ms += ms
     torch.cuda.synchronize()
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        stream = out_t[: int(res.out_bytes)].cpu().numpy()
+        np.save(os.path.join(args.dump_outputs, "deflate_out.npy"), stream.astype(np.float32))
     if dist:
         dist.barrier()
     wall_ms = (time.perf_counter() - t0) * 1e3
@@ -317,28 +333,12 @@ def main():
         _, res = eng.deflate(ins[0].data_ptr(), n=N, level=6, src_on_device=True, dst=out_t.data_ptr(), dst_cap=cap, dst_on_device=True)
         prof = eng.get_profile()
         eng.set_profile(False)
-        peaks = os.path.join(ROOT, "MEASURED_PEAKS.json")
-        if os.path.exists(peaks):
-            peak, peak_src = float(json.load(open(peaks))["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (burst)"
-        else:
-            peak, peak_src = 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md)"
+        peak, peak_src = HBM_PEAK_GBS, HBM_PEAK_SOURCE
         m = prof["match"]
         full_ms = prof.get("match_first", {"ms": m["ms"] / max(m["launches"], 1)})["ms"]
         achieved = N / (full_ms * 1e-3) / 1e9
-        # dram__bytes_read+write of one full k_match launch from the committed `ncu --set full` capture -- only if that capture
-        # was made from THIS build of the kernels (sha256 of zb_kernels.cu recorded beside the number), else null
-        traffic, traffic_note = None, None
-        tp = os.path.join(ROOT, "profiles", "k_match_traffic.json")
-        if os.path.exists(tp):
-            import hashlib
-            tj = json.load(open(tp))
-            src_sha = hashlib.sha256(open(os.path.join(ROOT, "zlib_rs_b200", "csrc", "zb_kernels.cu"), "rb").read()).hexdigest()
-            if tj.get("kernels_sha256") == src_sha:
-                traffic, traffic_note = tj.get("dram_bytes_per_launch"), tj.get("capture")
-            else:
-                traffic_note = "profiles/k_match_traffic.json was captured from another build of zb_kernels.cu"
         roof = {"bound": "hbm", "kernel": "k_match", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                "traffic": traffic, "traffic_source": traffic_note, "peak_source": peak_src, "algorithmic_bytes_per_launch": N, "launch_ms": full_ms,
+                "traffic": None, "traffic_source": "not measured", "peak_source": peak_src, "algorithmic_bytes_per_launch": N, "launch_ms": full_ms,
                 "phases_ms": {k: round(v["ms"], 4) for k, v in prof.items()}, "iterations": int(res.iterations)}
 
     # One stream cut into `world` contiguous ranges (SURVEY.md 8e, BASELINE config 4): every rank compresses its range as a raw
@@ -411,7 +411,7 @@ def main():
             other = {}
             best = min(eng.inflate(gz, N)[2].gpu_ms for _ in range(3))
             rc, got, r3 = eng.inflate(gz, N)
-            peak_i = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"]) if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else 6650.0
+            peak_i = HBM_PEAK_GBS
             alg = len(gz) + N  # SURVEY.md 8(d): compressed bytes in + raw bytes out
             other["inflate_silesia_small_tar_gz"] = {"ms": best, "out_GBps": N / best / 1e6, "bit_exact": bool(rc == 0 and got == tar),
                                                      "gpu_launches": int(r3.gpu_launches), "note": "config 3; host buffers, copies inside the timed region",
@@ -487,7 +487,7 @@ def main():
             "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "u8",
             "data": "silesia-small.tar (reference corpus, committed as data/silesia-small.tar.gz)",
             "config": {"workload": workload(world), "parity": "output byte-identical to the reference's compress2 (sha256 pinned in tests/)",
-                       "l2": "inputs rotate over 10 device copies (157 MB > 126 MB L2); ~480 MB of intermediates per step",
+                       "l2": "inputs rotate over 10 device copies (157 MB > 50 MB L2); ~480 MB of intermediates per step",
                        "compressed_bytes": out_bytes, "wall_ms_per_step": wall_ms / K,
                        "parallelism": "1 stream per GPU" + (", NCCL all-gather of compressed segments" if world > 1 else "")},
             "clocks": clocks,

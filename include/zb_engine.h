@@ -1,5 +1,5 @@
 /*
- * zb_engine.h -- low-level C ABI of the B200 DEFLATE engine (libz_b200.so).
+ * zb_engine.h -- low-level C ABI of the GPU DEFLATE engine (libz_b200.so).
  *
  * Plain pointers and sizes only.  This is the layer the zlib-compatible entry points in zlib_b200.h are
  * built on, and what a Rust `zlib-rs` FFI shim would bind for the hot path (see INTEGRATION.md):

@@ -1,5 +1,5 @@
 /*
- * zlib_b200.h -- the zlib C ABI as exported by libz_b200.so (the B200 DEFLATE engine).
+ * zlib_b200.h -- the zlib C ABI as exported by libz_b200.so (the GPU DEFLATE engine).
  *
  * This header declares, with the reference's exact signatures and struct layout, the entry points of
  * libz-rs-sys (zlib-rs's `extern "C"` layer) that this library replaces.  A C program written against

@@ -2,7 +2,7 @@
  * zo_deflate.c -- oracle (TEST INFRASTRUCTURE ONLY, see zoracle.h).
  *
  * Plain-C restatement of the reference's deflate engine.  Each function cites
- * the zlib-rs file:line it follows (paths relative to /root/reference/).
+ * the zlib-rs file:line it follows (paths relative to the root of a zlib-rs checkout).
  * The compressed bytes must equal zlib-rs's (== zlib-ng's) for every level
  * and strategy; this is pinned by tests/golden/kat.json.
  */

@@ -1,4 +1,4 @@
-"""Inflate timing on the GPU box: device-resident zlib/gzip streams -> device output (scripts/gpu_quick helper)."""
+"""Inflate timing on the GPU: zlib/gzip streams of the corpus through Engine.inflate; prints one line per case and a JSON summary."""
 import sys, os, zlib, hashlib, json
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
@@ -26,5 +26,4 @@ for name, (comp, plain, wb) in cases.items():
     out[name] = {"ok": ok, "rc": rc, "gpu_ms": round(best, 3), "launches": res.gpu_launches,
                  "out_MBps": round(len(plain) / best / 1e3, 1), "in_bytes": len(comp), "out_bytes": len(plain)}
     print(name, out[name], flush=True)
-os.makedirs("gpurun_out", exist_ok=True)
-json.dump(out, open("gpurun_out/inflate_bench.json", "w"), indent=1)
+print(json.dumps(out))

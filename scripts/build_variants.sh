@@ -5,7 +5,7 @@ set -e
 cd "$(dirname "$0")/../zlib_rs_b200/csrc"
 make -j8 > /dev/null
 mkdir -p ../variants _build/var
-ARCH="-gencode arch=compute_100a,code=sm_100a"
+ARCH="-gencode arch=compute_90a,code=sm_90a"
 for spec in "$@"; do
   name=${spec%%:*}; flags=${spec#*:}
   ( nvcc $ARCH -std=c++17 -O3 -lineinfo -Xcompiler -fPIC -Xcompiler -fvisibility=hidden -diag-suppress 177 -rdc=false $flags -c zb_kernels.cu -o _build/var/zb_kernels_$name.o && nvcc $ARCH -std=c++17 -O3 -lineinfo -Xcompiler -fPIC -Xcompiler -fvisibility=hidden -diag-suppress 177 -rdc=false $flags -c zb_engine.cu -o _build/var/zb_engine_$name.o && nvcc $ARCH -std=c++17 -O3 -lineinfo -Xcompiler -fPIC -Xcompiler -fvisibility=hidden -diag-suppress 177 -rdc=false $flags -c ${SLOW_SRC:-zb_slow.cu} -o _build/var/zb_slow_$name.o &&

@@ -6,7 +6,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 obj = os.path.join(ROOT, "zlib_rs_b200", "csrc", "_build", "zb_kernels.o")
 sass = subprocess.run(["cuobjdump", "-sass", "-fun", "_ZN2zb7k_matchENS_7JobBufsE", obj], capture_output=True, text=True).stdout
 lines = [re.sub(r"\s*/\* 0x[0-9a-f]+ \*/\s*$", "", l.rstrip()) for l in sass.splitlines() if re.match(r"\s+/\*[0-9a-f]{4}\*/", l)]
-out = ["# k_match (sm_100a): cuobjdump -sass excerpts of zlib_rs_b200/csrc/_build/zb_kernels.o (scripts/sass_excerpt.py)",
+out = ["# k_match (sm_90a): cuobjdump -sass excerpts of zlib_rs_b200/csrc/_build/zb_kernels.o (scripts/sass_excerpt.py)",
        "# 1. TMA bulk copy of the data window (cp.async.bulk + mbarrier): UBLKCP.S.G / SYNCS.*", ""]
 for i, l in enumerate(lines):
     if re.search(r"UBLKCP|SYNCS\.|FENCE\.VIEW\.ASYNC|ELECT", l):

@@ -1,8 +1,8 @@
 #!/usr/bin/env python3
 """Extract the reference's literal known-answer vectors into tests/golden/kat.json.
 
-Run in the authoring container (needs /root/reference, which does NOT exist on
-the GPU box):   python tests/golden/extract_vectors.py
+Run where a zlib-rs checkout exists (ZLIB_RS_REFERENCE, default: ../reference beside
+this repository):   python tests/golden/extract_vectors.py
 
 Every vector is a literal in the reference's own Rust test sources; nothing here
 is produced by running code of ours.  The JSON records, per vector, the source
@@ -14,7 +14,7 @@ import os
 import re
 import sys
 
-REF = os.environ.get("ZLIB_RS_REFERENCE", "/root/reference")
+REF = os.environ.get("ZLIB_RS_REFERENCE", os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "..", "..", "reference"))
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "kat.json")
 OS_CODE = 3  # gz_header::OS_CODE on unix, zlib-rs/src/c_api.rs:242-252
 

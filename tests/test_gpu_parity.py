@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box): every call goes through the C ABI of libz_b200.so and is
+"""GPU parity tests (need an H100): every call goes through the C ABI of libz_b200.so and is
 compared with the CPU oracle on the same inputs -- bit-exact for the one-shot path at every level."""
 import hashlib
 import json

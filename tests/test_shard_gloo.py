@@ -1,5 +1,5 @@
 """world_size-2 gloo test (CPU) of the N>1 host logic: shard plan, one all-gather of the compressed segments,
-stitching and check-value combination.  The segment compressor here is the oracle; on the GPU box the same function is
+stitching and check-value combination.  The segment compressor here is the oracle; on a GPU machine the same function is
 driven by Engine.deflate(..., flags=ZB_FLAG_NOT_LAST) (tests/test_gpu_parity.py::test_segments_stitch_like_split_deflate)."""
 import os
 import sys

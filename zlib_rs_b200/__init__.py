@@ -1,6 +1,6 @@
-"""zlib_rs_b200 -- Python host-side mirror of the zlib-rs interface for the B200 DEFLATE engine.
+"""zlib_rs_b200 -- Python host-side mirror of the zlib-rs interface for the GPU DEFLATE engine.
 
-Everything here is a thin ctypes binding of ``libz_b200.so`` (built in-tree from ``csrc/`` for sm_100a).
+Everything here is a thin ctypes binding of ``libz_b200.so`` (built in-tree from ``csrc/`` for sm_90a).
 The names and argument meaning follow the reference's own API for this path:
 
 * ``compress2 / compress / uncompress / compressBound / crc32 / adler32`` and the combine helpers --
@@ -66,7 +66,7 @@ def lib():
     if _lib is None:
         if not os.path.exists(LIB_PATH):
             raise RuntimeError("libz_b200.so is not built: run `python -c 'import __graft_entry__ as g; g.build()'` "
-                               "or `make -C zlib_rs_b200/csrc` (needs nvcc, sm_100a)")
+                               "or `make -C zlib_rs_b200/csrc` (needs nvcc, sm_90a)")
         L = ctypes.CDLL(LIB_PATH, mode=ctypes.RTLD_LOCAL)
         vp, sz, u32, u64, ci = ctypes.c_void_p, ctypes.c_size_t, ctypes.c_uint32, ctypes.c_uint64, ctypes.c_int
         ul = ctypes.c_ulong

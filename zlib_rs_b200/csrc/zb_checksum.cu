@@ -1,4 +1,4 @@
-// zb_checksum.cu -- adler32 / crc32 kernels (sm_100a).
+// zb_checksum.cu -- adler32 / crc32 kernels (sm_90a).
 //
 // Replaces zlib-rs/src/adler32.rs:19-47 (+ SIMD variants) and zlib-rs/src/crc32.rs:19-29 (braid /
 // pclmulqdq folding).  Both checksums are chunk-parallel:
@@ -133,7 +133,7 @@ __device__ __forceinline__ uint32_t x2nmodp(uint64_t n, uint32_t k)
 }
 
 // k_crc_partial.  Byte-sliced table CRC costs one shared-memory lookup per input byte; what else the L1/shared pipe has to do decides
-// the speed (ncu, profiles/r02c: with one contiguous segment per THREAD every 128-bit load touches 32 different lines -- 32 tag
+// the speed (with one contiguous segment per THREAD every 128-bit load touches 32 different lines -- 32 tag
 // cycles per 512 bytes next to the 16 lookup wavefronts).  This version:
 //  * conflict-free lookups: every lane owns a private copy of the four slice tables in its own bank (128 KiB per CTA), laid out so
 //    that a lookup address is one byte-permute of the data word into the table base (crc_lds);
@@ -306,12 +306,27 @@ __global__ void __launch_bounds__(1024) k_crc_final(const uint32_t *part, uint32
 }
 
 // host-side launchers -------------------------------------------------------------------------
+int device_sm_count()
+{
+    static int sm_count[64]; // per device
+    int dev = 0;
+    cudaGetDevice(&dev);
+    dev &= 63;
+    if (sm_count[dev] == 0) {
+        int v = 0;
+        cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
+        sm_count[dev] = v > 0 ? v : 1;
+    }
+    return sm_count[dev];
+}
+
 cudaError_t launch_adler32(const uint8_t *d_buf, uint64_t len, uint32_t start, void *d_scratch, size_t scratch_bytes, uint32_t *d_out,
                            cudaStream_t st)
 {
     uint64_t chunk = 16384, nchunks = 0;
     if (len) {
-        chunk = (len + 148 * 16 - 1) / (148 * 16);
+        const uint64_t parts = (uint64_t)device_sm_count() * 16;
+        chunk = (len + parts - 1) / parts;
         chunk = (chunk + 4095) & ~4095ull;
         if (chunk < 16384) chunk = 16384;
         if (chunk > (1u << 20)) chunk = 1u << 20;
@@ -326,18 +341,16 @@ cudaError_t launch_adler32(const uint8_t *d_buf, uint64_t len, uint32_t start, v
 cudaError_t launch_crc32(const uint8_t *d_buf, uint64_t len, uint32_t start, void *d_scratch, size_t scratch_bytes, uint32_t *d_out,
                          cudaStream_t st)
 {
-    static int sm_count[64]; // per device; the opt-in for 128 KiB of dynamic shared memory is per device too
+    static bool smem_opt_in[64]; // the opt-in for 128 KiB of dynamic shared memory is per device
     int dev = 0;
     cudaGetDevice(&dev);
     dev &= 63;
-    if (sm_count[dev] == 0) {
-        int v = 0;
-        cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
+    if (!smem_opt_in[dev]) {
         cudaError_t e = cudaFuncSetAttribute(k_crc_partial, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kCrcTabBytes);
         if (e != cudaSuccess) return e;
-        sm_count[dev] = v > 0 ? v : 148;
+        smem_opt_in[dev] = true;
     }
-    const int n_sm = sm_count[dev];
+    const int n_sm = device_sm_count();
     // main part: up to the last 16-byte boundary; the rest (< 16 bytes) is appended by k_crc_final
     uint32_t tail_len = (uint32_t)((reinterpret_cast<uintptr_t>(d_buf) + len) & 15u);
     if (tail_len > len) tail_len = (uint32_t)len;

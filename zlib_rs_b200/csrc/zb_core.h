@@ -1,4 +1,4 @@
-// zb_core.h -- per-position logic of the B200 deflate engine (level 3..6 "deflate_medium" path).
+// zb_core.h -- per-position logic of the GPU deflate engine (level 3..6 "deflate_medium" path).
 //
 // Everything here is `__host__ __device__`: the CUDA kernels in zb_kernels.cu call these functions on
 // the device; tests/hostmodel compiles the same header with g++ to unit-test the parallel algorithm on

@@ -1,4 +1,4 @@
-// zb_engine.cu -- host orchestration of the B200 DEFLATE engine and the low-level C ABI (zb_engine.h).
+// zb_engine.cu -- host orchestration of the GPU DEFLATE engine and the low-level C ABI (zb_engine.h).
 // Host code only allocates, copies and launches; every byte of compute happens in kernels.
 #include <cuda_runtime.h>
 #include <stdio.h>
@@ -391,7 +391,7 @@ int Engine::deflate(const void *src, size_t n_in, bool src_dev, void *dst, size_
     CK(cudaEventRecord(ev0, st));
     if (profile) { for (int i = 0; i < kPhases; i++) { phase_ms[i] = 0; phase_launches[i] = 0; } }
     // A host input of some size for the chain-based levels arrives in chunks on the second stream; the link pass of a tile starts
-    // as soon as its bytes are there (the upload of 15.7 MB takes 0.6 ms, the link pass 0.4: they overlap instead of adding up).
+    // as soon as its bytes are there (the upload and the link pass overlap instead of adding up).
     uint32_t up_chunks = 0;
     size_t up_len[kUpChunks] = {0};
     static const bool up_off = getenv("ZB_UPLOAD_CHUNKED") && atoi(getenv("ZB_UPLOAD_CHUNKED")) == 0; // measurement switch
@@ -400,7 +400,7 @@ int Engine::deflate(const void *src, size_t n_in, bool src_dev, void *dst, size_
     if (chunked_upload) {
         // a chunk is at least one wave of the link kernel (one CTA per tile and SM): smaller launches only add CTA latencies
         size_t chunk = (n_in / kUpChunks + kLinkTile - 1) / kLinkTile * kLinkTile;
-        if (chunk < (size_t)148 * kLinkTile) chunk = (size_t)148 * kLinkTile;
+        if (chunk < (size_t)device_sm_count() * kLinkTile) chunk = (size_t)device_sm_count() * kLinkTile;
         CK(cudaStreamWaitEvent(st2, ev0, 0));
         for (size_t off = 0; off < n_in; off += chunk) {
             const size_t len = n_in - off < chunk ? n_in - off : chunk;
@@ -501,7 +501,7 @@ int Engine::deflate(const void *src, size_t n_in, bool src_dev, void *dst, size_
                     if (jb.slow_mode == 2) k_rle<<<(N + 255) / 256, 256, 0, st>>>(jb);
                     else {
                         // positions per CTA.  A CTA lasts about as long as its most expensive node (at level 9 single lazy chains
-                        // cost milliseconds), so the level with the longest searches takes the largest pieces (measured, r3g/r3h)
+                        // cost milliseconds), so the level with the longest searches takes the largest pieces
                         static const char *e_ss = getenv("ZB_SLOW_SUB");
                         jb.match_sub = e_ss ? (uint32_t)atoi(e_ss) : level >= 9 ? ZB_SLOW_SUB9 : level == 8 ? 4096u : 8192u;
                         k_slow<<<(N + jb.match_sub - 1) / jb.match_sub, 1024, (kWSize + jb.match_sub + kSlowAhead) * 3, st>>>(jb);
@@ -534,7 +534,7 @@ int Engine::deflate(const void *src, size_t n_in, bool src_dev, void *dst, size_
                     if (iters == 1) jb.match_sub = ZB_MATCH_CTX ? 8192 : 4096; // context schedule: one CTA of 1024 threads per SM
                     else if (n_dirty <= ZB_TAIL_TILES) { jb.match_sub = ZB_TAIL_SUB; mthreads = 256; }
                     else {
-                        const uint64_t per_cta = (uint64_t)n_dirty * kMatchTile / (4 * 148);
+                        const uint64_t per_cta = (uint64_t)n_dirty * kMatchTile / (4 * (uint64_t)device_sm_count());
                         jb.match_sub = per_cta >= 8192 ? 8192 : per_cta >= 4096 ? 4096 : per_cta >= 2048 ? 2048 : 1024;
                     }
                     {   // experiment knobs for the dense passes (not part of the interface)
@@ -848,7 +848,7 @@ int zb_device_fill_random(zb_engine *z, void *dst, size_t bytes, uint64_t seed)
 {
     if (!z) return ZB_E_NODEVICE;
     cudaSetDevice(z->e.device);
-    zb::k_fill_random<<<148 * 8, 256, 0, z->e.st>>>(static_cast<uint64_t *>(dst), bytes / 8, seed);
+    zb::k_fill_random<<<zb::device_sm_count() * 8, 256, 0, z->e.st>>>(static_cast<uint64_t *>(dst), bytes / 8, seed);
     return cudaStreamSynchronize(z->e.st) == cudaSuccess ? ZB_OK : ZB_E_CUDA;
 }
 

@@ -1,4 +1,4 @@
-// zb_huff.h -- per-block Huffman construction and block framing of the B200 deflate engine.
+// zb_huff.h -- per-block Huffman construction and block framing of the GPU deflate engine.
 //
 // `__host__ __device__` like zb_core.h (device: one thread per block in k_build_blocks; host: unit tests).
 // Restates, bit-exactly, zng_tr_flush_block and friends: build_tree / Heap / gen_bitlen / gen_codes

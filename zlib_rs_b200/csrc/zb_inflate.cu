@@ -1,4 +1,4 @@
-// zb_inflate.cu -- GPU inflate (sm_100a), round-1 version: one warp per stream.
+// zb_inflate.cu -- GPU inflate (sm_90a), round-1 version: one warp per stream.
 //
 // Reference: zlib-rs/src/inflate.rs (Mode machine :896-1839, inflate_fast_help :1880-2158),
 // inflate/inftrees.rs:42-245 (two-level decode tables), inflate/writer.rs (match copy),
@@ -1307,7 +1307,8 @@ int Engine::inflate(const void *src, size_t n, bool src_dev, void *dst, size_t d
                 if ((rc = reserve(4 /*S_M*/, (hpar.total_out + 64) * 2, &p)) != ZB_OK) return rc;
                 dtmp = static_cast<uint16_t *>(p);
                 const uint64_t quads = (hpar.total_out + 1023) / 1024;
-                const unsigned rgrid = (unsigned)(quads < 148 * 16 ? (quads ? quads : 1) : 148 * 16);
+                const uint64_t rmax = (uint64_t)device_sm_count() * 16;
+                const unsigned rgrid = (unsigned)(quads < rmax ? (quads ? quads : 1) : rmax);
                 uint32_t *dcum = nullptr;
                 if (darena && hpar.all_kept && !getenv("ZB_INFLATE_BLOCKWISE") &&
                     reserve(37 /* inflate cumulative offsets */, (size_t)hpar.ncand * kSlotSyms * 4, &p) == ZB_OK)

@@ -1,4 +1,4 @@
-// zb_kernels.cu -- CUDA kernels of the B200 deflate engine (compiled for sm_100a only).
+// zb_kernels.cu -- CUDA kernels of the GPU deflate engine (compiled for sm_90a).
 //
 // Pipeline for one level-3..6 job (DESIGN.md has the full picture):
 //   k_links2/fix L[x]   : previous position with the same 4-byte hash (the reference's head/prev chains)
@@ -269,9 +269,8 @@ __global__ void __launch_bounds__(1024) k_skip(JobBufs jb)
         }
     }
     __syncthreads();
-    // Pointer jumping over the staged window.  Measured alternatives (r2e, r2h): visiting only the set bits of the hole bitmap
-    // (0.13 instead of 0.07..0.11 ms per launch) and one serial walk per position through the holes (0.62 ms on the hole-dense
-    // tiles of the first iterations) were both slower than this dense sweep.
+    // Pointer jumping over the staged window.  Alternatives tried earlier, on another GPU: visiting only the set bits of the hole
+    // bitmap and one serial walk per position through the holes were both slower than this dense sweep.
     // Warp w owns the bitmap words [64 w, 64 w + 64), lane l the bit l of each; it first notes which of its words hold a hole in
     // play at all (two ballots) and then visits only those, IN ASCENDING ORDER and each until it is stable: a jump is extended by the
     // jump of its target, and targets lie below -- within the warp's range they are final by the time they are used, so a chain
@@ -361,15 +360,15 @@ constexpr uint32_t kMatchSmem = kMatchData + (kWSize + kMatchSub) * 2 + ((kWSize
 #define ZB_SECOND_LOOK 1
 #endif
 #ifndef ZB_CMP16
-#define ZB_CMP16 0 // 16 bytes per compare step instead of 8: measured equal (r3a: 9.01 vs 8.98 ms), the simpler one stays
+#define ZB_CMP16 0 // 16 bytes per compare step instead of 8: measured equal on another GPU, the simpler one stays
 #endif
 #ifndef ZB_DRAIN
 #define ZB_DRAIN 0 // with the piece used up and at most this many lanes of a warp still walking, the warp shares their walks (0: off).
-                   // Measured (r2y): 8 changes nothing (9.26 vs 9.23 ms), 32 costs 4 ms -- off
+                   // Measured on another GPU: 8 changed nothing, 32 was slower -- off
 #endif
 #ifndef ZB_COOP_CMP
 #define ZB_COOP_CMP 4 // stragglers: with at most this many lanes still busy, the warp finishes a long compare together
-                      // (256 bytes per step).  Offering it to every compare burst was measured slower (r2p: +0.26 ms at 12 lanes).
+                      // (256 bytes per step).  Offering it to every compare burst was measured slower on another GPU.
 #endif
 constexpr uint32_t kBatch = ZB_T_IDLE;         // idle lanes that trigger a refill
 constexpr uint32_t kBatchCmp = ZB_T_CMP;       // pending lanes that trigger a compare burst
@@ -1185,8 +1184,8 @@ __device__ __forceinline__ bool path_tile_dirty(const JobBufs &jb, uint32_t pt)
 __global__ void __launch_bounds__(1024) k_nxt(JobBufs jb)
 {
     // 16 CTAs per path tile, one position per thread; CTAs of clean tiles exit at once.  (Staging M and the nearby data bytes of a
-    // CTA's 1024 positions in shared memory was measured slower, 2.1 instead of 1.4 ms over the twelve passes: the threads that
-    // have work are few in the later passes and the loads of the first pass are not what bounds it.)
+    // CTA's 1024 positions in shared memory was measured slower on another GPU: the threads that have work are few in the later
+    // passes and the loads of the first pass are not what bounds it.)
     constexpr uint32_t per = kPathTile / 1024;
     const uint32_t tile = jb.nxt_list ? jb.nxt_list[blockIdx.x / per] : blockIdx.x / per;
     if (!path_tile_dirty(jb, tile)) return;

@@ -1,4 +1,4 @@
-// zb_kernels.cuh -- CUDA kernels of the B200 deflate engine (sm_100a).  See DESIGN.md for the data
+// zb_kernels.cuh -- CUDA kernels of the GPU deflate engine (sm_90a).  See DESIGN.md for the data
 // flow.  All device logic that has reference semantics lives in zb_core.h / zb_huff.h; the kernels
 // here provide the parallel schedule, shared-memory staging and the bit packing.
 #pragma once
@@ -25,7 +25,7 @@ constexpr uint32_t kPathHead = ZB_PATH_HEAD; // leading positions of a path tile
 constexpr uint32_t kChainChunkTiles = ZB_PATH_HEAD > 64 ? 96 : 320; // tiles per staged chunk of that table in k_path_chain
 #ifndef ZB_MATCH_CTX
 #define ZB_MATCH_CTX 0 // k_match schedule: 0 = one walk context per lane in registers; 1 = contexts in shared memory, rounds of one kind per
-                       // warp (experiment, measured slower: first pass 2.45..2.7 ms against 1.98 ms, r2r)
+                       // warp (experiment, measured slower on another GPU)
 #endif
 #ifndef ZB_CTX
 #define ZB_CTX 4       // contexts per lane (16 bytes of shared memory each)
@@ -121,6 +121,7 @@ struct JobBufs {
 };
 
 cudaError_t upload_tables();
+int device_sm_count(); // streaming multiprocessors of the current device: grids meant to fill the GPU once are sized from it
 cudaError_t launch_adler32(const uint8_t *d_buf, uint64_t len, uint32_t start, void *d_scratch, size_t scratch_bytes, uint32_t *d_out,
                            cudaStream_t st);
 cudaError_t launch_crc32(const uint8_t *d_buf, uint64_t len, uint32_t start, void *d_scratch, size_t scratch_bytes, uint32_t *d_out,

@@ -1,4 +1,4 @@
-// zb_slow.cu -- kernels of the level 7..9 path (deflate_slow, lazy matching; sm_100a).
+// zb_slow.cu -- kernels of the level 7..9 path (deflate_slow, lazy matching; sm_90a).
 //
 //   k_links2_roll L[x]   : previous position with the same rolling 3-byte hash (level 9; levels 7/8 use k_links2_std; zb_kernels.cu)
 //   k_slow        nxt[p] : macro step of the lazy parser from every position taken as a fresh loop-top
@@ -49,7 +49,7 @@ constexpr uint32_t kSlowBatch = 8;
 #define ZB_COOP_START 16
 #endif
 #ifndef ZB_MONSTER
-#define ZB_MONSTER 0x7fffffff // off: measured (r3k, r3l) 64 -> 135 ms, 256..2048 -> 120..133 ms against 116..123 ms without, run-to-run spread 5 %
+#define ZB_MONSTER 0x7fffffff // off: not faster at any threshold from 64 to 2048 when measured on another GPU
 #endif
 constexpr uint32_t kMonster = ZB_MONSTER; // candidates after which the warp takes over a lane's search (level 9; 0x7fffffff: never)
 constexpr uint32_t kCoopStart = ZB_COOP_START; // prev_length from which the warp shares a lane's re-rooting scan (level 9)
@@ -151,9 +151,8 @@ __global__ void __launch_bounds__(1024) k_slow(JobBufs jb)
     // The search semantics are those of the round-1 kernel; the schedule is the one measured on k_match (zb_kernels.cu).
     if (sp.slow) {
         // Level 9 (rolling hash, longest_match_slow): the round-1 schedule -- one phase per pass, START and PEND before the walk, the
-        // walk step with the byte filter and the 3/4-byte pre-check.  The round-2 schedule below was measured slower here (133 vs
-        // 160..176 ms for the corpus: the re-rooting loops of START / PEND dominate and do not mix well with the unrolled burst),
-        // and faster at levels 7 / 8 (11.3 -> 7.3 ms, 29.5 -> 19.3 ms).
+        // walk step with the byte filter and the 3/4-byte pre-check.  The round-2 schedule below was measured slower here on another
+        // GPU (the re-rooting loops of START / PEND dominate and do not mix well with the unrolled burst), and faster at levels 7 / 8.
         constexpr uint32_t kBurst9 = 4;
     for (;;) {
         const uint32_t m_idle = __ballot_sync(0xffffffffu, state == SS_IDLE);
@@ -300,7 +299,7 @@ __global__ void __launch_bounds__(1024) k_slow(JobBufs jb)
             // 2. the re-rooting of a long match, shared by the warp, one lane's at a time.  Serially it is a scan over the len - 2
             // windows of the match (one link each, a running minimum with an exit test at every new minimum) and one head_at() walk
             // of up to len hops -- per ACCEPTED candidate, and on record-like data a search accepts hundreds: single lanes spent
-            // 10^8 cycles here and one SM stayed busy eight times as long as the average (profiles/r3_tail_iteration_digests.txt).
+            // 10^8 cycles here and one SM stayed busy eight times as long as the average.
             {
                 uint32_t mb = __ballot_sync(0xffffffffu, reroot && len >= kCoopStart);
                 uint32_t *tab = s_tab[tid >> 5];

@@ -517,7 +517,7 @@ int deflatePrime(z_streamp strm, int bits, int value)
     if (!d) return Z_STREAM_ERROR;
     if (bits < 0 || bits > 32) return Z_BUF_ERROR;
     if (bits == 0) return Z_OK;
-    if (d->wrap != 0 && !d->header_done) { strm->msg = "deflatePrime before the stream header is not implemented by the B200 engine"; return Z_STREAM_ERROR; }
+    if (d->wrap != 0 && !d->header_done) { strm->msg = "deflatePrime before the stream header is not implemented by the GPU engine"; return Z_STREAM_ERROR; }
     uint64_t buf = (uint64_t)d->carry_val | (((uint64_t)(uint32_t)value & ((bits == 32 ? 0ull : (1ull << bits)) - 1ull)) << d->carry_bits);
     uint32_t nb = d->carry_bits + (uint32_t)bits;
     while (nb >= 8) { d->out.push_back((uint8_t)buf); buf >>= 8; nb -= 8; }
@@ -600,7 +600,7 @@ int deflateTune(z_streamp strm, int good_length, int max_lazy, int nice_length, 
                                    {8, 16, 128, 128}, {8, 32, 128, 256}, {32, 128, 258, 1024}, {32, 258, 258, 4096}};
     const int *t = tab[d->level];
     if (good_length == t[0] && max_lazy == t[1] && nice_length == t[2] && max_chain == t[3]) return Z_OK;
-    strm->msg = "deflateTune: matcher parameters other than the level's own are not implemented by the B200 engine";
+    strm->msg = "deflateTune: matcher parameters other than the level's own are not implemented by the GPU engine";
     return Z_STREAM_ERROR;
 }
 
