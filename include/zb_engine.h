@@ -127,6 +127,61 @@ typedef struct zb_inflate_seg {
 ZB_API int zb_inflate_blocks(zb_engine *e, const void *src, size_t src_len, uint64_t start_bit, const void *dict, size_t dict_len,
                              void *dst, size_t dst_cap, int check_kind, uint32_t check_start, zb_inflate_seg *out);
 
+/* Chunk-sharded deflate with the one-stream bytes (levels 7..9; see DESIGN.md §5).  One input of total_len bytes is cut into
+ * contiguous ranges [S_r, E_r), one per rank (every range but the last >= 64 KiB); each rank runs the four calls below on its
+ * own engine, and the caller moves the small records between them (the library has no transport):
+ *
+ *   1. zb_shard_parse   parses the range with its left and right context and fills the entry table: for each of the
+ *                       ZB_SHARD_CAND positions S_r + i where the serial parser can enter the range, the position where it
+ *                       leaves it (>= E_r) and the symbols it emits on the way.  The caller all-gathers the tables and composes
+ *                       them: e_0 = 0, e_{r+1} = T_r[e_r - S_r].exit, O_r = sum of T_q[e_q - S_q].count over q < r.
+ *   2. zb_shard_symbols emits the symbols from the true entry e_r (global symbol index O_r + i) and returns the edge records of the
+ *                       first and last deflate block they fall in (blocks are cut every (1 << (memLevel + 6)) - 1 symbols of the
+ *                       whole stream).  The caller all-gathers the records, two per rank, in rank order.
+ *   3. zb_shard_size    builds the trees of every block the rank touches (merged histograms for blocks shared with other ranks,
+ *                       so all ranks reach the same trees and block types) and returns the bit span of the rank's part: header
+ *                       where it holds a block's first symbol, its symbols, the end-of-block code where it holds the block's end;
+ *                       a stored block is written whole by the holder of its first symbol.  A span is a function of the start
+ *                       offset (stored blocks pad to a byte): end = aligned ? ((start + pre_bits + 7) & ~7) + post_bits
+ *                                                                         : start + pre_bits.
+ *                       The caller all-gathers the spans; offset_0 = 0, offset_{r+1} = end_r(offset_r).
+ *   4. zb_shard_encode  writes the part starting at bit (bit_offset & 7) of its first byte; byte 0 of the part is byte
+ *                       bit_offset >> 3 of the raw deflate stream, and the seams are joined by OR-ing the one shared byte.
+ *
+ * The stitched raw stream, behind the zlib header 78 da and in front of the adler32 trailer (adler32_combine of the ranges'
+ * checksums from zb_shard_parse), is byte for byte compress2(data, level) of zlib-rs for levels 7, 8 and 9, strategies
+ * Z_DEFAULT_STRATEGY, Z_FILTERED and Z_FIXED, windowBits 15 and memLevel 1..9, whatever the number of ranges and wherever
+ * the cuts are.  Other parameters give ZB_E_PARAM.  The shard state lives in the engine between the calls: a call out of
+ * order, or any other engine call in between, gives ZB_E_PARAM. */
+#define ZB_SHARD_CAND 513 /* a macro step spans at most 255 lazy literals + a 258-byte match */
+typedef struct zb_shard_entry {
+    uint32_t exit;  /* first node of the path at or behind range_end (global position) */
+    uint32_t count; /* symbols emitted by the nodes in front of it */
+} zb_shard_entry;
+typedef struct zb_shard_edge {
+    uint32_t block;                 /* global block index; 0xffffffff: the rank has no symbols */
+    uint32_t nsyms;                 /* symbols of this rank in the block */
+    uint32_t first_pos, end_pos;    /* input covered by them: position of the first, end of the last (global) */
+    uint32_t last_pos, last_lit;    /* position of the last one, and whether it is a literal */
+    uint32_t flush_base;            /* window base when the block would be flushed behind that symbol */
+    uint32_t sym_offset, sym_count; /* all symbols of the rank: [sym_offset, sym_offset + sym_count) */
+    uint32_t is_last;               /* the rank owns the end of the input */
+    uint32_t freq[320];             /* literal/length (286) and distance (30) histogram of its symbols in the block */
+} zb_shard_edge;
+typedef struct zb_shard_span {
+    uint64_t pre_bits, post_bits;
+    uint32_t aligned, reserved;
+} zb_shard_span;
+/* flags: ZB_FLAG_MEMLEVEL(m).  src is the whole input (host, or device when src_on_device); only the range's slice and its context
+ * are copied.  table: ZB_SHARD_CAND entries (positions S_r + i at or behind E_r map to themselves with count 0).
+ * adler: adler32 of the range's bytes. */
+ZB_API int zb_shard_parse(zb_engine *e, const void *src, size_t total_len, int src_on_device, size_t range_begin, size_t range_end,
+                          int level, int strategy, uint32_t flags, zb_shard_entry *table, uint32_t *adler);
+ZB_API int zb_shard_symbols(zb_engine *e, uint32_t entry, uint32_t sym_offset, zb_shard_edge *first, zb_shard_edge *last);
+ZB_API int zb_shard_size(zb_engine *e, const zb_shard_edge *all, size_t n, zb_shard_span *span);
+/* bytes: length of the part, ceil(((bit_offset & 7) + part bits) / 8); ZB_E_BUF when cap is smaller. */
+ZB_API int zb_shard_encode(zb_engine *e, uint64_t bit_offset, void *dst, size_t cap, int dst_on_device, uint64_t *bytes);
+
 ZB_API int zb_adler32(zb_engine *e, uint32_t start, const void *buf, size_t len, int on_device, uint32_t *out, float *gpu_ms);
 ZB_API int zb_crc32(zb_engine *e, uint32_t start, const void *buf, size_t len, int on_device, uint32_t *out, float *gpu_ms);
 

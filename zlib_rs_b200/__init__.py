@@ -50,6 +50,24 @@ class InflateResult(ctypes.Structure):
                 ("msg", ctypes.c_char * 64)]
 
 
+SHARD_CAND = 513  # ZB_SHARD_CAND
+
+
+class ShardEntry(ctypes.Structure):
+    _fields_ = [("exit", ctypes.c_uint32), ("count", ctypes.c_uint32)]
+
+
+class ShardEdge(ctypes.Structure):
+    """zb_shard_edge: what one rank knows about a deflate block it shares with other ranks."""
+    _fields_ = [(f, ctypes.c_uint32) for f in ("block", "nsyms", "first_pos", "end_pos", "last_pos", "last_lit", "flush_base",
+                                              "sym_offset", "sym_count", "is_last")] + [("freq", ctypes.c_uint32 * 320)]
+
+
+class ShardSpan(ctypes.Structure):
+    _fields_ = [("pre_bits", ctypes.c_uint64), ("post_bits", ctypes.c_uint64), ("aligned", ctypes.c_uint32),
+                ("reserved", ctypes.c_uint32)]
+
+
 class ZlibError(Exception):
     def __init__(self, code, msg=""):
         super().__init__("zlib error %d %s" % (code, msg))
@@ -116,6 +134,11 @@ def lib():
         L.zb_copy_to_device.argtypes = [vp, vp, vp, sz]
         L.zb_copy_to_host.argtypes = [vp, vp, vp, sz]
         L.zb_device_fill_random.argtypes = [vp, vp, sz, u64]
+        if hasattr(L, "zb_shard_parse"):  # builds before the range calls (ZB_LIB_PATH baselines of scripts/gpu_ab.sh) lack them
+            L.zb_shard_parse.argtypes = [vp, vp, sz, ci, sz, sz, ci, ci, u32, ctypes.POINTER(ShardEntry), ctypes.POINTER(u32)]
+            L.zb_shard_symbols.argtypes = [vp, u32, u32, ctypes.POINTER(ShardEdge), ctypes.POINTER(ShardEdge)]
+            L.zb_shard_size.argtypes = [vp, ctypes.POINTER(ShardEdge), sz, ctypes.POINTER(ShardSpan)]
+            L.zb_shard_encode.argtypes = [vp, u64, vp, sz, ci, ctypes.POINTER(u64)]
         _lib = L
     return _lib
 
@@ -388,3 +411,39 @@ class Engine:
 
     def fill_random(self, dptr, n, seed=42):
         self._check(lib().zb_device_fill_random(self.h, dptr, n, seed))
+
+    # ------------------------------------------------------------ chunk-sharded deflate, one-stream bytes (zb_shard_*)
+    # The four steps of one rank (include/zb_engine.h); zlib_rs_b200.shard.compress_sharded_exact drives them.  Records travel
+    # as plain Python values (entry table: list of (exit, count); edges: bytes; span: (pre_bits, post_bits, aligned)).
+    def shard_parse(self, src, range_begin, range_end, level=9, strategy=0, mem_level=8, n=None, src_on_device=False):
+        keep = None
+        if not src_on_device:
+            data, keep = _buf(src)
+            n = len(data)
+            src = ctypes.addressof(keep)
+        table = (ShardEntry * SHARD_CAND)()
+        adler = ctypes.c_uint32(0)
+        self._check(lib().zb_shard_parse(self.h, src, n, int(src_on_device), range_begin, range_end, level, strategy,
+                                         (mem_level & 15) << 8, table, ctypes.byref(adler)))
+        return [(t.exit, t.count) for t in table], adler.value
+
+    def shard_symbols(self, entry, sym_offset):
+        first, last = ShardEdge(), ShardEdge()
+        self._check(lib().zb_shard_symbols(self.h, entry, sym_offset, ctypes.byref(first), ctypes.byref(last)))
+        return bytes(first), bytes(last)
+
+    def shard_size(self, edges):
+        arr = (ShardEdge * len(edges))(*[ShardEdge.from_buffer_copy(e) for e in edges])
+        span = ShardSpan()
+        self._check(lib().zb_shard_size(self.h, arr, len(edges), ctypes.byref(span)))
+        return span.pre_bits, span.post_bits, span.aligned
+
+    def shard_encode(self, bit_offset, cap=None):
+        """The rank's part, written from bit (bit_offset & 7) of its first byte."""
+        n = ctypes.c_uint64(0)
+        rc = lib().zb_shard_encode(self.h, bit_offset, None, 0, 0, ctypes.byref(n))
+        if rc not in (0, Z_BUF_ERROR):
+            self._check(rc)
+        dst = ctypes.create_string_buffer(max(n.value, 1))
+        self._check(lib().zb_shard_encode(self.h, bit_offset, dst, n.value, 0, ctypes.byref(n)))
+        return dst.raw[: n.value]

@@ -174,9 +174,6 @@ int Engine::stage(size_t bytes)
     return ZB_OK;
 }
 
-enum { S_IN, S_L, S_HOLES, S_HOLESN, S_M, S_NXT, S_PEXIT, S_PCNT, S_SYMIDX, S_TENTRY, S_TSYMB, S_TDIRTY, S_SYMS, S_SYMB,
-       S_BLOCKS, S_SCRATCH, S_FREQ, S_OUT, S_CK, S_INF0, S_INF1, S_PHEAD, S_SK, S_MARKN, S_LLIST, S_LCNT, S_BMAP, S_HDIFF, S_HCOARSE, S_CSTATE, S_LISTS, S_LR, S_LLAST, S_BBASE, S_MCHG, S_GFN, S_KEYS, S_COUNT };
-static_assert(S_COUNT <= Engine::kSlots, "slots");
 
 size_t deflate_bound(size_t n)
 {
@@ -730,6 +727,7 @@ int zb_deflate(zb_engine *z, const void *src, size_t n, int src_dev, void *dst, 
                int window_bits, zb_deflate_result *res)
 {
     if (!z) return ZB_E_NODEVICE;
+    z->e.shard.phase = 0; // a range job in progress is gone (its buffers are reused)
     return z->e.deflate(src, n, src_dev != 0, dst, cap, dst_dev != 0, level, strategy, window_bits, 0, res);
 }
 
@@ -737,6 +735,7 @@ int zb_deflate_dict(zb_engine *z, const void *dict, size_t dict_len, const void 
                     int level, int strategy, int window_bits, uint32_t flags, zb_deflate_result *res)
 {
     if (!z) return ZB_E_NODEVICE;
+    z->e.shard.phase = 0; // a range job in progress is gone (its buffers are reused)
     return z->e.deflate(src, n, src_dev != 0, dst, cap, dst_dev != 0, level, strategy, window_bits, flags, res, dict, dict_len);
 }
 
@@ -744,6 +743,7 @@ int zb_deflate_ex(zb_engine *z, const void *src, size_t n, int src_dev, void *ds
                   int window_bits, uint32_t flags, zb_deflate_result *res)
 {
     if (!z) return ZB_E_NODEVICE;
+    z->e.shard.phase = 0; // a range job in progress is gone (its buffers are reused)
     return z->e.deflate(src, n, src_dev != 0, dst, cap, dst_dev != 0, level, strategy, window_bits, flags, res);
 }
 
@@ -753,6 +753,7 @@ int zb_inflate(zb_engine *z, const void *src, size_t n, int src_dev, void *dst, 
                zb_inflate_result *res)
 {
     if (!z) return ZB_E_NODEVICE;
+    z->e.shard.phase = 0; // a range job in progress is gone (its buffers are reused)
     return z->e.inflate(src, n, src_dev != 0, dst, cap, dst_dev != 0, window_bits, res);
 }
 
@@ -760,6 +761,7 @@ int zb_inflate_ex(zb_engine *z, const void *src, size_t n, int src_dev, void *ds
                   zb_inflate_result *res)
 {
     if (!z) return ZB_E_NODEVICE;
+    z->e.shard.phase = 0; // a range job in progress is gone (its buffers are reused)
     return z->e.inflate(src, n, src_dev != 0, dst, cap, dst_dev != 0, window_bits, res, flags);
 }
 
@@ -767,18 +769,21 @@ int zb_inflate_blocks(zb_engine *z, const void *src, size_t n, uint64_t start_bi
                       int check_kind, uint32_t check_start, zb_inflate_seg *out)
 {
     if (!z) return ZB_E_NODEVICE;
+    z->e.shard.phase = 0; // a range job in progress is gone (its buffers are reused)
     return z->e.inflate_blocks(src, n, start_bit, dict, dict_len, dst, cap, check_kind, check_start, out);
 }
 
 int zb_adler32(zb_engine *z, uint32_t start, const void *buf, size_t len, int on_dev, uint32_t *out, float *ms)
 {
     if (!z) return ZB_E_NODEVICE;
+    z->e.shard.phase = 0; // a range job in progress is gone (its buffers are reused)
     return z->e.checksum(false, start, buf, len, on_dev != 0, out, ms);
 }
 
 int zb_crc32(zb_engine *z, uint32_t start, const void *buf, size_t len, int on_dev, uint32_t *out, float *ms)
 {
     if (!z) return ZB_E_NODEVICE;
+    z->e.shard.phase = 0; // a range job in progress is gone (its buffers are reused)
     return z->e.checksum(true, start, buf, len, on_dev != 0, out, ms);
 }
 

@@ -11,6 +11,23 @@ namespace zb {
 extern thread_local char g_err[256];
 size_t deflate_bound(size_t n);
 
+// grow-only device buffer slots of an engine
+enum { S_IN, S_L, S_HOLES, S_HOLESN, S_M, S_NXT, S_PEXIT, S_PCNT, S_SYMIDX, S_TENTRY, S_TSYMB, S_TDIRTY, S_SYMS, S_SYMB,
+       S_BLOCKS, S_SCRATCH, S_FREQ, S_OUT, S_CK, S_INF0, S_INF1, S_PHEAD, S_SK, S_MARKN, S_LLIST, S_LCNT, S_BMAP, S_HDIFF, S_HCOARSE, S_CSTATE, S_LISTS, S_LR, S_LLAST, S_BBASE, S_MCHG, S_GFN, S_KEYS, S_SHARD, S_COUNT };
+
+// A range job of chunk-sharded deflate (zb_shard_*, zb_shard.cu) between its four calls.
+struct ShardState {
+    int phase = 0;                // 0 none, 1 parsed, 2 symbols emitted, 3 sized
+    JobBufs jb;
+    uint32_t off = 0, S = 0, E = 0, total = 0; // job offset in the input; range in job coordinates; input length
+    uint32_t bs = 0, npt = 0, O = 0, n = 0, blo = 0, nloc = 0;
+    bool is_last = false, tables = false;
+    uint4 *gfn = nullptr;         // two-level path chain scratch (k_path_groups / k_path_chain2)
+    uint32_t chainG = 0, chain_groups = 0, chain2_smem = 0;
+    uint32_t freq_lo[320], freq_hi[320]; // the rank's own histograms of its first and last block
+    zb_shard_span span;
+};
+
 struct Engine {
     static constexpr int kSlots = 40;
     struct Buf { void *p = nullptr; size_t cap = 0; };
@@ -51,6 +68,14 @@ struct Engine {
     int inflate_blocks(const void *src, size_t n, uint64_t start_bit, const void *dict, size_t dict_len, void *dst, size_t dst_cap,
                        int check_kind, uint32_t check_start, zb_inflate_seg *out);
     int checksum(bool crc, uint32_t start, const void *buf, size_t len, bool on_dev, uint32_t *out, float *ms);
+    ShardState shard;
+    int shard_parse(const void *src, size_t total, bool src_dev, size_t S, size_t E, int level, int strategy, uint32_t flags,
+                    zb_shard_entry *table, uint32_t *adler);
+    int shard_symbols(uint32_t entry, uint32_t sym_offset, zb_shard_edge *first, zb_shard_edge *last);
+    int shard_size(const zb_shard_edge *all, size_t n, zb_shard_span *span);
+    int shard_encode(uint64_t bit_offset, void *dst, size_t cap, bool dst_dev, uint64_t *bytes);
+    void shard_chain(); // path chain + marks from jb.start (k_path_groups/k_path_chain2 or k_path_chain, k_path_mark)
 };
+static_assert(S_COUNT <= Engine::kSlots, "slots");
 
 } // namespace zb

@@ -591,7 +591,7 @@ __device__ __forceinline__ uint32_t emit_step(const JobBufs &jb, uint32_t p, Sym
 __global__ void __launch_bounds__(256) k_emit_slow(JobBufs jb)
 {
     const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
-    if (p >= jb.N) return;
+    if (p >= jb.N || p >= jb.tail_start) return; // a range job (zb_shard.cu) parses up to tail_start < N
     const uint32_t idx = jb.symidx[p];
     if (!idx) return;
     emit_step(jb, p, jb.syms + jb.tile_symbase[p / kPathTile] + idx - 1);
