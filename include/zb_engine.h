@@ -31,6 +31,7 @@ extern "C" {
 #define ZB_E_PARAM (-2)      /* invalid argument (Z_STREAM_ERROR) */
 #define ZB_E_DATA (-3)       /* corrupt input (Z_DATA_ERROR) */
 #define ZB_E_INTERNAL (-102) /* engine invariant violated */
+#define ZB_E_DECLINED (-103) /* zb_inflate_ex with ZB_INF_NO_SERIAL: the block-parallel decoder did not deliver the output */
 
 typedef struct zb_engine zb_engine;
 
@@ -100,6 +101,11 @@ ZB_API int zb_inflate(zb_engine *e, const void *src, size_t src_len, int src_on_
 
 #define ZB_INF_CHECK_ADLER 1u /* zb_inflate_ex on a raw stream (window_bits < 0): also return the adler32 ... */
 #define ZB_INF_CHECK_CRC 2u   /* ... or the crc32 of the output in res->check (for callers that parse header and trailer themselves) */
+#define ZB_INF_NO_SERIAL 4u   /* never run the serial decoder: when the block-parallel decoder does not deliver the output, return
+                                 ZB_E_DECLINED with the stage that gave up in res->msg: "small" (input < 64 KiB), "header" (stream
+                                 header), "scout" (no or too many block candidates), "chain" (a block the chain cannot follow: fixed
+                                 codes, damage, too many blocks), "capacity" (output larger than dst_cap) or "decode" (a replay kernel
+                                 found an inconsistency).  For tests and diagnostics: it shows which decoder produced the bytes. */
 ZB_API int zb_inflate_ex(zb_engine *e, const void *src, size_t src_len, int src_on_device, void *dst, size_t dst_cap, int dst_on_device,
                          int window_bits, uint32_t flags, zb_inflate_result *res);
 

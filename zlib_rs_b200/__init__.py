@@ -26,6 +26,10 @@ ZB_FLAG_NOT_LAST = 1
 ZB_FLAG_LOW_PARALLEL = 2
 ZB_FLAG_CHECK_ADLER = 4
 ZB_FLAG_CHECK_CRC = 8
+ZB_INF_CHECK_ADLER = 1
+ZB_INF_CHECK_CRC = 2
+ZB_INF_NO_SERIAL = 4  # Engine.inflate: only the block-parallel decoder; ZB_E_DECLINED with the stage in res.msg when it gives up
+ZB_E_DECLINED = -103
 
 
 class ZStream(ctypes.Structure):
@@ -125,6 +129,7 @@ def lib():
         L.zb_deflate_ex.argtypes = [vp, vp, sz, ci, vp, sz, ci, ci, ci, ci, u32, ctypes.POINTER(DeflateResult)]
         L.zb_deflate_bound.argtypes, L.zb_deflate_bound.restype = [sz], sz
         L.zb_inflate.argtypes = [vp, vp, sz, ci, vp, sz, ci, ci, ctypes.POINTER(InflateResult)]
+        L.zb_inflate_ex.argtypes = [vp, vp, sz, ci, vp, sz, ci, ci, u32, ctypes.POINTER(InflateResult)]
         L.zb_adler32.argtypes = [vp, u32, vp, sz, ci, ctypes.POINTER(u32), ctypes.POINTER(ctypes.c_float)]
         L.zb_crc32.argtypes = [vp, u32, vp, sz, ci, ctypes.POINTER(u32), ctypes.POINTER(ctypes.c_float)]
         L.zb_engine_set_profile.argtypes = [vp, ci]
@@ -364,7 +369,8 @@ class Engine:
         self._check(rc)
         return (own.raw[: res.out_bytes] if own is not None else None), res
 
-    def inflate(self, src, out_cap, n=None, window_bits=15, src_on_device=False, dst=None, dst_on_device=False):
+    def inflate(self, src, out_cap, n=None, window_bits=15, src_on_device=False, dst=None, dst_on_device=False, flags=0):
+        """Returns (rc, bytes or None, InflateResult).  flags: ZB_INF_*."""
         res = InflateResult()
         keep = None
         if not src_on_device:
@@ -375,7 +381,8 @@ class Engine:
         if dst is None:
             own = ctypes.create_string_buffer(max(out_cap, 1))
             dst = ctypes.addressof(own)
-        rc = lib().zb_inflate(self.h, src, n, int(src_on_device), dst, out_cap, int(dst_on_device), window_bits, ctypes.byref(res))
+        rc = lib().zb_inflate_ex(self.h, src, n, int(src_on_device), dst, out_cap, int(dst_on_device), window_bits, flags,
+                                 ctypes.byref(res))
         return rc, (own.raw[: res.out_bytes] if own is not None else None), res
 
     def adler32(self, buf, n=None, start=1, on_device=False):

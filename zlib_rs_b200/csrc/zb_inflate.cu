@@ -1257,6 +1257,7 @@ int Engine::inflate(const void *src, size_t n, bool src_dev, void *dst, size_t d
     InfState *dis = static_cast<InfState *>(d_inf_state), *his = static_cast<InfState *>(h_inf_state);
     launches = 0;
     bool done = false;
+    const char *declined = "small"; // the stage of the block-parallel path that gave up (reported with ZB_INF_NO_SERIAL)
     if (n >= 65536) {
         // block-parallel path; anything it cannot follow falls through to the serial decoder below
         InfPar *dpar, hpar;
@@ -1278,6 +1279,7 @@ int Engine::inflate(const void *src, size_t n, bool src_dev, void *dst, size_t d
         launches += 2;
         CKI(cudaMemcpyAsync(&hpar, dpar, sizeof(InfPar), cudaMemcpyDeviceToHost, st));
         CKI(cudaStreamSynchronize(st));
+        declined = hpar.status != PS_OK ? "header" : "scout";
         if (hpar.status == PS_OK && hpar.ncand > 0 && hpar.ncand <= kMaxCand) {
             // symbol arena: one slot per candidate (a deflate block of zlib-family encoders has at most 32767 symbols + end of block)
             constexpr uint32_t kSlotSyms = 40960;
@@ -1302,7 +1304,9 @@ int Engine::inflate(const void *src, size_t n, bool src_dev, void *dst, size_t d
             launches += 2;
             CKI(cudaMemcpyAsync(&hpar, dpar, sizeof(InfPar), cudaMemcpyDeviceToHost, st));
             CKI(cudaStreamSynchronize(st));
+            declined = hpar.status != PS_OK || hpar.nblocks == 0 ? "chain" : "capacity";
             if (hpar.status == PS_OK && hpar.nblocks > 0 && hpar.total_out <= dst_cap) {
+                declined = "decode";
                 uint16_t *dtmp;
                 if ((rc = reserve(4 /*S_M*/, (hpar.total_out + 64) * 2, &p)) != ZB_OK) return rc;
                 dtmp = static_cast<uint16_t *>(p);
@@ -1339,6 +1343,15 @@ int Engine::inflate(const void *src, size_t n, bool src_dev, void *dst, size_t d
                 }
             }
         }
+    }
+    if (!done && (flags & ZB_INF_NO_SERIAL)) {
+        snprintf(res->msg, sizeof res->msg, "%s", declined);
+        CKI(cudaEventRecord(ev1, st));
+        CKI(cudaStreamSynchronize(st));
+        CKI(cudaEventElapsedTime(&res->gpu_ms, ev0, ev1));
+        res->status = ZB_E_DECLINED;
+        res->gpu_launches = launches;
+        return ZB_E_DECLINED;
     }
     if (!done) {
         k_inflate<<<1, 32, sizeof(InfShared), st>>>(d_src, n, d_dst, dst_cap, window_bits, dis, InfSeg{0, nullptr, 0, 0});
