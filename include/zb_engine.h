@@ -106,6 +106,16 @@ ZB_API int zb_inflate(zb_engine *e, const void *src, size_t src_len, int src_on_
                                  header), "scout" (no or too many block candidates), "chain" (a block the chain cannot follow: fixed
                                  codes, damage, too many blocks), "capacity" (output larger than dst_cap) or "decode" (a replay kernel
                                  found an inconsistency).  For tests and diagnostics: it shows which decoder produced the bytes. */
+#define ZB_INF_MEMBERS 8u     /* decode every member of a gzip file (RFC 1952 2.2), as gzip -d and gzread do.  Only with gzip framing,
+                                 window_bits 24..31; any other window_bits, or together with ZB_INF_NO_SERIAL, gives ZB_E_PARAM.
+                                 Members are decoded in order from offset 0; after each trailer decoding goes on when the next two
+                                 bytes are 1f 8b, and otherwise stops there (trailing zeros or junk, or the end: in_bytes is the end of
+                                 the last member).  out_bytes is the total output and check the crc32 of all of it.  The first bad
+                                 member decides the result: its return code and msg are those zb_inflate_ex gives for that member
+                                 alone, and out_bytes / in_bytes / check cover the members in front of it, whose output is in dst.
+                                 When dst_cap is too small: ZB_E_BUF, with the members that fit entirely decoded and counted.  Runs of
+                                 BGZF members (FEXTRA with a BC subfield: SAM/BAM, tabix, .vcf.gz) are decoded side by side on the GPU;
+                                 their BSIZE and ISIZE fields are only hints, which decide the speed but never the result. */
 ZB_API int zb_inflate_ex(zb_engine *e, const void *src, size_t src_len, int src_on_device, void *dst, size_t dst_cap, int dst_on_device,
                          int window_bits, uint32_t flags, zb_inflate_result *res);
 

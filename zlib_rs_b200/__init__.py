@@ -29,6 +29,7 @@ ZB_FLAG_CHECK_CRC = 8
 ZB_INF_CHECK_ADLER = 1
 ZB_INF_CHECK_CRC = 2
 ZB_INF_NO_SERIAL = 4  # Engine.inflate: only the block-parallel decoder; ZB_E_DECLINED with the stage in res.msg when it gives up
+ZB_INF_MEMBERS = 8  # Engine.inflate with gzip framing: every member of the file; runs of BGZF members decoded side by side
 ZB_E_DECLINED = -103
 
 

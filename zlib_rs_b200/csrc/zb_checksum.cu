@@ -373,4 +373,70 @@ cudaError_t launch_crc32(const uint8_t *d_buf, uint64_t len, uint32_t start, voi
     return cudaGetLastError();
 }
 
+// ------------------------------------------------------------------------------------------------
+// Member checks of a multi-member gzip batch (zb_inflate.cu, DESIGN.md §2g)
+// ------------------------------------------------------------------------------------------------
+// k_crc_segments: the crc32 of every segment [off[s], off[s] + len[s]) of buf, one CTA per segment (BGZF members hold at most
+// 64 KiB).  Thread t takes the t-th of 256 equal pieces counted from the END of the segment, so only the first piece is short (leading
+// zeros do not change a raw CRC); it runs the byte-table raw CRC over its piece, and a tree joins the pieces with shifts of
+// x^(8 * piece * 2^level).  crc32's pre- and post-inversion are applied once at the end.
+__global__ void __launch_bounds__(256) k_crc_segments(const uint8_t *__restrict__ buf, const uint64_t *__restrict__ off,
+                                                      const uint32_t *__restrict__ len, uint32_t *__restrict__ out)
+{
+    __shared__ uint32_t tab[256], part[256], shift[8];
+    const uint32_t tid = threadIdx.x, s = blockIdx.x;
+    uint32_t c = tid;
+    for (int k = 0; k < 8; k++) c = (c & 1) ? (c >> 1) ^ kCrcPoly : c >> 1;
+    tab[tid] = c;
+    const uint32_t L = len[s], piece = (L + 255) / 256;
+    if (tid < 8) shift[tid] = x2nmodp((uint64_t)piece << tid, 3);
+    __syncthreads();
+    const uint8_t *p = buf + off[s];
+    const int64_t e = (int64_t)L - (int64_t)(255 - tid) * piece, b = e - (int64_t)piece;
+    uint32_t r = 0;
+    for (int64_t i = b < 0 ? 0 : b; i < e; i++) r = tab[(r ^ p[i]) & 0xffu] ^ (r >> 8);
+    part[tid] = r;
+    __syncthreads();
+    for (uint32_t l = 0; l < 8; l++) {
+        const uint32_t h = 1u << l;
+        if ((tid & (2 * h - 1)) == 0) part[tid] = (part[tid] ? multmodp(shift[l], part[tid]) : 0) ^ part[tid + h];
+        __syncthreads();
+    }
+    if (tid == 0) out[s] = part[0] ^ multmodp(x2nmodp(L, 3), 0xffffffffu) ^ 0xffffffffu;
+}
+
+// k_crc_join: crc32_combine of the first *count segment checks, in order (one CTA: runs of segments per thread, then a tree).
+__global__ void __launch_bounds__(1024) k_crc_join(const uint32_t *__restrict__ crc, const uint32_t *__restrict__ len,
+                                                   const uint32_t *__restrict__ count, uint32_t *__restrict__ out)
+{
+    __shared__ uint32_t sc[1024];
+    __shared__ uint64_t sl[1024];
+    const uint32_t tid = threadIdx.x, n = *count, per = (n + 1023) / 1024;
+    const uint32_t beg = min(n, tid * per), end = min(n, beg + per);
+    uint32_t c = 0;
+    uint64_t l = 0;
+    for (uint32_t i = beg; i < end; i++) { c = multmodp(x2nmodp(len[i], 3), c) ^ crc[i]; l += len[i]; }
+    sc[tid] = c;
+    sl[tid] = l;
+    __syncthreads();
+    for (uint32_t h = 1; h < 1024; h <<= 1) {
+        if ((tid & (2 * h - 1)) == 0) { sc[tid] = multmodp(x2nmodp(sl[tid + h], 3), sc[tid]) ^ sc[tid + h]; sl[tid] += sl[tid + h]; }
+        __syncthreads();
+    }
+    if (tid == 0) *out = sc[0];
+}
+
+cudaError_t launch_crc32_segments(const uint8_t *d_buf, const uint64_t *d_off, const uint32_t *d_len, uint32_t nseg, uint32_t *d_crc,
+                                  cudaStream_t st)
+{
+    if (nseg) k_crc_segments<<<nseg, 256, 0, st>>>(d_buf, d_off, d_len, d_crc);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_crc32_join(const uint32_t *d_crc, const uint32_t *d_len, const uint32_t *d_count, uint32_t *d_out, cudaStream_t st)
+{
+    k_crc_join<<<1, 1024, 0, st>>>(d_crc, d_len, d_count, d_out);
+    return cudaGetLastError();
+}
+
 } // namespace zb

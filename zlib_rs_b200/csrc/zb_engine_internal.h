@@ -13,7 +13,9 @@ size_t deflate_bound(size_t n);
 
 // grow-only device buffer slots of an engine
 enum { S_IN, S_L, S_HOLES, S_HOLESN, S_M, S_NXT, S_PEXIT, S_PCNT, S_SYMIDX, S_TENTRY, S_TSYMB, S_TDIRTY, S_SYMS, S_SYMB,
-       S_BLOCKS, S_SCRATCH, S_FREQ, S_OUT, S_CK, S_INF0, S_INF1, S_PHEAD, S_SK, S_MARKN, S_LLIST, S_LCNT, S_BMAP, S_HDIFF, S_HCOARSE, S_CSTATE, S_LISTS, S_LR, S_LLAST, S_BBASE, S_MCHG, S_GFN, S_KEYS, S_SHARD, S_COUNT };
+       S_BLOCKS, S_SCRATCH, S_FREQ, S_OUT, S_CK, S_INF0, S_INF1, S_PHEAD, S_SK, S_MARKN, S_LLIST, S_LCNT, S_BMAP, S_HDIFF, S_HCOARSE, S_CSTATE, S_LISTS, S_LR, S_LLAST, S_BBASE, S_MCHG, S_GFN, S_KEYS, S_SHARD,
+       S_MEMT, S_MEMC, // multi-member gzip: tile counts and control block; candidate and member tables
+       S_COUNT };
 
 // A range job of chunk-sharded deflate (zb_shard_*, zb_shard.cu) between its four calls.
 struct ShardState {
@@ -65,6 +67,9 @@ struct Engine {
                 int window_bits, uint32_t flags, zb_deflate_result *res, const void *dict = nullptr, size_t dict_len = 0);
     int inflate(const void *src, size_t n, bool src_dev, void *dst, size_t dst_cap, bool dst_dev, int window_bits,
                 zb_inflate_result *res, uint32_t flags = 0);
+    int inflate_stream(const uint8_t *d_src, size_t n, uint8_t *d_dst, size_t dst_cap, int window_bits, uint32_t flags,
+                       zb_inflate_result *res);
+    int inflate_members(const uint8_t *d_src, size_t n, uint8_t *d_dst, size_t dst_cap, int window_bits, zb_inflate_result *res);
     int inflate_blocks(const void *src, size_t n, uint64_t start_bit, const void *dict, size_t dict_len, void *dst, size_t dst_cap,
                        int check_kind, uint32_t check_start, zb_inflate_seg *out);
     int checksum(bool crc, uint32_t start, const void *buf, size_t len, bool on_dev, uint32_t *out, float *ms);

@@ -13,8 +13,10 @@
 #include <string.h>
 #include <algorithm>
 #include <vector>
+#include "../../include/zlib_b200.h"
 #include "zb_engine_internal.h"
 #include "zb_inflate_core.h"
+#include "zb_members.h"
 
 namespace zb {
 
@@ -135,11 +137,11 @@ struct InfShared {
 
 enum Cmd { C_NONE = 0, C_REFILL, C_FLUSH, C_COPY, C_DONE };
 
-__global__ void __launch_bounds__(32) k_inflate(const uint8_t *__restrict__ src, uint64_t n, uint8_t *__restrict__ dst, uint64_t cap,
-                                                int window_bits, InfState *res, InfSeg seg)
+// The one-warp decoder: a whole stream (header, blocks, trailer) or, in segment mode, raw blocks from a bit position.  Output goes to
+// dst[0, cap) only.  k_inflate runs it on one stream, k_members on one gzip member per warp.
+__device__ __forceinline__ void inflate_warp(InfShared &S, const uint8_t *__restrict__ src, uint64_t n, uint8_t *__restrict__ dst,
+                                             uint64_t cap, int window_bits, InfState *res, InfSeg seg)
 {
-    extern __shared__ __align__(16) uint8_t smem_raw[];
-    InfShared &S = *reinterpret_cast<InfShared *>(smem_raw);
     const uint32_t lane = threadIdx.x;
     // shared between lanes through shuffles from lane 0
     uint64_t ifill = 0;   // input bytes loaded into the ring so far (absolute)
@@ -448,6 +450,13 @@ __global__ void __launch_bounds__(32) k_inflate(const uint8_t *__restrict__ src,
 #undef DROP
 #undef FAIL
 #undef REAL
+}
+
+__global__ void __launch_bounds__(32) k_inflate(const uint8_t *__restrict__ src, uint64_t n, uint8_t *__restrict__ dst, uint64_t cap,
+                                                int window_bits, InfState *res, InfSeg seg)
+{
+    extern __shared__ __align__(16) uint8_t smem_raw[];
+    inflate_warp(*reinterpret_cast<InfShared *>(smem_raw), src, n, dst, cap, window_bits, res, seg);
 }
 
 // ================================================================================================
@@ -1191,6 +1200,196 @@ __global__ void __launch_bounds__(256) k_inf_tile_resolve(InfPar *par, const uin
     }
 }
 
+// ================================================================================================
+// Multi-member gzip (ZB_INF_MEMBERS, DESIGN.md §2g).  A run of BGZF members is decoded as one batch, one warp per member:
+//   k_mem_count, k_mem_scan, k_mem_emit  every byte offset of the input is tested for a BGZF header (zb_members.h); the candidates
+//                                        are compacted in input order (once per call);
+//   k_mem_jump                           candidate i links to the candidate that starts where its BSIZE says it ends; pointer
+//                                        doubling tables of those links (once per call);
+//   k_mem_chain                          the run from a head candidate: its members by composing the doubling tables (a fake header
+//                                        inside a payload is never reached from the head), their ISIZE hints and output offsets;
+//   k_members                            the decoder of k_inflate on every member that fits dst, each warp into its own slot;
+//   k_crc_segments, k_mem_verdict, k_crc_join   member checks, the first member whose decode failed or whose hints were wrong,
+//                                        and the crc32 of the members in front of it.
+// The launch count of a batch does not depend on the number of members.
+// ================================================================================================
+constexpr uint32_t kMemTile = 4096;        // byte offsets per CTA of k_mem_count / k_mem_emit, 16 per thread
+constexpr uint32_t kMemMaxCand = 1u << 20; // more header candidates than this: every member takes the single-stream path
+
+struct MemCtl {
+    uint32_t ncand;             // BGZF header candidates in the input
+    uint32_t count, fit;        // members of the run; the leading ones whose output fits dst
+    uint32_t good;              // members in front of the first one the batch hands back
+    uint64_t good_out, good_in; // their output and input bytes
+    uint32_t good_crc;          // crc32 of their output
+};
+
+// Exclusive prefix sum over the threads of a CTA (blockDim.x a multiple of 32, at most 1024); `total` gets the sum.
+template <typename T>
+__device__ T cta_exclusive_scan(T v, T *warp_sums, T &total)
+{
+    const uint32_t lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    T x = v;
+    for (uint32_t d = 1; d < 32; d <<= 1) { const T t = __shfl_up_sync(0xffffffffu, x, d); if (lane >= d) x += t; }
+    if (lane == 31) warp_sums[w] = x;
+    __syncthreads();
+    if (w == 0) {
+        T s = lane < nw ? warp_sums[lane] : (T)0;
+        for (uint32_t d = 1; d < 32; d <<= 1) { const T t = __shfl_up_sync(0xffffffffu, s, d); if (lane >= d) s += t; }
+        warp_sums[lane] = s;
+    }
+    __syncthreads();
+    total = warp_sums[nw - 1];
+    const T r = x - v + (w ? warp_sums[w - 1] : (T)0);
+    __syncthreads();
+    return r;
+}
+
+__device__ __forceinline__ uint32_t mem_tests(const uint8_t *src, uint64_t n, uint64_t p0, int32_t *bs)
+{
+    uint32_t c = 0;
+    for (uint32_t i = 0; i < 16; i++) {
+        bs[i] = p0 + i < n ? zbm_bgzf_bsize(src + p0 + i, n - p0 - i) : -1;
+        c += bs[i] >= 0;
+    }
+    return c;
+}
+
+__global__ void __launch_bounds__(256) k_mem_count(const uint8_t *src, uint64_t n, uint32_t *tile_cnt)
+{
+    __shared__ uint32_t cnt;
+    if (threadIdx.x == 0) cnt = 0;
+    __syncthreads();
+    int32_t bs[16];
+    const uint32_t c = mem_tests(src, n, (uint64_t)blockIdx.x * kMemTile + threadIdx.x * 16, bs);
+    if (c) atomicAdd(&cnt, c);
+    __syncthreads();
+    if (threadIdx.x == 0) tile_cnt[blockIdx.x] = cnt;
+}
+
+// exclusive scan of the tile counts (one CTA)
+__global__ void __launch_bounds__(1024) k_mem_scan(const uint32_t *tile_cnt, uint32_t ntiles, uint32_t *tile_base, MemCtl *ctl)
+{
+    __shared__ uint32_t ws[32];
+    const uint32_t per = (ntiles + 1023) / 1024, beg = min(ntiles, threadIdx.x * per), end = min(ntiles, beg + per);
+    uint32_t s = 0;
+    for (uint32_t i = beg; i < end; i++) s += tile_cnt[i];
+    uint32_t total;
+    uint32_t run = cta_exclusive_scan(s, ws, total);
+    for (uint32_t i = beg; i < end; i++) { tile_base[i] = run; run += tile_cnt[i]; }
+    if (threadIdx.x == 0) ctl->ncand = total;
+}
+
+__global__ void __launch_bounds__(256) k_mem_emit(const uint8_t *src, uint64_t n, const uint32_t *tile_base, uint64_t *cand_off,
+                                                  uint32_t *cand_len)
+{
+    __shared__ uint32_t ws[32];
+    int32_t bs[16];
+    const uint64_t p0 = (uint64_t)blockIdx.x * kMemTile + threadIdx.x * 16;
+    const uint32_t c = mem_tests(src, n, p0, bs);
+    uint32_t total;
+    uint32_t k = tile_base[blockIdx.x] + cta_exclusive_scan(c, ws, total);
+    for (uint32_t i = 0; i < 16; i++)
+        if (bs[i] >= 0) { cand_off[k] = p0 + i; cand_len[k] = (uint32_t)bs[i] + 1; k++; }
+}
+
+// jmp[l * (nc + 1) + i]: the candidate 2^l members behind candidate i (nc: none).  One CTA: the levels depend on each other.
+__global__ void __launch_bounds__(1024) k_mem_jump(const uint64_t *off, const uint32_t *len, uint32_t nc, uint32_t levels, uint32_t *jmp)
+{
+    for (uint32_t i = threadIdx.x; i <= nc; i += 1024) {
+        uint32_t nx = nc;
+        if (i < nc) {
+            const uint64_t q = off[i] + len[i];
+            uint32_t lo = i + 1, hi = nc; // the first candidate at or behind q
+            while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (off[mid] < q) lo = mid + 1; else hi = mid; }
+            if (lo < nc && off[lo] == q) nx = lo;
+        }
+        jmp[i] = nx;
+    }
+    for (uint32_t l = 1; l < levels; l++) {
+        __syncthreads();
+        const uint32_t *a = jmp + (size_t)(l - 1) * (nc + 1);
+        uint32_t *b = jmp + (size_t)l * (nc + 1);
+        for (uint32_t i = threadIdx.x; i <= nc; i += 1024) b[i] = a[a[i]];
+    }
+}
+
+// The run from candidate `head`: member t is the t-th successor of head.  Member table, ISIZE hints, output offsets, and how many
+// leading members fit `cap` bytes of output (one CTA).
+__global__ void __launch_bounds__(1024) k_mem_chain(const uint8_t *src, const uint64_t *off, const uint32_t *len, const uint32_t *jmp,
+                                                    uint32_t nc, uint32_t levels, uint32_t head, uint64_t cap, uint64_t *moff,
+                                                    uint32_t *mlen, uint32_t *misz, uint64_t *mout, MemCtl *ctl)
+{
+    __shared__ uint32_t s_count, s_fit;
+    __shared__ uint64_t ws[32];
+    const uint32_t tid = threadIdx.x;
+    if (tid == 0) {
+        uint32_t node = head, c = 1;
+        for (int l = (int)levels - 1; l >= 0; l--) {
+            const uint32_t nx = jmp[(size_t)l * (nc + 1) + node];
+            if (nx != nc) { node = nx; c += 1u << l; }
+        }
+        s_count = c;
+        s_fit = 0;
+    }
+    __syncthreads();
+    const uint32_t count = s_count, per = (count + 1023) / 1024;
+    const uint32_t beg = min(count, tid * per), end = min(count, beg + per);
+    uint32_t node = head;
+    for (uint32_t l = 0; l < levels; l++) if ((beg >> l) & 1u) node = jmp[(size_t)l * (nc + 1) + node];
+    uint64_t sum = 0;
+    for (uint32_t t = beg; t < end; t++, node = jmp[node]) {
+        moff[t] = off[node];
+        mlen[t] = len[node];
+        misz[t] = zbm_isize(src + off[node], len[node]);
+        sum += misz[t];
+    }
+    uint64_t total;
+    uint64_t run = cta_exclusive_scan(sum, ws, total);
+    uint32_t fit = 0;
+    for (uint32_t t = beg; t < end; t++) {
+        mout[t] = run;
+        run += misz[t];
+        fit += run <= cap;
+    }
+    if (fit) atomicAdd(&s_fit, fit);
+    __syncthreads();
+    if (tid == 0) { ctl->count = count; ctl->fit = s_fit; }
+}
+
+// One member per warp, into its own slot [mout, mout + ISIZE) of dst.
+__global__ void __launch_bounds__(32) k_members(const uint8_t *__restrict__ src, const uint64_t *moff, const uint32_t *mlen,
+                                                const uint32_t *misz, const uint64_t *mout, uint8_t *__restrict__ dst, int window_bits,
+                                                InfState *mst)
+{
+    extern __shared__ __align__(16) uint8_t smem_raw[];
+    const uint32_t m = blockIdx.x;
+    inflate_warp(*reinterpret_cast<InfShared *>(smem_raw), src + moff[m], mlen[m], dst + mout[m], misz[m], window_bits, mst + m,
+                 InfSeg{0, nullptr, 0, 0});
+}
+
+// The first member whose decode failed, whose trailer did not end at BSIZE + 1, whose output length is not its ISIZE hint (nor, then,
+// its trailer's ISIZE) or whose crc32 differs from its trailer; the members in front of it are the batch's result (one CTA).
+__global__ void __launch_bounds__(1024) k_mem_verdict(const InfState *mst, const uint32_t *mcrc, const uint64_t *moff, const uint32_t *mlen,
+                                                      const uint32_t *misz, const uint64_t *mout, MemCtl *ctl)
+{
+    __shared__ uint32_t s_bad;
+    const uint32_t fit = ctl->fit;
+    if (threadIdx.x == 0) s_bad = fit;
+    __syncthreads();
+    for (uint32_t m = threadIdx.x; m < fit; m += 1024) {
+        const InfState &s = mst[m];
+        if (s.err != IE_OK || s.in_bytes != mlen[m] || s.out_bytes != misz[m] || s.trailer_check != mcrc[m]) atomicMin(&s_bad, m);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        const uint32_t g = s_bad;
+        ctl->good = g;
+        ctl->good_out = g ? mout[g - 1] + misz[g - 1] : 0;
+        ctl->good_in = g ? moff[g - 1] + mlen[g - 1] - moff[0] : 0;
+    }
+}
+
 static const char *inf_msg(uint32_t e)
 {
     switch (e) {
@@ -1220,6 +1419,8 @@ int Engine::inflate_init()
 {
     cudaError_t e = cudaFuncSetAttribute(k_inflate, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(InfShared));
     if (e != cudaSuccess) { snprintf(g_err, sizeof g_err, "k_inflate attr: %s", cudaGetErrorString(e)); return ZB_E_CUDA; }
+    e = cudaFuncSetAttribute(k_members, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(InfShared));
+    if (e != cudaSuccess) { snprintf(g_err, sizeof g_err, "k_members attr: %s", cudaGetErrorString(e)); return ZB_E_CUDA; }
     if (cudaMalloc(&d_inf_state, sizeof(InfState)) != cudaSuccess) return ZB_E_MEM;
     if (cudaMallocHost(&h_inf_state, sizeof(InfState)) != cudaSuccess) return ZB_E_MEM;
     return ZB_OK;
@@ -1239,6 +1440,7 @@ int Engine::inflate(const void *src, size_t n, bool src_dev, void *dst, size_t d
     if (window_bits < 0) { if (window_bits < -15 || window_bits > -8) return ZB_E_PARAM; }
     else if (window_bits != 0 && ((window_bits & 15) < 8) ) return ZB_E_PARAM;
     if (window_bits > 47) return ZB_E_PARAM;
+    if ((flags & ZB_INF_MEMBERS) && (window_bits < 24 || window_bits > 31 || (flags & ZB_INF_NO_SERIAL))) return ZB_E_PARAM;
     CKI(cudaSetDevice(device));
     int rc;
     void *p;
@@ -1254,8 +1456,132 @@ int Engine::inflate(const void *src, size_t n, bool src_dev, void *dst, size_t d
         if ((rc = reserve(20 /*S_INF1*/, dst_cap + 64, &p)) != ZB_OK) return rc;
         d_dst = static_cast<uint8_t *>(p);
     }
-    InfState *dis = static_cast<InfState *>(d_inf_state), *his = static_cast<InfState *>(h_inf_state);
     launches = 0;
+    const int status = (flags & ZB_INF_MEMBERS) ? inflate_members(d_src, n, d_dst, dst_cap, window_bits, res)
+                                                : inflate_stream(d_src, n, d_dst, dst_cap, window_bits, flags, res);
+    if (status != ZB_OK && status != ZB_E_BUF && status != ZB_E_DATA && status != ZB_E_DECLINED) return status;
+    if (!dst_dev && res->out_bytes) CKI(cudaMemcpyAsync(dst, d_dst, res->out_bytes, cudaMemcpyDeviceToHost, st));
+    CKI(cudaEventRecord(ev1, st));
+    CKI(cudaStreamSynchronize(st));
+    CKI(cudaEventElapsedTime(&res->gpu_ms, ev0, ev1));
+    res->status = status;
+    res->gpu_launches = launches;
+    return status;
+}
+
+// ZB_INF_MEMBERS: every member of a gzip file, from offset 0 on, while the next two bytes are 1f 8b (gz_look, libz-rs-sys gz.rs).
+// Runs of BGZF members go through the batch (k_mem_* / k_members); a member the batch hands back, and any other member, through
+// inflate_stream at the current offset.  The error of a member is the one inflate_stream gives for it alone; out_bytes / in_bytes
+// and check cover the members in front of it.
+int Engine::inflate_members(const uint8_t *d_src, size_t n, uint8_t *d_dst, size_t dst_cap, int window_bits, zb_inflate_result *res)
+{
+    int rc;
+    void *p;
+    // ---- member table of the whole input: BGZF header candidates in order, and the doubling tables of their BSIZE links
+    const uint64_t ntiles = (n + kMemTile - 1) / kMemTile;
+    if (ntiles > 0xffffffffull) return ZB_E_PARAM;
+    if ((rc = reserve(S_MEMT, sizeof(MemCtl) + 64 + 8 * ntiles, &p)) != ZB_OK) return rc;
+    MemCtl *d_ctl = static_cast<MemCtl *>(p), h_ctl;
+    uint32_t *d_tcnt = reinterpret_cast<uint32_t *>(static_cast<uint8_t *>(p) + ((sizeof(MemCtl) + 63) & ~(size_t)63));
+    uint32_t *d_tbase = d_tcnt + ntiles;
+    std::vector<uint64_t> cand; // candidate offsets, host copy
+    uint32_t nc = 0, levels = 0;
+    uint64_t *d_off = nullptr, *d_moff = nullptr, *d_mout = nullptr;
+    uint32_t *d_len = nullptr, *d_jmp = nullptr, *d_mlen = nullptr, *d_misz = nullptr, *d_mcrc = nullptr;
+    InfState *d_mst = nullptr;
+    if (ntiles) {
+        k_mem_count<<<(unsigned)ntiles, 256, 0, st>>>(d_src, n, d_tcnt);
+        k_mem_scan<<<1, 1024, 0, st>>>(d_tcnt, (uint32_t)ntiles, d_tbase, d_ctl);
+        launches += 2;
+        CKI(cudaMemcpyAsync(&h_ctl, d_ctl, sizeof h_ctl, cudaMemcpyDeviceToHost, st));
+        CKI(cudaStreamSynchronize(st));
+        nc = h_ctl.ncand;
+    }
+    if (nc > kMemMaxCand) nc = 0; // pathological input: every member goes through inflate_stream
+    if (nc) {
+        levels = 32 - __builtin_clz(nc); // 2^levels > nc - 1, the most hops a run can take
+        const size_t n1 = (size_t)nc + 1;
+        const size_t bytes = n1 * (8 + 4 + 4 * levels + 8 + 4 + 4 + 8 + 4 + sizeof(InfState)) + 16 * 64;
+        if ((rc = reserve(S_MEMC, bytes, &p)) != ZB_OK) return rc;
+        uint8_t *q = static_cast<uint8_t *>(p);
+        auto take = [&](size_t b) { uint8_t *r = q; q += (b + 63) & ~(size_t)63; return r; };
+        d_off = reinterpret_cast<uint64_t *>(take(8 * n1));
+        d_len = reinterpret_cast<uint32_t *>(take(4 * n1));
+        d_jmp = reinterpret_cast<uint32_t *>(take(4 * n1 * levels));
+        d_moff = reinterpret_cast<uint64_t *>(take(8 * n1));
+        d_mlen = reinterpret_cast<uint32_t *>(take(4 * n1));
+        d_misz = reinterpret_cast<uint32_t *>(take(4 * n1));
+        d_mout = reinterpret_cast<uint64_t *>(take(8 * n1));
+        d_mcrc = reinterpret_cast<uint32_t *>(take(4 * n1));
+        d_mst = reinterpret_cast<InfState *>(take(sizeof(InfState) * n1));
+        k_mem_emit<<<(unsigned)ntiles, 256, 0, st>>>(d_src, n, d_tbase, d_off, d_len);
+        k_mem_jump<<<1, 1024, 0, st>>>(d_off, d_len, nc, levels, d_jmp);
+        launches += 2;
+        cand.resize(nc);
+        CKI(cudaMemcpyAsync(cand.data(), d_off, 8 * (size_t)nc, cudaMemcpyDeviceToHost, st));
+        CKI(cudaStreamSynchronize(st));
+        CKI(cudaGetLastError());
+    }
+    uint64_t in = 0, out = 0;
+    uint32_t check = 0;
+    int status = ZB_OK;
+    for (bool first = true;; first = false) {
+        if (!first) { // another member only behind 1f 8b (gz_look)
+            if (n - in < 2) break;
+            uint8_t magic[2];
+            CKI(cudaMemcpy(magic, d_src + in, 2, cudaMemcpyDeviceToHost));
+            if (magic[0] != 0x1f || magic[1] != 0x8b) break;
+        }
+        const auto it = std::lower_bound(cand.begin(), cand.end(), in);
+        if (it != cand.end() && *it == in) {
+            // ---- a run of BGZF members starts here
+            k_mem_chain<<<1, 1024, 0, st>>>(d_src, d_off, d_len, d_jmp, nc, levels, (uint32_t)(it - cand.begin()), dst_cap - out, d_moff,
+                                            d_mlen, d_misz, d_mout, d_ctl);
+            launches += 1;
+            CKI(cudaMemcpyAsync(&h_ctl, d_ctl, sizeof h_ctl, cudaMemcpyDeviceToHost, st));
+            CKI(cudaStreamSynchronize(st));
+            if (h_ctl.fit) {
+                k_members<<<h_ctl.fit, 32, sizeof(InfShared), st>>>(d_src, d_moff, d_mlen, d_misz, d_mout, d_dst + out, window_bits, d_mst);
+                CKI(launch_crc32_segments(d_dst + out, d_mout, d_misz, h_ctl.fit, d_mcrc, st));
+                k_mem_verdict<<<1, 1024, 0, st>>>(d_mst, d_mcrc, d_moff, d_mlen, d_misz, d_mout, d_ctl);
+                CKI(launch_crc32_join(d_mcrc, d_misz, &d_ctl->good, &d_ctl->good_crc, st));
+                launches += 4;
+                CKI(cudaMemcpyAsync(&h_ctl, d_ctl, sizeof h_ctl, cudaMemcpyDeviceToHost, st));
+                CKI(cudaStreamSynchronize(st));
+                CKI(cudaGetLastError());
+                check = (uint32_t)crc32_combine64(check, h_ctl.good_crc, (z_off64_t)h_ctl.good_out);
+                out += h_ctl.good_out;
+                in += h_ctl.good_in;
+                if (h_ctl.good == h_ctl.count) continue;
+            }
+            // the member at `in` goes to inflate_stream: its hints were wrong, it failed, or it does not fit dst
+        }
+        zb_inflate_result r;
+        memset(&r, 0, sizeof r);
+        const int st1 = inflate_stream(d_src + in, n - in, d_dst + out, dst_cap - out, window_bits, 0, &r);
+        if (st1 != ZB_OK) {
+            if (st1 != ZB_E_BUF && st1 != ZB_E_DATA) return st1;
+            status = st1;
+            memcpy(res->msg, r.msg, sizeof res->msg);
+            break;
+        }
+        check = (uint32_t)crc32_combine64(check, r.check, (z_off64_t)r.out_bytes);
+        out += r.out_bytes;
+        in += r.in_bytes;
+    }
+    res->out_bytes = out;
+    res->in_bytes = in;
+    res->check = check;
+    return status;
+}
+
+// One stream at d_src[0, n) into d_dst[0, dst_cap): the block-parallel path, or k_inflate; then the check value and the trailer.
+int Engine::inflate_stream(const uint8_t *d_src, size_t n, uint8_t *d_dst, size_t dst_cap, int window_bits, uint32_t flags,
+                           zb_inflate_result *res)
+{
+    int rc;
+    void *p;
+    InfState *dis = static_cast<InfState *>(d_inf_state), *his = static_cast<InfState *>(h_inf_state);
     bool done = false;
     const char *declined = "small"; // the stage of the block-parallel path that gave up (reported with ZB_INF_NO_SERIAL)
     if (n >= 65536) {
@@ -1346,11 +1672,6 @@ int Engine::inflate(const void *src, size_t n, bool src_dev, void *dst, size_t d
     }
     if (!done && (flags & ZB_INF_NO_SERIAL)) {
         snprintf(res->msg, sizeof res->msg, "%s", declined);
-        CKI(cudaEventRecord(ev1, st));
-        CKI(cudaStreamSynchronize(st));
-        CKI(cudaEventElapsedTime(&res->gpu_ms, ev0, ev1));
-        res->status = ZB_E_DECLINED;
-        res->gpu_launches = launches;
         return ZB_E_DECLINED;
     }
     if (!done) {
@@ -1385,12 +1706,6 @@ int Engine::inflate(const void *src, size_t n, bool src_dev, void *dst, size_t d
         if (check != his->trailer_check) { status = ZB_E_DATA; snprintf(res->msg, sizeof res->msg, "incorrect data check"); }
         else if (his->kind == 2 && (uint32_t)his->out_bytes != his->trailer_len) { status = ZB_E_DATA; snprintf(res->msg, sizeof res->msg, "incorrect length check"); }
     }
-    if (!dst_dev && his->out_bytes) CKI(cudaMemcpyAsync(dst, d_dst, his->out_bytes, cudaMemcpyDeviceToHost, st));
-    CKI(cudaEventRecord(ev1, st));
-    CKI(cudaStreamSynchronize(st));
-    CKI(cudaEventElapsedTime(&res->gpu_ms, ev0, ev1));
-    res->status = status;
-    res->gpu_launches = launches;
     return status;
 }
 

@@ -120,5 +120,9 @@ cudaError_t launch_adler32(const uint8_t *d_buf, uint64_t len, uint32_t start, v
                            cudaStream_t st);
 cudaError_t launch_crc32(const uint8_t *d_buf, uint64_t len, uint32_t start, void *d_scratch, size_t scratch_bytes, uint32_t *d_out,
                          cudaStream_t st);
+// crc32 of every segment [off[s], off[s] + len[s]) of d_buf, and the crc32_combine of the first *d_count of them (multi-member gzip)
+cudaError_t launch_crc32_segments(const uint8_t *d_buf, const uint64_t *d_off, const uint32_t *d_len, uint32_t nseg, uint32_t *d_crc,
+                                  cudaStream_t st);
+cudaError_t launch_crc32_join(const uint32_t *d_crc, const uint32_t *d_len, const uint32_t *d_count, uint32_t *d_out, cudaStream_t st);
 
 } // namespace zb
