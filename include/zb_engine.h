@@ -76,6 +76,22 @@ ZB_API int zb_deflate(zb_engine *e, const void *src, size_t src_len, int src_on_
                                    starts with `bits` (< 8) bits of `val` (the partial last byte of the previous segment) */
 #define ZB_FLAG_MEMLEVEL(m) ((uint32_t)(m) << 8) /* deflateInit2's memLevel 1..9 (0 = default 8): lit_bufsize = 1 << (memLevel + 6)
                                                     sets the symbols per block (zlib-rs/src/deflate.rs:321, deflate/sym_buf.rs:23) */
+#define ZB_FLAG_BGZF 64u /* write a BGZF file (SAM/BAM specification 4.1: BAM, .vcf.gz, tabix, bgzip).  Only with window_bits 31,
+                            Z_DEFAULT_STRATEGY, level -1..9 and no other flag (memLevel 8); anything else gives ZB_E_PARAM.  The input
+                            is cut into blocks of 65280 bytes (0xff00, htslib's BGZF_BLOCK_SIZE; the last may be shorter, an empty input
+                            has none), and block m becomes one member:
+                              header   1f 8b 08 04 00000000 00 ff 0600 'B' 'C' 0200 BSIZE  (MTIME 0, XFL 0, OS 255, BSIZE = member
+                                       length - 1, little-endian)
+                              payload  the raw deflate stream of that block alone, byte for byte what deflateInit2(level, Z_DEFLATED,
+                                       -15, 8, Z_DEFAULT_STRATEGY) + deflate(Z_FINISH) give -- except when it would make the member
+                                       longer than 65536 bytes (BSIZE is 16 bits): then the block is written as one stored block,
+                                       01 LEN NLEN data.  Only level 1 (deflate_quick: one static block, no stored fallback) on
+                                       incompressible data gets there; htslib's libdeflate path does the same.
+                              trailer  crc32 and ISIZE of the block.
+                            The file ends with the 28-byte empty BGZF member that marks a BGZF end of file.  out_bytes is the file
+                            length, check the crc32 of the whole input, n_blocks the deflate blocks of all members, exact_parity 1.
+                            dst_cap below the file length gives ZB_E_BUF; zb_bgzf_bound(n) is always enough.  The members are
+                            compressed side by side: the launches of a call do not depend on its length. */
 ZB_API int zb_deflate_ex(zb_engine *e, const void *src, size_t src_len, int src_on_device, void *dst, size_t dst_cap, int dst_on_device,
                   int level, int strategy, int window_bits, uint32_t flags, zb_deflate_result *res);
 /* deflate with a preset dictionary (deflateSetDictionary, zlib-rs/src/deflate.rs:498-564): raw streams only (window_bits < 0; the
@@ -85,6 +101,7 @@ ZB_API int zb_deflate_ex(zb_engine *e, const void *src, size_t src_len, int src_
 ZB_API int zb_deflate_dict(zb_engine *e, const void *dict, size_t dict_len, const void *src, size_t src_len, int src_on_device, void *dst,
                            size_t dst_cap, int dst_on_device, int level, int strategy, int window_bits, uint32_t flags, zb_deflate_result *res);
 ZB_API size_t zb_deflate_bound(size_t src_len);
+ZB_API size_t zb_bgzf_bound(size_t src_len); /* ceil(src_len / 65280) * 65536 + 28: the largest ZB_FLAG_BGZF file */
 
 typedef struct zb_inflate_result {
     uint64_t out_bytes;

@@ -26,6 +26,7 @@ ZB_FLAG_NOT_LAST = 1
 ZB_FLAG_LOW_PARALLEL = 2
 ZB_FLAG_CHECK_ADLER = 4
 ZB_FLAG_CHECK_CRC = 8
+ZB_FLAG_BGZF = 64  # Engine.deflate with window_bits 31: a BGZF file, every 65280-byte block its own member (zb_engine.h)
 ZB_INF_CHECK_ADLER = 1
 ZB_INF_CHECK_CRC = 2
 ZB_INF_NO_SERIAL = 4  # Engine.inflate: only the block-parallel decoder; ZB_E_DECLINED with the stage in res.msg when it gives up
@@ -129,6 +130,7 @@ def lib():
         L.zb_deflate.argtypes = [vp, vp, sz, ci, vp, sz, ci, ci, ci, ci, ctypes.POINTER(DeflateResult)]
         L.zb_deflate_ex.argtypes = [vp, vp, sz, ci, vp, sz, ci, ci, ci, ci, u32, ctypes.POINTER(DeflateResult)]
         L.zb_deflate_bound.argtypes, L.zb_deflate_bound.restype = [sz], sz
+        L.zb_bgzf_bound.argtypes, L.zb_bgzf_bound.restype = [sz], sz
         L.zb_inflate.argtypes = [vp, vp, sz, ci, vp, sz, ci, ci, ctypes.POINTER(InflateResult)]
         L.zb_inflate_ex.argtypes = [vp, vp, sz, ci, vp, sz, ci, ci, u32, ctypes.POINTER(InflateResult)]
         L.zb_adler32.argtypes = [vp, u32, vp, sz, ci, ctypes.POINTER(u32), ctypes.POINTER(ctypes.c_float)]
@@ -155,6 +157,11 @@ def _buf(data):
 
 
 # ---------------------------------------------------------------- one-shot API (libz-rs-sys names)
+def bgzf_bound(n):
+    """Largest file Engine.deflate(..., window_bits=31, flags=ZB_FLAG_BGZF) writes for n input bytes: ceil(n / 65280) * 65536 + 28."""
+    return lib().zb_bgzf_bound(n)
+
+
 def compressBound(n):
     return lib().compressBound(n)
 
@@ -361,7 +368,7 @@ class Engine:
             src = ctypes.addressof(keep)
         own = None
         if dst is None:
-            dst_cap = lib().zb_deflate_bound(n) + 64
+            dst_cap = (lib().zb_bgzf_bound(n) if flags & ZB_FLAG_BGZF else lib().zb_deflate_bound(n)) + 64
             own = ctypes.create_string_buffer(dst_cap)
             dst = ctypes.addressof(own)
             dst_on_device = False

@@ -1,0 +1,164 @@
+// zb_bgzf.cu -- BGZF writing (ZB_FLAG_BGZF, zb_bgzf.h, DESIGN.md §2h): the member parsers of levels 3..9, the member sizes and
+// offsets, and the framing.  Every kernel covers all members of the call, so a call costs the same launches whatever its length.
+// Levels 1/2 parse in k_serial_low_members (zb_serial.cu); the block kernels k_bgzf_hist / k_bgzf_build / k_bgzf_encode share their
+// bodies with the single-stream ones (zb_kernels.cu).
+#include "zb_kernels.cuh"
+
+namespace zb {
+
+__global__ void __launch_bounds__(256) k_bgzf_setup(BgzfJob bj, uint64_t n)
+{
+    const uint32_t m = blockIdx.x * 256 + threadIdx.x;
+    if (m == 0) bj.ctl->count = bj.nm;
+    if (m >= bj.nm) return;
+    bj.moff[m] = (uint64_t)m * kBgzfStride;
+    bj.mlen[m] = bgzf_member_len(n, m);
+}
+
+// Levels 3..6: lane 0 runs the exact serial simulator over the whole member, as k_tail does over a short stream.  There are no
+// holes to iterate on: the simulator keeps its own inserted-positions bitmap (in shared memory, one bit per position of a member).
+__global__ void __launch_bounds__(32) k_bgzf_medium(JobBufs jb, BgzfJob bj)
+{
+    __shared__ uint32_t ins[kBgzfBlock / 32];
+    if (threadIdx.x != 0) return;
+    const uint32_t m = blockIdx.x, base = m * kBgzfStride, len = bj.mlen[m], bs = jb.block_syms;
+    const BgzfAcc a{jb.in + base, jb.L + base, len, 4u};
+    Sym *syms = jb.syms + base;
+    uint32_t *bb = jb.block_base + m * kBgzfMaxBlocks;
+    uint32_t k = 0, left = bs, blk = 0;
+    auto emit = [&](const Sym &s, uint32_t B) {
+        syms[k++] = s;
+        if (--left == 0) { bb[blk++] = B; left = bs; } // the window base when this symbol fills the block (k_block_hist's sym_base)
+    };
+    const uint32_t fb = serial_medium(a, len, 0, ins, kBgzfBlock / 32, jb.lp, emit);
+    JobInfo &mi = bj.minfo[m];
+    mi.n_syms = k;
+    mi.final_base = fb;
+    mi.n_blocks = k / bs + 1;
+}
+
+// Levels 7..9: deflate_slow has no holes, so the macro step from a fresh loop-top is a function of its position (zb_slow.h).  One
+// thread per staged position evaluates it through the member-relative accessor.
+__global__ void __launch_bounds__(256) k_bgzf_slow_steps(JobBufs jb, BgzfJob bj)
+{
+    const uint32_t x = blockIdx.x * 256 + threadIdx.x, m = x / kBgzfStride, y = x % kBgzfStride;
+    if (m >= bj.nm) return;
+    const uint32_t len = bj.mlen[m];
+    if (y >= len) return;
+    const BgzfAcc a{jb.in + (x - y), jb.L + (x - y), len, jb.sp.slow ? 3u : 4u};
+    const SlowStep s = slow_step(a, y, len, jb.sp);
+    jb.M[x] = pack_step(s);
+    jb.nxt[x] = s.next;
+}
+
+// ... and one thread per member walks the steps from position 0 and writes the symbols (k_emit_slow + k_tail_slow of one member).
+__global__ void __launch_bounds__(32) k_bgzf_slow_walk(JobBufs jb, BgzfJob bj)
+{
+    const uint32_t m = blockIdx.x * 32 + threadIdx.x;
+    if (m >= bj.nm) return;
+    const uint32_t base = m * kBgzfStride, len = bj.mlen[m], bs = jb.block_syms;
+    const uint8_t *d = jb.in + base;
+    const uint32_t *M = jb.M + base, *nxt = jb.nxt + base;
+    Sym *syms = jb.syms + base;
+    uint32_t n = 0;
+    for (uint32_t p = 0; p < len;) {
+        const uint32_t v = M[p], nlit = v >> 24;
+        for (uint32_t i = 0; i < nlit; i++) syms[n++] = Sym{0, d[p + i], p + i};
+        if (v & 0x8000u) syms[n++] = Sym{(uint16_t)((v & 0x7fffu) + 1u), (uint16_t)((v >> 16) & 0xffu), p + nlit};
+        const uint32_t q = nxt[p];
+        if (q <= p) { atomicOr(&bj.ctl->error, 2u); return; }
+        p = q;
+    }
+    JobInfo &mi = bj.minfo[m];
+    mi.n_syms = n;
+    mi.final_base = base_at(len, len, jb.wsize);
+    uint32_t nb = n / bs + 1;
+    // k_tail_slow's rule: a pending last literal tallied into a just-filled symbol buffer makes that block the last one
+    if (n > 0 && n % bs == 0 && syms[n - 1].dist == 0 && syms[n - 1].pos + 1 == len) nb--;
+    mi.n_blocks = nb;
+}
+
+// One thread per member: the payload's length from its blocks (stored blocks align to a byte, as in k_scan_blocks), the stored
+// fallback, the member's length in the file.  The blocks' bit positions are left relative to the payload.
+__global__ void __launch_bounds__(256) k_bgzf_size(JobBufs jb, BgzfJob bj)
+{
+    const uint32_t m = blockIdx.x * 256 + threadIdx.x;
+    if (m >= bj.nm) return;
+    const uint32_t len = bj.mlen[m];
+    bool stored = jb.level == 0;
+    uint64_t payload = 0;
+    uint32_t nb = 1;
+    if (!stored) {
+        nb = bj.minfo[m].n_blocks;
+        if (nb == 0 || nb > kBgzfMaxBlocks) { atomicOr(&bj.ctl->error, 1u); return; }
+        uint64_t bit = 0;
+        for (uint32_t k = 0; k < nb; k++) {
+            BlockDesc &bd = jb.blocks[m * kBgzfMaxBlocks + k];
+            bd.bit_base = bit;
+            bit = bd.type == 0 ? ((bit + 3 + 7) & ~7ull) + 32 + 8ull * (uint16_t)bd.in_len : bit + bd.hdr_bits + bd.body_bits;
+        }
+        payload = (bit + 7) >> 3;
+        atomicAdd(&bj.ctl->n_syms, bj.minfo[m].n_syms);
+        if (bgzf_stored(payload)) { stored = true; nb = 1; }
+    }
+    if (stored) payload = bgzf_stored_payload(len);
+    atomicAdd(&bj.ctl->n_blocks, nb);
+    bj.mstored[m] = stored;
+    bj.mbytes[m] = kBgzfHeader + (uint32_t)payload + kBgzfTrailer;
+}
+
+// One CTA: the members' offsets in the file (exclusive scan of their lengths), the blocks' absolute bit positions, the file length.
+__global__ void __launch_bounds__(1024) k_bgzf_scan(JobBufs jb, BgzfJob bj)
+{
+    __shared__ uint64_t part[1024];
+    const uint32_t tid = threadIdx.x, n = bj.nm, per = (n + 1023) / 1024;
+    const uint32_t beg = min(n, tid * per), end = min(n, beg + per);
+    if (bj.ctl->error) return;
+    uint64_t s = 0;
+    for (uint32_t i = beg; i < end; i++) s += bj.mbytes[i];
+    part[tid] = s;
+    __syncthreads();
+    for (uint32_t h = 1; h < 1024; h <<= 1) {
+        const uint64_t v = tid >= h ? part[tid - h] : 0;
+        __syncthreads();
+        part[tid] += v;
+        __syncthreads();
+    }
+    uint64_t off = part[tid] - s;
+    for (uint32_t i = beg; i < end; i++) {
+        bj.mout[i] = off;
+        if (!bj.mstored[i]) {
+            const uint32_t nb = bj.minfo[i].n_blocks;
+            for (uint32_t k = 0; k < nb; k++) jb.blocks[i * kBgzfMaxBlocks + k].bit_base += 8ull * (off + kBgzfHeader);
+        }
+        off += bj.mbytes[i];
+    }
+    if (tid == 1023) bj.ctl->out_bytes = part[1023] + kBgzfEofLen;
+    if (tid == 0) bj.ctl->data_type = (n && !bj.mstored[0] && jb.blocks[0].sym_count) ? jb.blocks[0].data_type : 2u;
+}
+
+// One CTA per member: header with BSIZE, trailer, and the stored block of a member written stored; the last CTA writes the
+// end-of-file member.  Runs behind k_bgzf_encode (the payload bits are OR-ed into the zeroed output).
+__global__ void __launch_bounds__(256) k_bgzf_frame(JobBufs jb, BgzfJob bj)
+{
+    const uint32_t m = blockIdx.x, tid = threadIdx.x;
+    if (bj.ctl->error) return;
+    if (m == bj.nm) {
+        if (tid < kBgzfEofLen) jb.out[bj.ctl->out_bytes - kBgzfEofLen + tid] = bgzf_eof(tid);
+        return;
+    }
+    uint8_t *o = jb.out + bj.mout[m];
+    const uint32_t len = bj.mlen[m], bytes = bj.mbytes[m];
+    const bool stored = bj.mstored[m] != 0;
+    if (tid == 0) {
+        bgzf_header(o, bytes);
+        bgzf_trailer(o + bytes - kBgzfTrailer, bj.mcrc[m], len);
+        if (stored) bgzf_stored_header(o + kBgzfHeader, len);
+    }
+    if (stored) {
+        const uint8_t *src = jb.in + m * kBgzfStride;
+        for (uint32_t i = tid; i < len; i += 256) o[kBgzfHeader + 5 + i] = src[i];
+    }
+}
+
+} // namespace zb

@@ -60,6 +60,18 @@ __global__ void k_tail_slow(JobBufs);
 __global__ void k_serial_low(JobBufs);
 __global__ void k_links_dict_ghost(JobBufs, uint32_t *);
 __global__ void k_links_dict_ghost_apply(JobBufs, const uint32_t *);
+// BGZF writing (zb_bgzf.cu, zb_serial.cu, zb_kernels.cu)
+__global__ void k_bgzf_setup(BgzfJob, uint64_t);
+__global__ void k_serial_low_members(JobBufs, BgzfJob);
+__global__ void k_bgzf_medium(JobBufs, BgzfJob);
+__global__ void k_bgzf_slow_steps(JobBufs, BgzfJob);
+__global__ void k_bgzf_slow_walk(JobBufs, BgzfJob);
+__global__ void k_bgzf_hist(JobBufs, BgzfJob, uint32_t *);
+__global__ void k_bgzf_build(JobBufs, BgzfJob, const uint32_t *);
+__global__ void k_bgzf_size(JobBufs, BgzfJob);
+__global__ void k_bgzf_scan(JobBufs, BgzfJob);
+__global__ void k_bgzf_encode(JobBufs, BgzfJob);
+__global__ void k_bgzf_frame(JobBufs, BgzfJob);
 
 constexpr uint32_t kMatchSmemBytes = (kWSize + kMatchSub + 512) + (kWSize + kMatchSub) * 2 + ((kWSize + kMatchSub) / 32 + 1) * 4 * 4 + 8192;
 constexpr uint32_t kPathSmemBytes = kPathTile * 4 * 3;
@@ -103,6 +115,7 @@ int Engine::init(int dev)
     CK(cudaFuncSetAttribute(k_path_groups, cudaFuncAttributeMaxDynamicSharedMemorySize, kChain2MaxSmem));
     CK(cudaFuncSetAttribute(k_path_chain2, cudaFuncAttributeMaxDynamicSharedMemorySize, kChain2MaxSmem));
     CK(cudaFuncSetAttribute(k_serial_low, cudaFuncAttributeMaxDynamicSharedMemorySize, kSerialSmemBytes));
+    CK(cudaFuncSetAttribute(k_serial_low_members, cudaFuncAttributeMaxDynamicSharedMemorySize, kSerialSmemBytes));
     CK(cudaMallocHost(&h_info, sizeof(JobInfo)));
     CK(cudaMalloc(&d_info, sizeof(JobInfo)));
     CK(cudaMalloc(&d_check, 16));
@@ -189,6 +202,15 @@ int Engine::deflate(const void *src, size_t n_in, bool src_dev, void *dst, size_
     // A preset dictionary (deflate::set_dictionary, deflate.rs:498-564) is the input's prefix in the window: the kernels work on
     // dictionary ++ input in absolute coordinates and start parsing at `dstart`.  A dictionary that would fill the window
     // (>= 2 * w_size) is cut to its last w_size bytes (:517-531).
+    if (flags & ZB_FLAG_BGZF) {
+        const uint32_t ml = (flags >> 8) & 15u; // memLevel 8, given or by default
+        if ((flags & ~(ZB_FLAG_BGZF | ZB_FLAG_MEMLEVEL(15))) || (ml && ml != 8) || dict_len || window_bits != 31 || strategy != 0 ||
+            level < -1 || level > 9) {
+            snprintf(g_err, sizeof g_err, "ZB_FLAG_BGZF takes window_bits 31, Z_DEFAULT_STRATEGY, level -1..9 and no other flag");
+            return ZB_E_PARAM;
+        }
+        return deflate_bgzf(src, n_in, src_dev, dst, dst_cap, dst_dev, level, res);
+    }
     size_t dstart = 0;
     if (dict_len) {
         if (!dict || window_bits >= 0) { snprintf(g_err, sizeof g_err, "a dictionary needs a raw stream (the caller frames FDICT / DICTID)"); return ZB_E_PARAM; }
@@ -657,6 +679,158 @@ int Engine::deflate(const void *src, size_t n_in, bool src_dev, void *dst, size_
     return ZB_OK;
 }
 
+// ZB_FLAG_BGZF (zb_bgzf.h, DESIGN.md §2h): every 65280-byte block of the input is deflated alone and framed as one BGZF member.  The
+// members are staged side by side and every kernel covers all of them, so a call costs a fixed number of launches and two host
+// syncs (the file length, then the end of the copy) whatever its length.
+int Engine::deflate_bgzf(const void *src, size_t n, bool src_dev, void *dst, size_t dst_cap, bool dst_dev, int level, zb_deflate_result *res)
+{
+    if (!res || (!src && n) || !dst) return ZB_E_PARAM;
+    memset(res, 0, sizeof *res);
+    const uint64_t nm64 = bgzf_members(n);
+    if (nm64 >= 65535) { snprintf(g_err, sizeof g_err, "input too large for one job (%zu)", n); return ZB_E_PARAM; } // staged offsets are 32-bit
+    if (level == -1) level = 6;
+    CK(cudaSetDevice(device));
+    launches = 0;
+    const uint32_t nm = (uint32_t)nm64;
+    const uint32_t S = nm ? (nm - 1) * kBgzfStride + bgzf_member_len(n, nm - 1) : 0; // staged length: the link kernels' N
+    const size_t span = (size_t)nm * kBgzfStride;
+    const uint32_t nmt = S / kLinkTile + 1, nslots = nm * kBgzfMaxBlocks;
+    const bool links = level >= 3, slow = level >= 7;
+    JobBufs jb;
+    memset(&jb, 0, sizeof jb);
+    int rc;
+    void *p;
+#define RES(slot, bytes, field, type)                                   \
+    if ((rc = reserve(slot, bytes, &p)) != ZB_OK) return rc;            \
+    jb.field = static_cast<type>(p);
+    RES(S_IN, span + kPad + 16, in, const uint8_t *)
+    uint8_t *d_in = const_cast<uint8_t *>(jb.in);
+    jb.N = S;
+    jb.level = (uint32_t)level;
+    jb.wsize = kWSize;
+    jb.block_syms = kBlockSyms; // memLevel 8; deflate_quick's pieces have the same size
+    jb.serial_mode = level == 1 || level == 2 ? (uint32_t)level : 0u;
+    if (level >= 3 && level <= 6) jb.lp = level_params(level);
+    if (slow) { jb.slow_mode = 1; jb.sp = slow_params(level); jb.sp.wsize = kWSize; }
+    const size_t out_cap = (bgzf_bound(n) + 15) & ~(size_t)15;
+    RES(S_OUT, out_cap + 16, out, uint8_t *)
+    jb.out_cap = out_cap;
+    uint32_t *d_freq = nullptr;
+    if (level > 0 && nm) {
+        RES(S_SYMS, (span + 64) * sizeof(Sym), syms, Sym *)
+        RES(S_BLOCKS, (size_t)nslots * sizeof(BlockDesc), blocks, BlockDesc *)
+        RES(S_BBASE, (size_t)nslots * 4, block_base, uint32_t *)
+        if ((rc = reserve(S_FREQ, (size_t)nslots * 320 * 4, &p)) != ZB_OK) return rc;
+        d_freq = static_cast<uint32_t *>(p);
+    }
+    if (links && nm) {
+        RES(S_L, (span + kPad) * 2, L, uint16_t *)
+        RES(S_KEYS, (span + kPad) * 2, keys, uint16_t *)
+        RES(S_LLAST, (size_t)nmt * 65536 * 2, link_last, uint16_t *)
+    }
+    if (slow && nm) {
+        RES(S_M, span * 4, M, uint32_t *)
+        RES(S_NXT, span * 4, nxt, uint32_t *)
+    }
+#undef RES
+    // member tables: moff | mout (8 bytes each) | mlen | mcrc | mbytes | mstored | minfo | ctl
+    const size_t m8 = ((size_t)nm * 8 + 15) & ~(size_t)15, m4 = ((size_t)nm * 4 + 15) & ~(size_t)15;
+    const size_t mi_bytes = ((size_t)nm * sizeof(JobInfo) + 15) & ~(size_t)15;
+    if ((rc = reserve(S_BGZF, 2 * m8 + 4 * m4 + mi_bytes + sizeof(BgzfCtl), &p)) != ZB_OK) return rc;
+    uint8_t *t = static_cast<uint8_t *>(p);
+    BgzfJob bj;
+    bj.nm = nm;
+    bj.moff = reinterpret_cast<uint64_t *>(t);
+    bj.mout = reinterpret_cast<uint64_t *>(t + m8);
+    bj.mlen = reinterpret_cast<uint32_t *>(t + 2 * m8);
+    bj.mcrc = reinterpret_cast<uint32_t *>(t + 2 * m8 + m4);
+    bj.mbytes = reinterpret_cast<uint32_t *>(t + 2 * m8 + 2 * m4);
+    bj.mstored = reinterpret_cast<uint32_t *>(t + 2 * m8 + 3 * m4);
+    bj.minfo = reinterpret_cast<JobInfo *>(t + 2 * m8 + 4 * m4);
+    bj.ctl = reinterpret_cast<BgzfCtl *>(t + 2 * m8 + 4 * m4 + mi_bytes);
+    if ((rc = stage(sizeof(BgzfCtl) + 16)) != ZB_OK) return rc;
+
+    CK(cudaEventRecord(ev0, st));
+    // staging: one pitched copy of the whole blocks, the short last one, zeros in the gaps and behind the last member
+    const cudaMemcpyKind kind = src_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+    const uint8_t *s8 = static_cast<const uint8_t *>(src);
+    if (nm > 1) {
+        CK(cudaMemcpy2DAsync(d_in, kBgzfStride, s8, kBgzfBlock, kBgzfBlock, nm - 1, kind, st));
+        CK(cudaMemset2DAsync(d_in + kBgzfBlock, kBgzfStride, 0, kBgzfStride - kBgzfBlock, nm - 1, st));
+    }
+    if (nm) CK(cudaMemcpyAsync(d_in + (size_t)(nm - 1) * kBgzfStride, s8 + (size_t)(nm - 1) * kBgzfBlock, S - (nm - 1) * kBgzfStride, kind, st));
+    CK(cudaMemsetAsync(d_in + S, 0, span - S + kPad + 16, st));
+    CK(cudaMemsetAsync(bj.minfo, 0, mi_bytes + sizeof(BgzfCtl), st));
+    CK(cudaMemsetAsync(jb.out, 0, out_cap, st));
+    k_bgzf_setup<<<nm / 256 + 1, 256, 0, st>>>(bj, (uint64_t)n);
+    CK(launch_crc32_segments(d_in, bj.moff, bj.mlen, nm, bj.mcrc, st));
+    CK(launch_crc32_join(bj.mcrc, bj.mlen, &bj.ctl->count, d_check, st));
+    launches += 3;
+    if (level > 0 && nm) {
+        if (links) {
+            if (jb.sp.slow) {
+                k_links2_roll<<<nmt, 1024, kLinks2SmemBytes, st>>>(jb, 0);
+                k_links_fix_roll<<<S / 256 + 1, 256, 0, st>>>(jb);
+            } else {
+                k_links2_std<<<nmt, 1024, kLinks2SmemBytes, st>>>(jb, 0);
+                k_links_fix_std<<<S / 256 + 1, 256, 0, st>>>(jb);
+            }
+            launches += 2;
+        }
+        if (jb.serial_mode) {
+            k_serial_low_members<<<nm, 32, jb.serial_mode == 2 ? kSerialSmemBytes : kSerialSmemQuick, st>>>(jb, bj);
+            launches++;
+        } else if (!slow) {
+            k_bgzf_medium<<<nm, 32, 0, st>>>(jb, bj);
+            launches++;
+        } else {
+            k_bgzf_slow_steps<<<nm * (kBgzfStride / 256), 256, 0, st>>>(jb, bj);
+            k_bgzf_slow_walk<<<(nm + 31) / 32, 32, 0, st>>>(jb, bj);
+            launches += 2;
+        }
+        k_bgzf_hist<<<nslots, 256, 0, st>>>(jb, bj, d_freq);
+        k_bgzf_build<<<nslots, 32, 0, st>>>(jb, bj, d_freq);
+        launches += 2;
+    }
+    k_bgzf_size<<<nm / 256 + 1, 256, 0, st>>>(jb, bj);
+    k_bgzf_scan<<<1, 1024, 0, st>>>(jb, bj);
+    launches += 2;
+    if (level > 0 && nm) {
+        k_bgzf_encode<<<nslots, 1024, 0, st>>>(jb, bj);
+        launches++;
+    }
+    k_bgzf_frame<<<nm + 1, 256, 0, st>>>(jb, bj);
+    launches++;
+    CK(cudaGetLastError());
+    BgzfCtl *h_ctl = static_cast<BgzfCtl *>(h_stage);
+    uint32_t *h_crc = reinterpret_cast<uint32_t *>(h_ctl + 1);
+    CK(cudaMemcpyAsync(h_ctl, bj.ctl, sizeof(BgzfCtl), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(h_crc, d_check, 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (h_ctl->error) { snprintf(g_err, sizeof g_err, "engine error flags 0x%x (bgzf)", h_ctl->error); return ZB_E_INTERNAL; }
+    const uint64_t out_bytes = h_ctl->out_bytes;
+    if (out_bytes > dst_cap) {
+        res->out_bytes = out_bytes;
+        return ZB_E_BUF;
+    }
+    CK(cudaMemcpyAsync(dst, jb.out, out_bytes, dst_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
+    CK(cudaEventRecord(ev1, st));
+    CK(cudaStreamSynchronize(st));
+    float ms = 0;
+    CK(cudaEventElapsedTime(&ms, ev0, ev1));
+    res->out_bytes = out_bytes;
+    res->check = *h_crc;
+    res->data_type = (int32_t)h_ctl->data_type;
+    res->iterations = level > 0 ? 1 : 0;
+    res->n_symbols = h_ctl->n_syms;
+    res->n_blocks = h_ctl->n_blocks;
+    res->gpu_launches = launches;
+    res->exact_parity = 1;
+    res->gpu_ms = ms;
+    res->bits_used = 8;
+    return ZB_OK;
+}
+
 int Engine::checksum(bool crc, uint32_t start, const void *buf, size_t len, bool on_dev, uint32_t *out, float *ms_out)
 {
     if (!out) return ZB_E_PARAM;
@@ -748,6 +922,8 @@ int zb_deflate_ex(zb_engine *z, const void *src, size_t n, int src_dev, void *ds
 }
 
 size_t zb_deflate_bound(size_t n) { return zb::deflate_bound(n); }
+
+size_t zb_bgzf_bound(size_t n) { return (size_t)zb::bgzf_bound(n); }
 
 int zb_inflate(zb_engine *z, const void *src, size_t n, int src_dev, void *dst, size_t cap, int dst_dev, int window_bits,
                zb_inflate_result *res)

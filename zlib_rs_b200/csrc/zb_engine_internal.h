@@ -15,6 +15,7 @@ size_t deflate_bound(size_t n);
 enum { S_IN, S_L, S_HOLES, S_HOLESN, S_M, S_NXT, S_PEXIT, S_PCNT, S_SYMIDX, S_TENTRY, S_TSYMB, S_TDIRTY, S_SYMS, S_SYMB,
        S_BLOCKS, S_SCRATCH, S_FREQ, S_OUT, S_CK, S_INF0, S_INF1, S_PHEAD, S_SK, S_MARKN, S_LLIST, S_LCNT, S_BMAP, S_HDIFF, S_HCOARSE, S_CSTATE, S_LISTS, S_LR, S_LLAST, S_BBASE, S_MCHG, S_GFN, S_KEYS, S_SHARD,
        S_MEMT, S_MEMC, // multi-member gzip: tile counts and control block; candidate and member tables
+       S_BGZF,         // BGZF writing: member tables and control block
        S_COUNT };
 
 // A range job of chunk-sharded deflate (zb_shard_*, zb_shard.cu) between its four calls.
@@ -31,7 +32,7 @@ struct ShardState {
 };
 
 struct Engine {
-    static constexpr int kSlots = 40;
+    static constexpr int kSlots = 41;
     struct Buf { void *p = nullptr; size_t cap = 0; };
     int device = -1;
     cudaStream_t st = nullptr, st2 = nullptr; // st2: the serial tail runs beside k_emit
@@ -65,6 +66,7 @@ struct Engine {
     int stage(size_t bytes);
     int deflate(const void *src, size_t n, bool src_dev, void *dst, size_t dst_cap, bool dst_dev, int level, int strategy,
                 int window_bits, uint32_t flags, zb_deflate_result *res, const void *dict = nullptr, size_t dict_len = 0);
+    int deflate_bgzf(const void *src, size_t n, bool src_dev, void *dst, size_t dst_cap, bool dst_dev, int level, zb_deflate_result *res);
     int inflate(const void *src, size_t n, bool src_dev, void *dst, size_t dst_cap, bool dst_dev, int window_bits,
                 zb_inflate_result *res, uint32_t flags = 0);
     int inflate_stream(const uint8_t *d_src, size_t n, uint8_t *d_dst, size_t dst_cap, int window_bits, uint32_t flags,

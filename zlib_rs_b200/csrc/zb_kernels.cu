@@ -1315,18 +1315,15 @@ __global__ void __launch_bounds__(32) k_tail(JobBufs jb)
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t sym_end(const Sym &s) { return s.pos + (s.dist ? (uint32_t)s.lc + 3u : 1u); }
 
-__global__ void __launch_bounds__(256) k_block_hist(JobBufs jb, uint32_t *freq /* nblocks x 320 */)
+// literal/length and distance histogram of syms[begin, begin + count) into fb (kLCodes + kDCodes words); one CTA
+__device__ __forceinline__ void block_hist_body(const Sym *syms, uint32_t begin, uint32_t count, uint32_t *fb)
 {
     __shared__ uint32_t lf[kLCodes], df[kDCodes];
-    const uint32_t b = blockIdx.x;
-    const uint32_t nsyms = jb.info->n_syms, nblocks = jb.info->n_blocks;
     for (uint32_t i = threadIdx.x; i < kLCodes; i += blockDim.x) lf[i] = 0;
     if (threadIdx.x < kDCodes) df[threadIdx.x] = 0;
     __syncthreads();
-    const uint32_t begin = b * jb.block_syms;
-    const uint32_t count = (b + 1 < nblocks) ? jb.block_syms : nsyms - begin;
     for (uint32_t i = threadIdx.x; i < count; i += blockDim.x) {
-        const Sym s = jb.syms[begin + i];
+        const Sym s = syms[begin + i];
         if (s.dist == 0) atomicAdd(&lf[s.lc], 1u);
         else {
             atomicAdd(&lf[257 + c_tab.length_code[s.lc]], 1u);
@@ -1334,8 +1331,17 @@ __global__ void __launch_bounds__(256) k_block_hist(JobBufs jb, uint32_t *freq /
         }
     }
     __syncthreads();
-    for (uint32_t i = threadIdx.x; i < kLCodes; i += blockDim.x) freq[b * 320 + i] = lf[i];
-    if (threadIdx.x < kDCodes) freq[b * 320 + kLCodes + threadIdx.x] = df[threadIdx.x];
+    for (uint32_t i = threadIdx.x; i < kLCodes; i += blockDim.x) fb[i] = lf[i];
+    if (threadIdx.x < kDCodes) fb[kLCodes + threadIdx.x] = df[threadIdx.x];
+}
+
+__global__ void __launch_bounds__(256) k_block_hist(JobBufs jb, uint32_t *freq /* nblocks x 320 */)
+{
+    const uint32_t b = blockIdx.x;
+    const uint32_t nsyms = jb.info->n_syms, nblocks = jb.info->n_blocks;
+    const uint32_t begin = b * jb.block_syms;
+    const uint32_t count = (b + 1 < nblocks) ? jb.block_syms : nsyms - begin;
+    block_hist_body(jb.syms, begin, count, freq + b * 320);
     if (threadIdx.x == 0) {
         BlockDesc &bd = jb.blocks[b];
         const bool last = b + 1 == nblocks;
@@ -1639,25 +1645,33 @@ __device__ void build_block_warp(TreeScratch &s, BlockDesc &b, const uint32_t *l
     __syncwarp();
 }
 
-__global__ void __launch_bounds__(32) k_build_blocks(JobBufs jb, const uint32_t *freq)
+// Trees and header of block gbd from its histogram fb, one warp: deflate_quick's static pieces (quick) or zng_tr_flush_block.
+__device__ __forceinline__ void build_blocks_body(BlockDesc *gbd, const uint32_t *fb, bool quick, bool first, bool last_piece,
+                                                  bool final_block, bool strategy_fixed)
 {
     __shared__ TreeScratch s;
     __shared__ BlockDesc bd;
     __shared__ uint32_t fr[320];
     __shared__ uint32_t sh_cnt[16];
     __shared__ TreeState sh_st;
+    for (uint32_t i = threadIdx.x; i < 320; i += 32) fr[i] = fb[i];
+    for (uint32_t i = threadIdx.x; i < sizeof(BlockDesc) / 4; i += 32)
+        reinterpret_cast<uint32_t *>(&bd)[i] = reinterpret_cast<const uint32_t *>(gbd)[i];
+    __syncwarp();
+    if (quick) {
+        if (threadIdx.x == 0) build_quick_piece(c_tab, bd, fr, fr + kLCodes, first, last_piece, final_block);
+    } else build_block_warp(s, bd, fr, fr + kLCodes, bd.have_window != 0, strategy_fixed, sh_cnt, &sh_st);
+    __syncwarp();
+    for (uint32_t i = threadIdx.x; i < sizeof(BlockDesc) / 4; i += 32)
+        reinterpret_cast<uint32_t *>(gbd)[i] = reinterpret_cast<const uint32_t *>(&bd)[i];
+}
+
+__global__ void __launch_bounds__(32) k_build_blocks(JobBufs jb, const uint32_t *freq)
+{
     const uint32_t b = blockIdx.x;
     if (b >= jb.info->n_blocks) return;
-    for (uint32_t i = threadIdx.x; i < 320; i += 32) fr[i] = freq[b * 320 + i];
-    for (uint32_t i = threadIdx.x; i < sizeof(BlockDesc) / 4; i += 32)
-        reinterpret_cast<uint32_t *>(&bd)[i] = reinterpret_cast<const uint32_t *>(&jb.blocks[b])[i];
-    __syncwarp();
-    if (jb.serial_mode == 1) {
-        if (threadIdx.x == 0) build_quick_piece(c_tab, bd, fr, fr + kLCodes, b == 0, b + 1 == jb.info->n_blocks, jb.not_last == 0);
-    } else build_block_warp(s, bd, fr, fr + kLCodes, bd.have_window != 0, jb.strategy_fixed != 0, sh_cnt, &sh_st);
-    __syncwarp();
-    for (uint32_t i = threadIdx.x; i < sizeof(BlockDesc) / 4; i += 32)
-        reinterpret_cast<uint32_t *>(&jb.blocks[b])[i] = reinterpret_cast<const uint32_t *>(&bd)[i];
+    build_blocks_body(&jb.blocks[b], freq + b * 320, jb.serial_mode == 1, b == 0, b + 1 == jb.info->n_blocks, jb.not_last == 0,
+                      jb.strategy_fixed != 0);
 }
 
 // OR `n` (<= 57) bits of `val` into the output at bit position `pos`.  The output was zeroed.
@@ -1734,15 +1748,15 @@ __global__ void __launch_bounds__(256) k_scan_blocks(JobBufs jb)
     }
 }
 
-__global__ void __launch_bounds__(1024) k_encode(JobBufs jb)
+// Bit packing of one block at bd.bit_base of the zeroed output, one CTA of 1024 threads; a body of other than body_bits bits sets
+// error bit 16.
+__device__ __forceinline__ void encode_body(const BlockDesc &bd, const Sym *syms, const uint8_t *in, uint8_t *out, uint32_t *error)
 {
     __shared__ HuffTables st;
     __shared__ uint16_t s_lcode[kLCodes], s_dcode[kDCodes];
     __shared__ uint8_t s_llen[kLCodes], s_dlen[kDCodes];
     __shared__ uint64_t warp_sum[32];
-    if (jb.info->error) return;
-    const BlockDesc &bd = jb.blocks[blockIdx.x];
-    uint32_t *out32 = reinterpret_cast<uint32_t *>(jb.out);
+    uint32_t *out32 = reinterpret_cast<uint32_t *>(out);
     const uint32_t tid = threadIdx.x;
     if (bd.type == 0) {
         // stored block (deflate.rs:1734-1763)
@@ -1750,12 +1764,12 @@ __global__ void __launch_bounds__(1024) k_encode(JobBufs jb)
         const uint32_t sl = (uint16_t)bd.in_len;
         if (tid == 0) {
             or_bits(out32, bd.bit_base, bd.hdr[0] & 7u, 3);
-            jb.out[p] = (uint8_t)sl;
-            jb.out[p + 1] = (uint8_t)(sl >> 8);
-            jb.out[p + 2] = (uint8_t)~sl;
-            jb.out[p + 3] = (uint8_t)((~sl) >> 8);
+            out[p] = (uint8_t)sl;
+            out[p + 1] = (uint8_t)(sl >> 8);
+            out[p + 2] = (uint8_t)~sl;
+            out[p + 3] = (uint8_t)((~sl) >> 8);
         }
-        for (uint32_t i = tid; i < sl; i += blockDim.x) jb.out[p + 4 + i] = jb.in[bd.in_start + i];
+        for (uint32_t i = tid; i < sl; i += blockDim.x) out[p + 4 + i] = in[bd.in_start + i];
         return;
     }
     for (uint32_t i = tid; i < sizeof(HuffTables) / 4; i += blockDim.x)
@@ -1786,7 +1800,7 @@ __global__ void __launch_bounds__(1024) k_encode(JobBufs jb)
             uint64_t v = 0;
             uint32_t n = 0;
             if (i < bd.sym_count) {
-                const Sym s = jb.syms[bd.sym_begin + i];
+                const Sym s = syms[bd.sym_begin + i];
                 if (s.dist == 0) { v = s_lcode[s.lc]; n = s_llen[s.lc]; }
                 else {
                     uint32_t code = st.length_code[s.lc];
@@ -1836,7 +1850,62 @@ __global__ void __launch_bounds__(1024) k_encode(JobBufs jb)
         round_bits += warp_sum[31];
         __syncthreads(); // warp_sum is rewritten by the next round
     }
-    if (tid == blockDim.x - 1 && round_bits != bd.body_bits) atomicOr(&jb.info->error, 16u);
+    if (tid == blockDim.x - 1 && round_bits != bd.body_bits) atomicOr(error, 16u);
+}
+
+__global__ void __launch_bounds__(1024) k_encode(JobBufs jb)
+{
+    if (jb.info->error) return;
+    encode_body(jb.blocks[blockIdx.x], jb.syms, jb.in, jb.out, &jb.info->error);
+}
+
+// ------------------------------------------------------------------------------------------------
+// BGZF members (zb_bgzf.h, zb_bgzf.cu): the block kernels above over every member at once, one CTA per block slot
+// m * kBgzfMaxBlocks + k.  Positions and symbols are member-relative; in_start and sym_begin point into the staged buffers.
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) k_bgzf_hist(JobBufs jb, BgzfJob bj, uint32_t *freq)
+{
+    const uint32_t b = blockIdx.x, m = b / kBgzfMaxBlocks, k = b % kBgzfMaxBlocks;
+    const JobInfo &mi = bj.minfo[m];
+    const uint32_t nsyms = mi.n_syms, nblocks = mi.n_blocks;
+    if (k >= nblocks) return;
+    const uint32_t base = m * kBgzfStride, len = bj.mlen[m];
+    const Sym *syms = jb.syms + base;
+    const uint32_t begin = k * jb.block_syms;
+    const uint32_t count = k + 1 < nblocks ? jb.block_syms : nsyms - begin;
+    block_hist_body(syms, begin, count, freq + (size_t)b * 320);
+    if (threadIdx.x == 0) {
+        BlockDesc &bd = jb.blocks[b];
+        const bool last = k + 1 == nblocks;
+        bd.sym_begin = base + begin;
+        bd.sym_count = count;
+        bd.last = last;
+        const uint32_t start = begin == 0 ? 0 : sym_end(syms[begin - 1]);
+        const uint32_t end = last ? len : sym_end(syms[begin + count - 1]);
+        bd.in_start = base + start;
+        bd.in_len = end - start;
+        uint32_t Bf;
+        if (last) Bf = mi.final_base;
+        else if (jb.slow_mode) Bf = base_at(syms[begin + count - 1].pos + 1, len, jb.wsize); // as k_block_hist
+        else Bf = jb.block_base[b]; // recorded by the parse at the flush (unused by deflate_quick's pieces)
+        bd.have_window = start >= Bf;
+    }
+}
+
+__global__ void __launch_bounds__(32) k_bgzf_build(JobBufs jb, BgzfJob bj, const uint32_t *freq)
+{
+    const uint32_t b = blockIdx.x, m = b / kBgzfMaxBlocks, k = b % kBgzfMaxBlocks;
+    const uint32_t nblocks = bj.minfo[m].n_blocks;
+    if (k >= nblocks) return;
+    build_blocks_body(&jb.blocks[b], freq + (size_t)b * 320, jb.serial_mode == 1, k == 0, k + 1 == nblocks, true, false);
+}
+
+// bit_base is absolute here (k_bgzf_scan); a member written stored has no blocks to encode
+__global__ void __launch_bounds__(1024) k_bgzf_encode(JobBufs jb, BgzfJob bj)
+{
+    const uint32_t b = blockIdx.x, m = b / kBgzfMaxBlocks, k = b % kBgzfMaxBlocks;
+    if (bj.ctl->error || k >= bj.minfo[m].n_blocks || bj.mstored[m]) return;
+    encode_body(jb.blocks[b], jb.syms, jb.in, jb.out, &bj.ctl->error);
 }
 
 __global__ void k_finish(JobBufs jb, const uint32_t *check)

@@ -6,6 +6,7 @@
 #include "zb_core.h"
 #include "zb_huff.h"
 #include "zb_slow.h"
+#include "zb_bgzf.h"
 
 namespace zb {
 
@@ -112,6 +113,30 @@ struct JobBufs {
     uint32_t *block_base;     // serial levels: window base in force when block b was flushed
     uint32_t wsize;           // window size of the serial small-window path (k_tail over the whole input), kWSize otherwise
     uint32_t cinfo;           // zlib header CINFO = windowBits - 8 (7 unless the whole input fits a smaller window's match range)
+};
+
+// One BGZF call (ZB_FLAG_BGZF, zb_bgzf.h): member m is staged at m * kBgzfStride of JobBufs::in, its symbols start at
+// syms[m * kBgzfStride], its deflate blocks are blocks[m * kBgzfMaxBlocks + k] and the window bases of their flushes
+// block_base[m * kBgzfMaxBlocks + k].
+struct BgzfCtl {
+    uint32_t count;     // members (k_crc_join)
+    uint32_t error;     // non-zero: internal invariant violated
+    uint32_t n_blocks;  // deflate blocks of the file
+    uint32_t n_syms;    // symbols of the compressed members
+    uint32_t data_type; // of the first block, as a single-stream job reports it
+    uint32_t pad;
+    uint64_t out_bytes; // file length
+};
+struct BgzfJob {
+    uint32_t nm;        // members
+    uint64_t *moff;     // staged offset of member m
+    uint32_t *mlen;     // its input bytes
+    uint32_t *mcrc;     // its crc32
+    uint32_t *mbytes;   // its length in the file
+    uint64_t *mout;     // its offset in the file
+    uint32_t *mstored;  // 1: written as one stored block (level 0, or the payload does not fit 64 KiB)
+    JobInfo *minfo;     // n_syms, n_blocks and final_base of its parse, as a single-stream parse reports them
+    BgzfCtl *ctl;
 };
 
 cudaError_t upload_tables();

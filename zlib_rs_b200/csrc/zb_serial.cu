@@ -94,4 +94,20 @@ __global__ void __launch_bounds__(32) k_serial_low(JobBufs jb)
     else serial_low_body<kRingFast, true>(jb, smem);
 }
 
+// BGZF (zb_bgzf.h): one CTA per member, each parsing its block alone as k_serial_low parses a stream.  At level 1 the 64 KiB ring
+// holds the whole member.
+__global__ void __launch_bounds__(32) k_serial_low_members(JobBufs jb, BgzfJob bj)
+{
+    extern __shared__ __align__(16) uint8_t smem[];
+    const uint32_t m = blockIdx.x, base = m * kBgzfStride;
+    JobBufs mj = jb;
+    mj.in = jb.in + base;
+    mj.N = bj.mlen[m];
+    mj.syms = jb.syms + base;
+    mj.block_base = jb.block_base + m * kBgzfMaxBlocks;
+    mj.info = bj.minfo + m;
+    if (jb.serial_mode == 1) serial_low_body<kRingQuick, false>(mj, smem);
+    else serial_low_body<kRingFast, true>(mj, smem);
+}
+
 } // namespace zb

@@ -28,11 +28,6 @@ struct SlowSAcc {
     __device__ __forceinline__ uint32_t link(uint32_t y) const { return y + need <= N ? sL[y - ws] : 0; }
 };
 
-__device__ __forceinline__ uint32_t pack_step(const SlowStep &s)
-{
-    return (s.nlit << 24) | (s.len ? ((s.len - 3u) << 16) | 0x8000u | (s.dist - 1u) : 0u);
-}
-
 constexpr uint32_t kSlowSafe = 1024; // nodes this close to the end of the input take the generic slow_step()
 constexpr uint32_t kSlowBatch = 8;
 constexpr uint32_t kCoopStart = 16; // prev_length from which the warp shares a lane's re-rooting scan (level 9)

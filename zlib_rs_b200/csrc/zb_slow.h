@@ -177,6 +177,12 @@ struct SlowStep {
     uint32_t dist;
 };
 
+// A macro step as the kernels store it: literal count << 24 | (len - 3) << 16 | 0x8000 | (dist - 1) (no match: the count alone)
+ZB_HD uint32_t pack_step(const SlowStep &s)
+{
+    return (s.nlit << 24) | (s.len ? ((s.len - 3u) << 16) | 0x8000u | (s.dist - 1u) : 0u);
+}
+
 // Search at loop-top q with prev_length pl (slow.rs:56-82).  Returns the new match_len (2 = none) and start.
 template <class A>
 ZB_HD Match slow_search(const A &a, uint32_t q, uint32_t pl, uint32_t ms, uint32_t B, uint32_t N, const SlowParams &sp)
