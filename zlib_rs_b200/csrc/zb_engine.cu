@@ -411,7 +411,9 @@ int Engine::deflate(const void *src, size_t n_in, bool src_dev, void *dst, size_
                                 !jb.serial_mode && jb.slow_mode != 2;
     if (chunked_upload) {
         // a chunk is at least one wave of the link kernel (one CTA per tile and SM): smaller launches only add CTA latencies
-        size_t chunk = (n_in / kUpChunks + kLinkTile - 1) / kLinkTile * kLinkTile;
+        // (ceil(n_in / kUpChunks), not the floor: with the floor a whole number of tiles per chunk and a remainder of 1..7 bytes made a
+        // ninth chunk, one past evc[] and up_len[])
+        size_t chunk = ((n_in + kUpChunks - 1) / kUpChunks + kLinkTile - 1) / kLinkTile * kLinkTile;
         if (chunk < (size_t)device_sm_count() * kLinkTile) chunk = (size_t)device_sm_count() * kLinkTile;
         CK(cudaStreamWaitEvent(st2, ev0, 0));
         for (size_t off = 0; off < n_in; off += chunk) {
@@ -596,9 +598,9 @@ int Engine::deflate(const void *src, size_t n_in, bool src_dev, void *dst, size_
                         static unsigned long long last[3];
                         if (iters == 1) memset(last, 0, sizeof last);
                         const double ctas = (double)(h_info->dbg[0] - last[0]) + 1e-9;
-                        fprintf(stderr, "iter %u dirty %u: ctas %llu stage %.1f walk %.1f kcyc/cta, holes_changed %u\n", iters, n_dirty,
-                                h_info->dbg[0] - last[0], (h_info->dbg[1] - last[1]) / 1e3 / ctas, (h_info->dbg[2] - last[2]) / 1e3 / ctas,
-                                h_info->holes_changed);
+                        fprintf(stderr, "iter %u dirty %u: ctas %llu stage %.1f walk %.1f kcyc/cta, holes_changed %u, sub %u first_tile %u chain %u\n",
+                                iters, n_dirty, h_info->dbg[0] - last[0], (h_info->dbg[1] - last[1]) / 1e3 / ctas,
+                                (h_info->dbg[2] - last[2]) / 1e3 / ctas, h_info->holes_changed, jb.match_sub, first_ptile, chain2 ? 2u : 1u);
                         memcpy(last, h_info->dbg, sizeof last);
                     }
                     if (!h_info->holes_changed) break;
