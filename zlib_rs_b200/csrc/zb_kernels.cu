@@ -1935,12 +1935,19 @@ __global__ void __launch_bounds__(256) k_literal_syms(JobBufs jb)
     if (p == 0) {
         jb.info->n_mid_syms = n;
         jb.info->n_syms = n;
-        jb.info->n_blocks = n / jb.block_syms + 1;
+        // Z_FINISH always flushes a last block, empty or not; a segment (Z_SYNC_FLUSH) flushes only pending symbols
+        // (huff.rs:36-45).  So a segment whose symbols fill its last block exactly ends with that block, which the loop flushed
+        // when it filled up.  An empty segment is the exception here: the engine plans at least one block for every job, so it
+        // writes an empty static block before the marker where the reference writes the marker alone.
+        const bool full_last = jb.not_last && n && n % jb.block_syms == 0;
+        jb.info->n_blocks = n / jb.block_syms + (full_last ? 0 : 1);
         // deflate_huff refills only when lookahead == 0: the base moves when strstart reaches 2w + k*w; the last fill_window call
-        // (strstart == N) still slides when strstart >= w_size + max_dist (deflate.rs:1787)
+        // (strstart == N) still slides when strstart >= w_size + max_dist (deflate.rs:1787).  That call comes after the flush of
+        // a block the loop filled, so such a last block keeps the base its own last symbol saw (as k_block_hist gives a block
+        // that is not the last one).
         const uint32_t w = jb.wsize, q = jb.N ? jb.N - 1 : 0;
         uint32_t B = q < 2 * w ? 0 : w * (1 + (q - 2 * w) / w);
-        if (jb.N - B >= 2 * w - kMinLookahead) B += w;
+        if (!full_last && jb.N - B >= 2 * w - kMinLookahead) B += w;
         jb.info->final_base = B;
     }
     if (p < n) jb.syms[p] = Sym{0, jb.in[jb.start + p], jb.start + p};
