@@ -7,47 +7,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 import oracle_lib as O
 import test_hostmodel as T
+from parser_inputs import fuzz_case as gen  # the structured classes the GPU fuzzer draws from too
 
 H = T.H()
-
-
-def gen(rng):
-    kind = int(rng.integers(0, 8))
-    n = int(rng.choice([0, 1, 2, 3, 5, 17, 261, 262, 263, 300, 1000, 4000, 16383, 16384, 33000, 65535, 65536, 66000, 70000, 131072, 200000]))
-    n = max(0, n + int(rng.integers(-3, 4))) if n > 3 else n
-    if kind == 0:
-        return rng.integers(0, 256, n, dtype=np.uint8).tobytes()
-    if kind == 1:
-        return rng.integers(0, int(rng.integers(1, 5)), n, dtype=np.uint8).tobytes()
-    if kind == 2:  # periodic with mutations
-        per = rng.integers(0, 256, int(rng.integers(1, 600)), dtype=np.uint8).tobytes()
-        b = bytearray((per * (n // len(per) + 1))[:n])
-        for _ in range(int(rng.integers(0, 40))):
-            if n:
-                b[int(rng.integers(0, n))] = int(rng.integers(0, 256))
-        return bytes(b)
-    if kind == 3:  # runs
-        out = bytearray()
-        while len(out) < n:
-            out += bytes([int(rng.integers(0, 256))]) * int(rng.integers(1, 900))
-        return bytes(out[:n])
-    if kind == 4:  # words
-        words = [bytes(rng.integers(97, 123, size=int(rng.integers(1, 12)), dtype=np.uint8)) for _ in range(int(rng.integers(2, 300)))]
-        out = bytearray()
-        while len(out) < n:
-            out += words[int(rng.integers(0, len(words)))] + b" "
-        return bytes(out[:n])
-    if kind == 5:  # long repeats at a distance near the window edges
-        blk = rng.integers(0, 256, int(rng.integers(300, 3000)), dtype=np.uint8).tobytes()
-        gap = int(rng.choice([32000, 32506 - len(blk) % 7, 32768, 65274, 100]))
-        out = bytearray()
-        while len(out) < n:
-            out += blk + rng.integers(0, 256, max(0, gap - len(blk)), dtype=np.uint8).tobytes()
-        return bytes(out[:n])
-    if kind == 6:
-        return bytes(n)
-    a = gen(rng)
-    return (a + gen(rng))[:max(n, 1)]
 
 
 def deflate_main(d, level):
