@@ -103,6 +103,26 @@ ZB_API int zb_deflate_dict(zb_engine *e, const void *dict, size_t dict_len, cons
 ZB_API size_t zb_deflate_bound(size_t src_len);
 ZB_API size_t zb_bgzf_bound(size_t src_len); /* ceil(src_len / 65280) * 65536 + 28: the largest ZB_FLAG_BGZF file */
 
+/* Batches of independent streams (DESIGN.md §2i): many small buffers (database or Parquet pages, messages, 64 KiB chunks of a file)
+ * in one call each way, with a fixed number of kernel launches and host syncs whatever the number and lengths of the items.
+ *
+ * zb_deflate_batch: item i is src[src_off[i], src_off[i+1]) (src_off: a host array of n_items + 1 offsets into src, which is a host
+ * or, with src_on_device, a device pointer).  Its stream is dst[dst_off[i], dst_off[i+1]), byte for byte what
+ * zb_deflate(item_i, level, strategy, window_bits) returns -- for window_bits 15 that is compress2(item_i, level).  The streams are
+ * packed back to back in input order from dst[0]; dst_off (host, n_items + 1 entries) is filled.  checks[i] (host, n_items entries,
+ * or NULL) is what res->check of that single call would be: adler32 (zlib), crc32 (gzip), 0 (raw).  res carries the totals:
+ * out_bytes = dst_off[n_items], n_blocks, n_symbols, gpu_launches, gpu_ms, exact_parity = 1.
+ * Accepted: window_bits 15 (zlib), -15 (raw) or 31 (gzip: MTIME 0, XFL by level, OS 3); Z_DEFAULT_STRATEGY; level -1..9; flags 0 or
+ * ZB_FLAG_MEMLEVEL(8).  Each item at most 65536 bytes, at most 65535 items, at most 2^31 bytes in all.  Anything else gives
+ * ZB_E_PARAM with a zb_last_error() text.  An empty batch and empty items are valid (an empty item is the reference's empty stream).
+ * dst_cap below the total gives ZB_E_BUF with res->out_bytes set to the size needed; zb_deflate_batch_bound is always enough.
+ * Items are compressed side by side, one item per warp or thread, through the kernels of ZB_FLAG_BGZF: a batch of a few large items
+ * at levels 3..6 can be slower than zb_deflate on each of them (DESIGN.md §2i). */
+ZB_API int zb_deflate_batch(zb_engine *e, const void *src, const uint64_t *src_off, size_t n_items, int src_on_device, void *dst,
+                            size_t dst_cap, int dst_on_device, int level, int strategy, int window_bits, uint32_t flags, uint64_t *dst_off,
+                            uint32_t *checks, zb_deflate_result *res);
+ZB_API size_t zb_deflate_batch_bound(const uint64_t *src_off, size_t n_items); /* sum of zb_deflate_bound(len_i) */
+
 typedef struct zb_inflate_result {
     uint64_t out_bytes;
     uint64_t in_bytes;   /* compressed bytes consumed */
@@ -135,6 +155,17 @@ ZB_API int zb_inflate(zb_engine *e, const void *src, size_t src_len, int src_on_
                                  their BSIZE and ISIZE fields are only hints, which decide the speed but never the result. */
 ZB_API int zb_inflate_ex(zb_engine *e, const void *src, size_t src_len, int src_on_device, void *dst, size_t dst_cap, int dst_on_device,
                          int window_bits, uint32_t flags, zb_inflate_result *res);
+/* zb_inflate_batch: item i of src[src_off[i], src_off[i+1]) decodes into its own slot dst[dst_off[i], dst_off[i+1]) (both offset
+ * tables on the host, n_items + 1 entries; src and dst host pointers or, with *_on_device, device pointers).  window_bits is any
+ * value zb_inflate_ex accepts, +32 auto-detection included, and applies to every item.  items[i] gets the status, msg, out_bytes,
+ * in_bytes and check that zb_inflate_ex gives for that item alone with dst_cap set to its slot's length: corrupt or truncated
+ * items, a slot too small (ZB_E_BUF), an FDICT header ("need dictionary") and trailing bytes behind a stream (not consumed) behave
+ * as they do there, and one bad item never changes another item's result.  With a host dst every slot is written whole: behind
+ * an item's output it holds zeros.  Returns ZB_OK when every item is OK, else the status of the first item that failed; every
+ * entry of items is filled either way.  Item lengths are not limited, slots must be below 4 GiB, at most 2^20 items (else
+ * ZB_E_PARAM).  Each item is decoded by one warp: a single large stream decodes faster through zb_inflate_ex. */
+ZB_API int zb_inflate_batch(zb_engine *e, const void *src, const uint64_t *src_off, size_t n_items, int src_on_device, void *dst,
+                            const uint64_t *dst_off, int dst_on_device, int window_bits, zb_inflate_result *items);
 
 /* Streaming building block (what inflate() of the zlib ABI runs on, zlib-rs/src/inflate.rs:2376-2457): decode the COMPLETE deflate
  * blocks of a raw deflate segment.  src/dict/dst are host buffers; decoding starts at bit `start_bit` of src with the last

@@ -133,6 +133,12 @@ def lib():
         L.zb_bgzf_bound.argtypes, L.zb_bgzf_bound.restype = [sz], sz
         L.zb_inflate.argtypes = [vp, vp, sz, ci, vp, sz, ci, ci, ctypes.POINTER(InflateResult)]
         L.zb_inflate_ex.argtypes = [vp, vp, sz, ci, vp, sz, ci, ci, u32, ctypes.POINTER(InflateResult)]
+        if hasattr(L, "zb_deflate_batch"):  # builds before the batch calls (ZB_LIB_PATH baselines of scripts/gpu_ab.sh) lack them
+            u64p = ctypes.POINTER(u64)
+            L.zb_deflate_batch.argtypes = [vp, vp, u64p, sz, ci, vp, sz, ci, ci, ci, ci, u32, u64p, ctypes.POINTER(u32),
+                                           ctypes.POINTER(DeflateResult)]
+            L.zb_deflate_batch_bound.argtypes, L.zb_deflate_batch_bound.restype = [u64p, sz], sz
+            L.zb_inflate_batch.argtypes = [vp, vp, u64p, sz, ci, vp, u64p, ci, ci, ctypes.POINTER(InflateResult)]
         L.zb_adler32.argtypes = [vp, u32, vp, sz, ci, ctypes.POINTER(u32), ctypes.POINTER(ctypes.c_float)]
         L.zb_crc32.argtypes = [vp, u32, vp, sz, ci, ctypes.POINTER(u32), ctypes.POINTER(ctypes.c_float)]
         L.zb_engine_set_profile.argtypes = [vp, ci]
@@ -160,6 +166,29 @@ def _buf(data):
 def bgzf_bound(n):
     """Largest file Engine.deflate(..., window_bits=31, flags=ZB_FLAG_BGZF) writes for n input bytes: ceil(n / 65280) * 65536 + 28."""
     return lib().zb_bgzf_bound(n)
+
+
+def _offsets(lengths):
+    off = (ctypes.c_uint64 * (len(lengths) + 1))()
+    t = 0
+    for i, n in enumerate(lengths):
+        off[i] = t
+        t += n
+    off[len(lengths)] = t
+    return off
+
+
+def _gather(items):
+    """A list of bytes-like items as one host buffer and its offset table."""
+    items = [bytes(x) for x in items]
+    data = b"".join(items)
+    return (ctypes.c_char * max(len(data), 1)).from_buffer_copy(data or b"\0"), _offsets([len(x) for x in items])
+
+
+def deflate_batch_bound(lengths):
+    """Largest output Engine.deflate_batch writes for items of these lengths: the sum of their zb_deflate_bound."""
+    off = _offsets(list(lengths))
+    return lib().zb_deflate_batch_bound(off, len(off) - 1)
 
 
 def compressBound(n):
@@ -392,6 +421,73 @@ class Engine:
         rc = lib().zb_inflate_ex(self.h, src, n, int(src_on_device), dst, out_cap, int(dst_on_device), window_bits, flags,
                                  ctypes.byref(res))
         return rc, (own.raw[: res.out_bytes] if own is not None else None), res
+
+    def deflate_batch(self, items, level=-1, window_bits=15, strategy=0, mem_level=8, flags=0, src_on_device=False, src_off=None,
+                      dst=None, dst_cap=0, dst_on_device=False):
+        """Deflate every item as its own stream in one call (zb_deflate_batch): item i's stream is byte for byte what
+        Engine.deflate gives for it alone.  Host `items`: a list of bytes-like objects; device `items`: a pointer, with `src_off`
+        (n + 1 offsets into it).  Returns (list of bytes or None, offsets (n + 1), checks, DeflateResult); with a caller's `dst`
+        the streams are packed back to back there and the first element is None.  Raises ZlibError (.needed: the size a too
+        small dst_cap would have to be)."""
+        res = DeflateResult()
+        flags |= (mem_level & 15) << 8
+        keep = None
+        if src_on_device:
+            off = (ctypes.c_uint64 * len(src_off))(*src_off)
+            src = items
+        else:
+            keep, off = _gather(items)
+            src = ctypes.addressof(keep)
+        n = len(off) - 1
+        own = None
+        if dst is None:
+            dst_cap = lib().zb_deflate_batch_bound(off, n) + 64
+            own = ctypes.create_string_buffer(dst_cap)
+            dst = ctypes.addressof(own)
+            dst_on_device = False
+        dst_off = (ctypes.c_uint64 * (n + 1))()
+        checks = (ctypes.c_uint32 * max(n, 1))()
+        rc = lib().zb_deflate_batch(self.h, src, off, n, int(src_on_device), dst, dst_cap, int(dst_on_device), level, strategy,
+                                    window_bits, flags, dst_off, checks, ctypes.byref(res))
+        if rc != 0:
+            e = ZlibError(rc, lib().zb_last_error().decode())
+            e.needed = res.out_bytes
+            raise e
+        offs = list(dst_off)
+        raw = own.raw if own is not None else None
+        outs = [raw[offs[i]:offs[i + 1]] for i in range(n)] if own is not None else None
+        return outs, offs, list(checks)[:n], res
+
+    def inflate_batch(self, items, out_caps, window_bits=15, src_on_device=False, src_off=None, dst=None, dst_off=None,
+                      dst_on_device=False):
+        """Inflate every item into its own slot in one call (zb_inflate_batch).  Host `items`: a list of bytes-like objects and
+        `out_caps` the slot length of each; device `items`: a pointer with `src_off`.  A caller's `dst` takes `dst_off` (n + 1
+        offsets) instead of out_caps.  Returns (rc, list of bytes or None, list of InflateResult): each result is what
+        Engine.inflate gives for that item alone."""
+        keep = None
+        if src_on_device:
+            off = (ctypes.c_uint64 * len(src_off))(*src_off)
+            src = items
+        else:
+            keep, off = _gather(items)
+            src = ctypes.addressof(keep)
+        n = len(off) - 1
+        own = None
+        if dst is None:
+            doff = _offsets(list(out_caps))
+            own = ctypes.create_string_buffer(max(doff[n], 1))
+            dst = ctypes.addressof(own)
+            dst_on_device = False
+        else:
+            doff = (ctypes.c_uint64 * len(dst_off))(*dst_off)
+        res = (InflateResult * max(n, 1))()
+        rc = lib().zb_inflate_batch(self.h, src, off, n, int(src_on_device), dst, doff, int(dst_on_device), window_bits, res)
+        results = list(res)[:n]
+        outs = None
+        if own is not None:
+            raw = own.raw
+            outs = [raw[doff[i]:doff[i] + results[i].out_bytes] for i in range(n)]
+        return rc, outs, results
 
     def adler32(self, buf, n=None, start=1, on_device=False):
         out, ms = ctypes.c_uint32(0), ctypes.c_float(0)

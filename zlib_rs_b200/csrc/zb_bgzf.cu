@@ -1,7 +1,8 @@
-// zb_bgzf.cu -- BGZF writing (ZB_FLAG_BGZF, zb_bgzf.h, DESIGN.md §2h): the member parsers of levels 3..9, the member sizes and
-// offsets, and the framing.  Every kernel covers all members of the call, so a call costs the same launches whatever its length.
-// Levels 1/2 parse in k_serial_low_members (zb_serial.cu); the block kernels k_bgzf_hist / k_bgzf_build / k_bgzf_encode share their
-// bodies with the single-stream ones (zb_kernels.cu).
+// zb_bgzf.cu -- member writing (zb_bgzf.h): BGZF files (ZB_FLAG_BGZF, DESIGN.md §2h) and batches of streams (zb_deflate_batch,
+// DESIGN.md §2i).  The batch staging, the member parsers of levels 3..9, the member sizes and offsets, and the framing.  Every kernel
+// covers all members of the call, so a call costs the same launches whatever its length.  Levels 1/2 parse in k_serial_low_members
+// (zb_serial.cu); the block kernels k_bgzf_hist / k_bgzf_build / k_bgzf_encode share their bodies with the single-stream ones
+// (zb_kernels.cu).
 #include "zb_kernels.cuh"
 
 namespace zb {
@@ -15,13 +16,26 @@ __global__ void __launch_bounds__(256) k_bgzf_setup(BgzfJob bj, uint64_t n)
     bj.mlen[m] = bgzf_member_len(n, m);
 }
 
+// Batch staging: item m of the contiguous source `src` (item m at src[soff[m] - soff[0]], the member table filled by the host) goes
+// to its staged offset, and the gap behind it up to the next item's offset (or `span`) is zeroed.  One CTA per item.
+__global__ void __launch_bounds__(256) k_batch_stage(const uint8_t *__restrict__ src, const uint64_t *__restrict__ soff, BgzfJob bj,
+                                                     uint8_t *__restrict__ in, uint64_t span)
+{
+    const uint32_t m = blockIdx.x;
+    const uint8_t *s = src + (soff[m] - soff[0]);
+    uint8_t *d = in + bj.moff[m];
+    const uint32_t len = bj.mlen[m];
+    const uint64_t end = (m + 1 < bj.nm ? bj.moff[m + 1] : span) - bj.moff[m];
+    for (uint32_t i = threadIdx.x; i < end; i += 256) d[i] = i < len ? s[i] : 0;
+}
+
 // Levels 3..6: lane 0 runs the exact serial simulator over the whole member, as k_tail does over a short stream.  There are no
 // holes to iterate on: the simulator keeps its own inserted-positions bitmap (in shared memory, one bit per position of a member).
 __global__ void __launch_bounds__(32) k_bgzf_medium(JobBufs jb, BgzfJob bj)
 {
-    __shared__ uint32_t ins[kBgzfBlock / 32];
+    __shared__ uint32_t ins[kMemberMax / 32];
     if (threadIdx.x != 0) return;
-    const uint32_t m = blockIdx.x, base = m * kBgzfStride, len = bj.mlen[m], bs = jb.block_syms;
+    const uint32_t m = blockIdx.x, base = (uint32_t)bj.moff[m], len = bj.mlen[m], bs = jb.block_syms;
     const BgzfAcc a{jb.in + base, jb.L + base, len, 4u};
     Sym *syms = jb.syms + base;
     uint32_t *bb = jb.block_base + m * kBgzfMaxBlocks;
@@ -30,7 +44,7 @@ __global__ void __launch_bounds__(32) k_bgzf_medium(JobBufs jb, BgzfJob bj)
         syms[k++] = s;
         if (--left == 0) { bb[blk++] = B; left = bs; } // the window base when this symbol fills the block (k_block_hist's sym_base)
     };
-    const uint32_t fb = serial_medium(a, len, 0, ins, kBgzfBlock / 32, jb.lp, emit);
+    const uint32_t fb = serial_medium(a, len, 0, ins, kMemberMax / 32, jb.lp, emit);
     JobInfo &mi = bj.minfo[m];
     mi.n_syms = k;
     mi.final_base = fb;
@@ -38,14 +52,15 @@ __global__ void __launch_bounds__(32) k_bgzf_medium(JobBufs jb, BgzfJob bj)
 }
 
 // Levels 7..9: deflate_slow has no holes, so the macro step from a fresh loop-top is a function of its position (zb_slow.h).  One
-// thread per staged position evaluates it through the member-relative accessor.
+// thread per position of a member evaluates it through the member-relative accessor: kMemberMax / 256 CTAs per member.
 __global__ void __launch_bounds__(256) k_bgzf_slow_steps(JobBufs jb, BgzfJob bj)
 {
-    const uint32_t x = blockIdx.x * 256 + threadIdx.x, m = x / kBgzfStride, y = x % kBgzfStride;
+    const uint32_t m = blockIdx.x / (kMemberMax / 256), y = (blockIdx.x % (kMemberMax / 256)) * 256 + threadIdx.x;
     if (m >= bj.nm) return;
     const uint32_t len = bj.mlen[m];
     if (y >= len) return;
-    const BgzfAcc a{jb.in + (x - y), jb.L + (x - y), len, jb.sp.slow ? 3u : 4u};
+    const uint32_t base = (uint32_t)bj.moff[m], x = base + y;
+    const BgzfAcc a{jb.in + base, jb.L + base, len, jb.sp.slow ? 3u : 4u};
     const SlowStep s = slow_step(a, y, len, jb.sp);
     jb.M[x] = pack_step(s);
     jb.nxt[x] = s.next;
@@ -56,7 +71,7 @@ __global__ void __launch_bounds__(32) k_bgzf_slow_walk(JobBufs jb, BgzfJob bj)
 {
     const uint32_t m = blockIdx.x * 32 + threadIdx.x;
     if (m >= bj.nm) return;
-    const uint32_t base = m * kBgzfStride, len = bj.mlen[m], bs = jb.block_syms;
+    const uint32_t base = (uint32_t)bj.moff[m], len = bj.mlen[m], bs = jb.block_syms;
     const uint8_t *d = jb.in + base;
     const uint32_t *M = jb.M + base, *nxt = jb.nxt + base;
     Sym *syms = jb.syms + base;
@@ -78,8 +93,9 @@ __global__ void __launch_bounds__(32) k_bgzf_slow_walk(JobBufs jb, BgzfJob bj)
     mi.n_blocks = nb;
 }
 
-// One thread per member: the payload's length from its blocks (stored blocks align to a byte, as in k_scan_blocks), the stored
-// fallback, the member's length in the file.  The blocks' bit positions are left relative to the payload.
+// One thread per member: the payload's length from its blocks (stored blocks align to a byte, as in k_scan_blocks), BGZF's stored
+// fallback, the member's length in the output.  The blocks' bit positions are left relative to the payload, which starts on a
+// byte whatever the framing, so the payload's bits do not depend on it.
 __global__ void __launch_bounds__(256) k_bgzf_size(JobBufs jb, BgzfJob bj)
 {
     const uint32_t m = blockIdx.x * 256 + threadIdx.x;
@@ -87,7 +103,7 @@ __global__ void __launch_bounds__(256) k_bgzf_size(JobBufs jb, BgzfJob bj)
     const uint32_t len = bj.mlen[m];
     bool stored = jb.level == 0;
     uint64_t payload = 0;
-    uint32_t nb = 1;
+    uint32_t nb = 0;
     if (!stored) {
         nb = bj.minfo[m].n_blocks;
         if (nb == 0 || nb > kBgzfMaxBlocks) { atomicOr(&bj.ctl->error, 1u); return; }
@@ -99,15 +115,16 @@ __global__ void __launch_bounds__(256) k_bgzf_size(JobBufs jb, BgzfJob bj)
         }
         payload = (bit + 7) >> 3;
         atomicAdd(&bj.ctl->n_syms, bj.minfo[m].n_syms);
-        if (bgzf_stored(payload)) { stored = true; nb = 1; }
+        if (bj.wrap == kWrapBgzf && bgzf_stored(payload)) stored = true;
     }
-    if (stored) payload = bgzf_stored_payload(len);
+    if (stored) { payload = stored_payload(len); nb = (uint32_t)stored_blocks(len); } // one block for a BGZF member
     atomicAdd(&bj.ctl->n_blocks, nb);
     bj.mstored[m] = stored;
-    bj.mbytes[m] = kBgzfHeader + (uint32_t)payload + kBgzfTrailer;
+    bj.mbytes[m] = member_header_len(bj.wrap) + (uint32_t)payload + member_trailer_len(bj.wrap);
 }
 
-// One CTA: the members' offsets in the file (exclusive scan of their lengths), the blocks' absolute bit positions, the file length.
+// One CTA: the members' offsets in the output (exclusive scan of their lengths), the blocks' absolute bit positions, the output
+// length.
 __global__ void __launch_bounds__(1024) k_bgzf_scan(JobBufs jb, BgzfJob bj)
 {
     __shared__ uint64_t part[1024];
@@ -125,39 +142,44 @@ __global__ void __launch_bounds__(1024) k_bgzf_scan(JobBufs jb, BgzfJob bj)
         __syncthreads();
     }
     uint64_t off = part[tid] - s;
+    const uint32_t hl = member_header_len(bj.wrap);
     for (uint32_t i = beg; i < end; i++) {
         bj.mout[i] = off;
         if (!bj.mstored[i]) {
             const uint32_t nb = bj.minfo[i].n_blocks;
-            for (uint32_t k = 0; k < nb; k++) jb.blocks[i * kBgzfMaxBlocks + k].bit_base += 8ull * (off + kBgzfHeader);
+            for (uint32_t k = 0; k < nb; k++) jb.blocks[i * kBgzfMaxBlocks + k].bit_base += 8ull * (off + hl);
         }
         off += bj.mbytes[i];
     }
-    if (tid == 1023) bj.ctl->out_bytes = part[1023] + kBgzfEofLen;
+    if (tid == 1023) bj.ctl->out_bytes = part[1023] + (bj.wrap == kWrapBgzf ? kBgzfEofLen : 0);
     if (tid == 0) bj.ctl->data_type = (n && !bj.mstored[0] && jb.blocks[0].sym_count) ? jb.blocks[0].data_type : 2u;
 }
 
-// One CTA per member: header with BSIZE, trailer, and the stored block of a member written stored; the last CTA writes the
-// end-of-file member.  Runs behind k_bgzf_encode (the payload bits are OR-ed into the zeroed output).
+// One CTA per member: header (BGZF's with BSIZE, or the item's zlib / gzip header), trailer, and the stored blocks of a member
+// written stored; with BGZF the last CTA writes the end-of-file member.  Runs behind k_bgzf_encode (the payload bits are OR-ed
+// into the zeroed output).
 __global__ void __launch_bounds__(256) k_bgzf_frame(JobBufs jb, BgzfJob bj)
 {
     const uint32_t m = blockIdx.x, tid = threadIdx.x;
     if (bj.ctl->error) return;
     if (m == bj.nm) {
-        if (tid < kBgzfEofLen) jb.out[bj.ctl->out_bytes - kBgzfEofLen + tid] = bgzf_eof(tid);
+        if (bj.wrap == kWrapBgzf && tid < kBgzfEofLen) jb.out[bj.ctl->out_bytes - kBgzfEofLen + tid] = bgzf_eof(tid);
         return;
     }
     uint8_t *o = jb.out + bj.mout[m];
-    const uint32_t len = bj.mlen[m], bytes = bj.mbytes[m];
+    const uint32_t len = bj.mlen[m], bytes = bj.mbytes[m], hl = member_header_len(bj.wrap);
     const bool stored = bj.mstored[m] != 0;
     if (tid == 0) {
-        bgzf_header(o, bytes);
-        bgzf_trailer(o + bytes - kBgzfTrailer, bj.mcrc[m], len);
-        if (stored) bgzf_stored_header(o + kBgzfHeader, len);
+        if (bj.wrap == kWrapBgzf) bgzf_header(o, bytes);
+        else stream_header(o, bj.wrap, zlib_level_flags(jb.level, false), 7, gzip_xfl((int)jb.level, 0));
+        const uint32_t tw = bj.wrap == kWrapBgzf ? 2u : bj.wrap; // BGZF's trailer is gzip's
+        stream_trailer(o + bytes - member_trailer_len(bj.wrap), tw, bj.mcheck[m], len);
     }
     if (stored) {
-        const uint8_t *src = jb.in + m * kBgzfStride;
-        for (uint32_t i = tid; i < len; i += 256) o[kBgzfHeader + 5 + i] = src[i];
+        const uint32_t nb = (uint32_t)stored_blocks(len);
+        if (tid < nb) stored_header(o + hl + tid * (kStoredMax + 5), min(kStoredMax, len - tid * kStoredMax), tid + 1 == nb);
+        const uint8_t *src = jb.in + bj.moff[m];
+        for (uint32_t i = tid; i < len; i += 256) o[hl + 5 * (i / kStoredMax + 1) + i] = src[i];
     }
 }
 

@@ -1,31 +1,57 @@
-// zb_bgzf.h -- the rules of BGZF writing (ZB_FLAG_BGZF in zb_engine.h, DESIGN.md §2h).
+// zb_bgzf.h -- the rules of member writing: BGZF files (ZB_FLAG_BGZF in zb_engine.h, DESIGN.md §2h) and batches of independent
+// streams (zb_deflate_batch, DESIGN.md §2i).  Both compress many members side by side through the same kernels (zb_bgzf.cu).
 //
-// Like zb_members.h this is `__host__ __device__`: the kernels of zb_bgzf.cu follow these rules, and tests/bgzfmodel compiles the
-// same source, so the CPU tests check the member-relative parse against the oracle and the framing against Python's gzip.
+// Like zb_members.h this is `__host__ __device__`: the kernels of zb_bgzf.cu follow these rules, and tests/bgzfmodel and
+// tests/batchmodel compile the same source, so the CPU tests check the member-relative parse against the oracle and the framing
+// against Python's gzip and zlib.
 //
-// The input is cut into blocks of kBgzfBlock bytes (htslib's BGZF_BLOCK_SIZE; the last may be shorter, an empty input has none).
-// Block m becomes one gzip member: the 18-byte header below, the raw deflate stream the reference writes for that block alone
-// (deflateInit2(level, Z_DEFLATED, -15, 8, Z_DEFAULT_STRATEGY) + deflate(Z_FINISH)), crc32 and ISIZE.  One exception: a payload
-// that would make the member longer than 64 KiB (BSIZE is 16 bits) is replaced by one stored block, 01 LEN NLEN data.  Only
+// BGZF.  The input is cut into blocks of kBgzfBlock bytes (htslib's BGZF_BLOCK_SIZE; the last may be shorter, an empty input has
+// none).  Block m becomes one gzip member: the 18-byte header below, the raw deflate stream the reference writes for that block
+// alone (deflateInit2(level, Z_DEFLATED, -15, 8, Z_DEFAULT_STRATEGY) + deflate(Z_FINISH)), crc32 and ISIZE.  One exception: a
+// payload that would make the member longer than 64 KiB (BSIZE is 16 bits) is replaced by one stored block, 01 LEN NLEN data.  Only
 // deflate_quick (level 1) on incompressible data gets there: it writes a single static block and has no stored fallback
 // (algorithm/quick.rs).  htslib's libdeflate path does the same (`uncomp:` in bgzf_compress).  The file ends with the 28-byte
 // empty member htslib writes as its end-of-file marker.
 //
-// On the device, member m is staged at m * kBgzfStride of the engine's input buffer, with zeros behind its bytes.  The stride is
-// two 32 KiB link tiles, so the link kernels of the single-stream path run over the staged buffer unchanged; BgzfAcc then reads
-// member m in its own coordinates and cuts every hash chain at the member's start.
+// Batch.  Item i (at most kMemberMax bytes) becomes the stream zb_deflate writes for it alone: stream_header / stream_trailer of
+// zb_core.h around the same raw payload.  There is no stored fallback (a level-1 item may come out longer than it went in, as with
+// the reference), and level 0 cuts stored blocks at 65535 bytes as the single-stream writer does (stored_blocks in zb_core.h), so a
+// 65536-byte item has two.  The items' streams are packed back to back in input order.
+//
+// Staging.  Member m is staged at moff[m] of the engine's input buffer with at least kMemberGap zero bytes behind it: BGZF at
+// m * kBgzfStride, a batch packed by batch_stage_next().  The link kernels of the single-stream path run over the whole staged
+// buffer unchanged, as if it were one stream; BgzfAcc then reads member m in its own coordinates.  That is exact whatever lies
+// in front of or behind the member:
+//   - a link is the nearest earlier position with the same hash.  If that position lies in front of the member's start, no
+//     position of the member has that hash earlier either, so cutting the link ("no link") is what the member alone has;
+//   - the hash of a position whose `need` bytes reach past the member's end reads bytes that are not the member's: no link, as a
+//     one-shot input of that length never inserts it;
+//   - bytes behind the member are never read from the staged buffer (BgzfAcc::byte gives the reference's window contents);
+//     only the 16-byte refills of the level-1/2 input ring (RingAcc, zb_serial.h) load them, and read the zero gap.
+// The symbols, M and nxt entries of member m live at the same offset moff[m] of their buffers (at most one per input byte).
 #pragma once
 #include "zb_core.h"
 
 namespace zb {
 
-constexpr uint32_t kBgzfBlock = 0xff00;      // input bytes per member
-constexpr uint32_t kBgzfStride = 65536;      // staging stride of the members on the device
+constexpr uint32_t kBgzfBlock = 0xff00;      // input bytes per BGZF member
+constexpr uint32_t kBgzfStride = 65536;      // staging stride of the BGZF members on the device
 constexpr uint32_t kBgzfHeader = 18;         // 1f 8b 08 04 MTIME(0) XFL(0) OS(ff) XLEN(6) 'B' 'C' SLEN(2) BSIZE
 constexpr uint32_t kBgzfTrailer = 8;         // crc32, ISIZE
 constexpr uint32_t kBgzfMaxMember = 65536;   // BSIZE + 1
 constexpr uint32_t kBgzfEofLen = 28;
-constexpr uint32_t kBgzfMaxBlocks = 5;       // deflate blocks of a member: 16383 symbols each (memLevel 8), at most 65280 symbols
+constexpr uint32_t kMemberMax = 65536;       // input bytes of a member: BGZF members have at most kBgzfBlock, batch items this many
+constexpr uint32_t kMemberGap = 64;          // zero bytes staged behind every batch item (>= the 16 bytes a ring refill reads)
+// deflate blocks of a member: 16383 symbols each (memLevel 8; deflate_quick's pieces have the same size), so at most
+// 65536 / 16383 + 1 = 5 for a member of kMemberMax bytes (one symbol per byte at most)
+constexpr uint32_t kBgzfMaxBlocks = kMemberMax / kBlockSyms + 1;
+static_assert(kBgzfMaxBlocks == 5, "block slots per member");
+constexpr uint32_t kWrapBgzf = 3;            // BgzfJob::wrap of a BGZF file; 0 / 1 / 2 are the raw / zlib / gzip batch items
+
+// batch limits (zb_deflate_batch): staged offsets and symbol indices are 32-bit
+constexpr uint64_t kBatchMaxItems = 65535;
+constexpr uint64_t kBatchMaxBytes = 1ull << 31;
+constexpr uint64_t kBatchMaxInflateItems = 1ull << 20;
 
 ZB_HD uint64_t bgzf_members(uint64_t n) { return (n + kBgzfBlock - 1) / kBgzfBlock; }
 ZB_HD uint32_t bgzf_member_len(uint64_t n, uint64_t m)
@@ -36,30 +62,16 @@ ZB_HD uint32_t bgzf_member_len(uint64_t n, uint64_t m)
 // file length bound: every member at most 64 KiB, plus the end-of-file member
 ZB_HD uint64_t bgzf_bound(uint64_t n) { return bgzf_members(n) * kBgzfMaxMember + kBgzfEofLen; }
 
-// the payload does not fit a member: write the block stored instead
+// the payload does not fit a BGZF member: write the block stored instead
 ZB_HD bool bgzf_stored(uint64_t payload) { return kBgzfHeader + payload + kBgzfTrailer > kBgzfMaxMember; }
-ZB_HD uint32_t bgzf_stored_payload(uint32_t len) { return len + 5; }
-// 01 LEN NLEN: the one stored block (BFINAL set) in front of the block's bytes
-ZB_HD void bgzf_stored_header(uint8_t *p, uint32_t len)
-{
-    p[0] = 1;
-    p[1] = (uint8_t)len;
-    p[2] = (uint8_t)(len >> 8);
-    p[3] = (uint8_t)~len;
-    p[4] = (uint8_t)(~len >> 8);
-}
 
-// header of a member of `member_bytes` bytes in all (BSIZE = member_bytes - 1)
+// header of a BGZF member of `member_bytes` bytes in all (BSIZE = member_bytes - 1)
 ZB_HD void bgzf_header(uint8_t *h, uint32_t member_bytes)
 {
     const uint8_t fixed[16] = {0x1f, 0x8b, 8, 4, 0, 0, 0, 0, 0, 0xff, 6, 0, 'B', 'C', 2, 0};
     for (int i = 0; i < 16; i++) h[i] = fixed[i];
     h[16] = (uint8_t)(member_bytes - 1);
     h[17] = (uint8_t)((member_bytes - 1) >> 8);
-}
-ZB_HD void bgzf_trailer(uint8_t *t, uint32_t crc, uint32_t isize)
-{
-    for (int i = 0; i < 4; i++) { t[i] = (uint8_t)(crc >> (8 * i)); t[4 + i] = (uint8_t)(isize >> (8 * i)); }
 }
 // byte i of the end-of-file member: a BGZF member with an empty payload (03 00: an empty static block) and an empty trailer
 ZB_HD uint8_t bgzf_eof(uint32_t i)
@@ -68,13 +80,27 @@ ZB_HD uint8_t bgzf_eof(uint32_t i)
     return eof[i];
 }
 
-// Member m of a staged input, in its own coordinates: position y reads in[m * kBgzfStride + y].  Behind the member's `n` bytes it
-// reads what the reference's window buffer holds behind a one-shot input of n bytes (zeros up to 64 KiB, cf. GAcc), which is what
-// the padded single-stream buffer gives.  A link that reaches farther back than y crosses the member's start: "no link".  `need`
-// is the span of the hash (4 bytes, 3 for the rolling hash of level 9): a position whose hash reaches past the end has no link.
-// Every position counts as inserted: serial_medium keeps its own bitmap, and deflate_slow inserts every position.
+// Framing of a member: BGZF (the trailer is gzip's), or the stream of a batch item.
+ZB_HD uint32_t member_header_len(uint32_t wrap) { return wrap == kWrapBgzf ? kBgzfHeader : stream_header_len(wrap); }
+ZB_HD uint32_t member_trailer_len(uint32_t wrap) { return wrap == kWrapBgzf ? kBgzfTrailer : stream_trailer_len(wrap); }
+
+// Where batch item i is staged: each item at a 64-byte aligned offset with at least kMemberGap zero bytes behind it.  off(0) = 0;
+// off(i + 1) = batch_stage_next(off(i), len(i)).
+ZB_HD uint64_t batch_stage_next(uint64_t off, uint64_t len) { return (off + len + kMemberGap + 63) & ~63ull; }
+// Largest stream zb_deflate writes for n bytes (zb_deflate_bound; zb_deflate_batch_bound is the sum over the items): the
+// conservative bound of the reference (deflate.rs:3193-3205: n + (n+7)/8 + (n+63)/64 + 5 + wrapper).  deflate_quick has no stored
+// fallback and codes a literal in up to 9 bits (deflate_quick_overhead, :3169-3176); every other path of the engine stays below
+// stored + framing, which this covers for every memLevel.
+ZB_HD uint64_t stream_bound(uint64_t n) { return n + ((n + 7) >> 3) + ((n + 63) >> 6) + 5 + 18 + 64; }
+
+// Member m of a staged input, in its own coordinates: position y reads in[moff[m] + y].  Behind the member's `n` bytes it
+// reads what the reference's window buffer holds behind a one-shot input of n bytes (zeros up to 64 KiB, then the bytes one window
+// earlier, cf. GAcc: a member of kMemberMax bytes slides the window once), so it never reads the staged buffer behind the member.
+// A link that reaches farther back than y crosses the member's start: "no link".  `need` is the span of the hash (4 bytes, 3 for
+// the rolling hash of level 9): a position whose hash reaches past the end has no link.  Every position counts as inserted:
+// serial_medium keeps its own bitmap, and deflate_slow inserts every position.
 struct BgzfAcc {
-    const uint8_t *data; // in + m * kBgzfStride
+    const uint8_t *data; // in + moff[m]
     const uint16_t *L;   // links of the staged buffer, from the same offset
     uint32_t N;          // the member's length
     uint32_t need;

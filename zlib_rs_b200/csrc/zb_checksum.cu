@@ -426,6 +426,48 @@ __global__ void __launch_bounds__(1024) k_crc_join(const uint32_t *__restrict__ 
     if (tid == 0) *out = sc[0];
 }
 
+// k_adler_segments: the adler32 of every segment [off[s], off[s] + len[s]) of buf, one CTA per segment (batch items: zlib-framed
+// deflate items, zlib items on inflate), the counterpart of k_crc_segments.  Thread t takes the t-th of 256 equal pieces and sums
+// (A, B, n) over it (B = sum (n - i) d_i, as k_adler_partial); the pieces join in order as k_adler_final joins chunks.
+__global__ void __launch_bounds__(256) k_adler_segments(const uint8_t *__restrict__ buf, const uint64_t *__restrict__ off,
+                                                        const uint32_t *__restrict__ len, uint32_t *__restrict__ out)
+{
+    __shared__ unsigned long long sA[256], sB[256], sN[256];
+    const uint32_t tid = threadIdx.x, s = blockIdx.x;
+    const uint32_t L = len[s], piece = (L + 255) / 256;
+    const uint8_t *p = buf + off[s];
+    const uint64_t b0 = min((uint64_t)tid * piece, (uint64_t)L), e0 = min(b0 + piece, (uint64_t)L);
+    unsigned long long a = 0, b = 0;
+    for (uint64_t i = b0; i < e0; i++) {
+        const uint32_t d = p[i];
+        a += d;
+        b += (e0 - i) * d; // a piece of a segment below 4 GiB is below 2^24 bytes: b < 2^56
+    }
+    sA[tid] = a % kAdlerBase;
+    sB[tid] = b % kAdlerBase;
+    sN[tid] = e0 - b0;
+    __syncthreads();
+    for (uint32_t h = 1; h < 256; h <<= 1) {
+        if ((tid & (2 * h - 1)) == 0) {
+            sB[tid] = (sB[tid] + (sN[tid + h] % kAdlerBase) * sA[tid] + sB[tid + h]) % kAdlerBase;
+            sA[tid] = (sA[tid] + sA[tid + h]) % kAdlerBase;
+            sN[tid] += sN[tid + h];
+        }
+        __syncthreads();
+    }
+    if (tid == 0) { // start value 1: s1 = 1 + A, s2 = n + B
+        const unsigned long long r1 = (1 + sA[0]) % kAdlerBase, r2 = (L % kAdlerBase + sB[0]) % kAdlerBase;
+        out[s] = (uint32_t)(r1 | (r2 << 16));
+    }
+}
+
+cudaError_t launch_adler32_segments(const uint8_t *d_buf, const uint64_t *d_off, const uint32_t *d_len, uint32_t nseg, uint32_t *d_adler,
+                                    cudaStream_t st)
+{
+    if (nseg) k_adler_segments<<<nseg, 256, 0, st>>>(d_buf, d_off, d_len, d_adler);
+    return cudaGetLastError();
+}
+
 cudaError_t launch_crc32_segments(const uint8_t *d_buf, const uint64_t *d_off, const uint32_t *d_len, uint32_t nseg, uint32_t *d_crc,
                                   cudaStream_t st)
 {

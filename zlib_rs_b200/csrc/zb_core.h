@@ -45,6 +45,53 @@ constexpr uint32_t kTailZone = 1024;              // bytes at the end handled by
 constexpr uint32_t kMSafe = 640;                  // M(x) is only consulted for x + kMSafe <= N
 constexpr uint32_t kPad = 1024;                   // zero padding after the input in device memory
 
+// Stream framing without gz_header: the single-stream writer (k_scan_blocks, k_stored, k_finish) and the batch members
+// (k_bgzf_frame) both write it from here.  wrap: 0 raw, 1 zlib, 2 gzip (deflate.rs:286-298).
+// zlib FLEVEL (deflate.rs:1591-1601): strategy >= Z_HUFFMAN_ONLY or level < 2 -> 0
+ZB_HD uint32_t zlib_level_flags(uint32_t level, bool plain_strategy)
+{
+    return (plain_strategy || level < 2) ? 0u : level < 6 ? 1u : level == 6 ? 2u : 3u;
+}
+// gzip XFL (deflate.rs:2574-2599)
+ZB_HD uint32_t gzip_xfl(int level, int strategy) { return level == 9 ? 2u : (strategy >= 2 || level < 2) ? 4u : 0u; }
+ZB_HD uint32_t stream_header_len(uint32_t wrap) { return wrap == 1 ? 2u : wrap == 2 ? 10u : 0u; }
+ZB_HD uint32_t stream_trailer_len(uint32_t wrap) { return wrap == 1 ? 4u : wrap == 2 ? 8u : 0u; }
+// zlib: CMF/FLG with the window's CINFO and FCHECK (deflate.rs:1572-1601); gzip: 1f 8b 08 00, MTIME 0, XFL, OS 3 (unix)
+ZB_HD void stream_header(uint8_t *h, uint32_t wrap, uint32_t level_flags, uint32_t cinfo, uint32_t xfl)
+{
+    if (wrap == 1) {
+        uint32_t v = ((8u + (cinfo << 4)) << 8) | (level_flags << 6);
+        v += 31 - (v % 31);
+        h[0] = (uint8_t)(v >> 8);
+        h[1] = (uint8_t)v;
+    } else if (wrap == 2) {
+        const uint8_t g[10] = {31, 139, 8, 0, 0, 0, 0, 0, (uint8_t)xfl, 3};
+        for (int i = 0; i < 10; i++) h[i] = g[i];
+    }
+}
+// zlib: adler32 big-endian (deflate.rs:2786-2789); gzip: crc32 and ISIZE little-endian (deflate.rs:2773-2785)
+ZB_HD void stream_trailer(uint8_t *t, uint32_t wrap, uint32_t check, uint32_t isize)
+{
+    if (wrap == 1) {
+        for (int i = 0; i < 4; i++) t[i] = (uint8_t)(check >> (24 - 8 * i));
+    } else if (wrap == 2) {
+        for (int i = 0; i < 4; i++) { t[i] = (uint8_t)(check >> (8 * i)); t[4 + i] = (uint8_t)(isize >> (8 * i)); }
+    }
+}
+// level 0 (deflate/algorithm/stored.rs, one-shot with ample output): stored blocks of at most 65535 bytes, one (empty) block for
+// an empty input; each is 00/01 LEN NLEN data, byte aligned
+constexpr uint32_t kStoredMax = 65535;
+ZB_HD uint64_t stored_blocks(uint64_t n) { return n == 0 ? 1 : (n + kStoredMax - 1) / kStoredMax; }
+ZB_HD uint64_t stored_payload(uint64_t n) { return n + 5 * stored_blocks(n); }
+ZB_HD void stored_header(uint8_t *p, uint32_t len, bool last)
+{
+    p[0] = last ? 1 : 0;
+    p[1] = (uint8_t)len;
+    p[2] = (uint8_t)(len >> 8);
+    p[3] = (uint8_t)~len;
+    p[4] = (uint8_t)(~len >> 8);
+}
+
 struct LevelParams {
     uint32_t good, lazy, nice, chain;
     uint32_t early_exit;  // level < 5: no look-ahead, early chain exit (longest_match.rs:3,130)

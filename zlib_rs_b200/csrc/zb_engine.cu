@@ -60,7 +60,7 @@ __global__ void k_tail_slow(JobBufs);
 __global__ void k_serial_low(JobBufs);
 __global__ void k_links_dict_ghost(JobBufs, uint32_t *);
 __global__ void k_links_dict_ghost_apply(JobBufs, const uint32_t *);
-// BGZF writing (zb_bgzf.cu, zb_serial.cu, zb_kernels.cu)
+// member writing: BGZF and batches (zb_bgzf.cu, zb_serial.cu, zb_kernels.cu)
 __global__ void k_bgzf_setup(BgzfJob, uint64_t);
 __global__ void k_serial_low_members(JobBufs, BgzfJob);
 __global__ void k_bgzf_medium(JobBufs, BgzfJob);
@@ -72,6 +72,7 @@ __global__ void k_bgzf_size(JobBufs, BgzfJob);
 __global__ void k_bgzf_scan(JobBufs, BgzfJob);
 __global__ void k_bgzf_encode(JobBufs, BgzfJob);
 __global__ void k_bgzf_frame(JobBufs, BgzfJob);
+__global__ void k_batch_stage(const uint8_t *, const uint64_t *, BgzfJob, uint8_t *, uint64_t);
 
 constexpr uint32_t kMatchSmemBytes = (kWSize + kMatchSub + 512) + (kWSize + kMatchSub) * 2 + ((kWSize + kMatchSub) / 32 + 1) * 4 * 4 + 8192;
 constexpr uint32_t kPathSmemBytes = kPathTile * 4 * 3;
@@ -188,13 +189,7 @@ int Engine::stage(size_t bytes)
 }
 
 
-size_t deflate_bound(size_t n)
-{
-    // The conservative bound of the reference (deflate.rs:3193-3205: n + (n+7)/8 + (n+63)/64 + 5 + wrapper): deflate_quick has no
-    // stored fallback and codes a literal in up to 9 bits (deflate_quick_overhead, :3169-3176); every other path of the engine
-    // stays below stored + framing, which this covers for every memLevel.
-    return n + ((n + 7) >> 3) + ((n + 63) >> 6) + 5 + 18 + 64;
-}
+size_t deflate_bound(size_t n) { return (size_t)stream_bound(n); } // zb_bgzf.h
 
 int Engine::deflate(const void *src, size_t n_in, bool src_dev, void *dst, size_t dst_cap, bool dst_dev, int level, int strategy,
                     int window_bits, uint32_t flags, zb_deflate_result *res, const void *dict, size_t dict_len)
@@ -348,7 +343,7 @@ int Engine::deflate(const void *src, size_t n_in, bool src_dev, void *dst, size_
     jb.prime_bits = (flags >> 12) & 7u;
     if ((jb.end_mode && !jb.not_last) || (jb.prime_bits && wrap != 0)) { snprintf(g_err, sizeof g_err, "END_* needs NOT_LAST, PRIME a raw stream"); return ZB_E_PARAM; }
     if (jb.not_last && (level == 0 || wrap != 0)) { snprintf(g_err, sizeof g_err, "NOT_LAST needs raw deflate and level > 0"); return ZB_E_PARAM; }
-    jb.xfl = level == 9 ? 2 : (strategy >= 2 || level < 2) ? 4 : 0;
+    jb.xfl = gzip_xfl(level, strategy);
     // levels 3..9 and Z_RLE follow the reference parser exactly; levels 1 and 2 run the level-3 kernel set
     int eng_level = level;
     // Only the 32 KiB window is implemented.  A smaller window changes nothing but the header's CINFO as long as the input never
@@ -681,24 +676,13 @@ int Engine::deflate(const void *src, size_t n_in, bool src_dev, void *dst, size_
     return ZB_OK;
 }
 
-// ZB_FLAG_BGZF (zb_bgzf.h, DESIGN.md §2h): every 65280-byte block of the input is deflated alone and framed as one BGZF member.  The
-// members are staged side by side and every kernel covers all of them, so a call costs a fixed number of launches and two host
-// syncs (the file length, then the end of the copy) whatever its length.
-int Engine::deflate_bgzf(const void *src, size_t n, bool src_dev, void *dst, size_t dst_cap, bool dst_dev, int level, zb_deflate_result *res)
+// The member core of BGZF writing and the batch (zb_bgzf.h): buffers for `nm` members staged in `span` bytes, of which the link
+// kernels cover the first S, and the member tables.  The caller stages the members and fills moff / mlen / mcheck.
+int Engine::members_reserve(JobBufs &jb, BgzfJob &bj, uint32_t nm, uint32_t S, size_t span, int level, size_t out_cap, uint32_t wrap,
+                            uint32_t **d_freq)
 {
-    if (!res || (!src && n) || !dst) return ZB_E_PARAM;
-    memset(res, 0, sizeof *res);
-    const uint64_t nm64 = bgzf_members(n);
-    if (nm64 >= 65535) { snprintf(g_err, sizeof g_err, "input too large for one job (%zu)", n); return ZB_E_PARAM; } // staged offsets are 32-bit
-    if (level == -1) level = 6;
-    CK(cudaSetDevice(device));
-    launches = 0;
-    const uint32_t nm = (uint32_t)nm64;
-    const uint32_t S = nm ? (nm - 1) * kBgzfStride + bgzf_member_len(n, nm - 1) : 0; // staged length: the link kernels' N
-    const size_t span = (size_t)nm * kBgzfStride;
     const uint32_t nmt = S / kLinkTile + 1, nslots = nm * kBgzfMaxBlocks;
     const bool links = level >= 3, slow = level >= 7;
-    JobBufs jb;
     memset(&jb, 0, sizeof jb);
     int rc;
     void *p;
@@ -706,7 +690,6 @@ int Engine::deflate_bgzf(const void *src, size_t n, bool src_dev, void *dst, siz
     if ((rc = reserve(slot, bytes, &p)) != ZB_OK) return rc;            \
     jb.field = static_cast<type>(p);
     RES(S_IN, span + kPad + 16, in, const uint8_t *)
-    uint8_t *d_in = const_cast<uint8_t *>(jb.in);
     jb.N = S;
     jb.level = (uint32_t)level;
     jb.wsize = kWSize;
@@ -714,16 +697,15 @@ int Engine::deflate_bgzf(const void *src, size_t n, bool src_dev, void *dst, siz
     jb.serial_mode = level == 1 || level == 2 ? (uint32_t)level : 0u;
     if (level >= 3 && level <= 6) jb.lp = level_params(level);
     if (slow) { jb.slow_mode = 1; jb.sp = slow_params(level); jb.sp.wsize = kWSize; }
-    const size_t out_cap = (bgzf_bound(n) + 15) & ~(size_t)15;
     RES(S_OUT, out_cap + 16, out, uint8_t *)
     jb.out_cap = out_cap;
-    uint32_t *d_freq = nullptr;
+    *d_freq = nullptr;
     if (level > 0 && nm) {
         RES(S_SYMS, (span + 64) * sizeof(Sym), syms, Sym *)
         RES(S_BLOCKS, (size_t)nslots * sizeof(BlockDesc), blocks, BlockDesc *)
         RES(S_BBASE, (size_t)nslots * 4, block_base, uint32_t *)
         if ((rc = reserve(S_FREQ, (size_t)nslots * 320 * 4, &p)) != ZB_OK) return rc;
-        d_freq = static_cast<uint32_t *>(p);
+        *d_freq = static_cast<uint32_t *>(p);
     }
     if (links && nm) {
         RES(S_L, (span + kPad) * 2, L, uint16_t *)
@@ -735,39 +717,29 @@ int Engine::deflate_bgzf(const void *src, size_t n, bool src_dev, void *dst, siz
         RES(S_NXT, span * 4, nxt, uint32_t *)
     }
 #undef RES
-    // member tables: moff | mout (8 bytes each) | mlen | mcrc | mbytes | mstored | minfo | ctl
+    // member tables: moff | mout (8 bytes each) | mlen | mcheck | mbytes | mstored | minfo | ctl
     const size_t m8 = ((size_t)nm * 8 + 15) & ~(size_t)15, m4 = ((size_t)nm * 4 + 15) & ~(size_t)15;
     const size_t mi_bytes = ((size_t)nm * sizeof(JobInfo) + 15) & ~(size_t)15;
     if ((rc = reserve(S_BGZF, 2 * m8 + 4 * m4 + mi_bytes + sizeof(BgzfCtl), &p)) != ZB_OK) return rc;
     uint8_t *t = static_cast<uint8_t *>(p);
-    BgzfJob bj;
     bj.nm = nm;
+    bj.wrap = wrap;
     bj.moff = reinterpret_cast<uint64_t *>(t);
     bj.mout = reinterpret_cast<uint64_t *>(t + m8);
     bj.mlen = reinterpret_cast<uint32_t *>(t + 2 * m8);
-    bj.mcrc = reinterpret_cast<uint32_t *>(t + 2 * m8 + m4);
+    bj.mcheck = reinterpret_cast<uint32_t *>(t + 2 * m8 + m4);
     bj.mbytes = reinterpret_cast<uint32_t *>(t + 2 * m8 + 2 * m4);
     bj.mstored = reinterpret_cast<uint32_t *>(t + 2 * m8 + 3 * m4);
     bj.minfo = reinterpret_cast<JobInfo *>(t + 2 * m8 + 4 * m4);
     bj.ctl = reinterpret_cast<BgzfCtl *>(t + 2 * m8 + 4 * m4 + mi_bytes);
-    if ((rc = stage(sizeof(BgzfCtl) + 16)) != ZB_OK) return rc;
+    return ZB_OK;
+}
 
-    CK(cudaEventRecord(ev0, st));
-    // staging: one pitched copy of the whole blocks, the short last one, zeros in the gaps and behind the last member
-    const cudaMemcpyKind kind = src_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
-    const uint8_t *s8 = static_cast<const uint8_t *>(src);
-    if (nm > 1) {
-        CK(cudaMemcpy2DAsync(d_in, kBgzfStride, s8, kBgzfBlock, kBgzfBlock, nm - 1, kind, st));
-        CK(cudaMemset2DAsync(d_in + kBgzfBlock, kBgzfStride, 0, kBgzfStride - kBgzfBlock, nm - 1, st));
-    }
-    if (nm) CK(cudaMemcpyAsync(d_in + (size_t)(nm - 1) * kBgzfStride, s8 + (size_t)(nm - 1) * kBgzfBlock, S - (nm - 1) * kBgzfStride, kind, st));
-    CK(cudaMemsetAsync(d_in + S, 0, span - S + kPad + 16, st));
-    CK(cudaMemsetAsync(bj.minfo, 0, mi_bytes + sizeof(BgzfCtl), st));
-    CK(cudaMemsetAsync(jb.out, 0, out_cap, st));
-    k_bgzf_setup<<<nm / 256 + 1, 256, 0, st>>>(bj, (uint64_t)n);
-    CK(launch_crc32_segments(d_in, bj.moff, bj.mlen, nm, bj.mcrc, st));
-    CK(launch_crc32_join(bj.mcrc, bj.mlen, &bj.ctl->count, d_check, st));
-    launches += 3;
+// ... and its launches behind the staging: links, parse, blocks, sizes and offsets, encoding, framing.
+int Engine::members_launch(JobBufs &jb, BgzfJob &bj, int level, uint32_t *d_freq)
+{
+    const uint32_t nm = bj.nm, S = jb.N, nmt = S / kLinkTile + 1, nslots = nm * kBgzfMaxBlocks;
+    const bool links = level >= 3, slow = level >= 7;
     if (level > 0 && nm) {
         if (links) {
             if (jb.sp.slow) {
@@ -786,7 +758,7 @@ int Engine::deflate_bgzf(const void *src, size_t n, bool src_dev, void *dst, siz
             k_bgzf_medium<<<nm, 32, 0, st>>>(jb, bj);
             launches++;
         } else {
-            k_bgzf_slow_steps<<<nm * (kBgzfStride / 256), 256, 0, st>>>(jb, bj);
+            k_bgzf_slow_steps<<<nm * (kMemberMax / 256), 256, 0, st>>>(jb, bj);
             k_bgzf_slow_walk<<<(nm + 31) / 32, 32, 0, st>>>(jb, bj);
             launches += 2;
         }
@@ -804,6 +776,51 @@ int Engine::deflate_bgzf(const void *src, size_t n, bool src_dev, void *dst, siz
     k_bgzf_frame<<<nm + 1, 256, 0, st>>>(jb, bj);
     launches++;
     CK(cudaGetLastError());
+    return ZB_OK;
+}
+
+// ZB_FLAG_BGZF (zb_bgzf.h, DESIGN.md §2h): every 65280-byte block of the input is deflated alone and framed as one BGZF member.  The
+// members are staged side by side and every kernel covers all of them, so a call costs a fixed number of launches and two host
+// syncs (the file length, then the end of the copy) whatever its length.
+int Engine::deflate_bgzf(const void *src, size_t n, bool src_dev, void *dst, size_t dst_cap, bool dst_dev, int level, zb_deflate_result *res)
+{
+    if (!res || (!src && n) || !dst) return ZB_E_PARAM;
+    memset(res, 0, sizeof *res);
+    const uint64_t nm64 = bgzf_members(n);
+    if (nm64 >= 65535) { snprintf(g_err, sizeof g_err, "input too large for one job (%zu)", n); return ZB_E_PARAM; } // staged offsets are 32-bit
+    if (level == -1) level = 6;
+    CK(cudaSetDevice(device));
+    launches = 0;
+    const uint32_t nm = (uint32_t)nm64;
+    const uint32_t S = nm ? (nm - 1) * kBgzfStride + bgzf_member_len(n, nm - 1) : 0; // staged length: the link kernels' N
+    const size_t span = (size_t)nm * kBgzfStride;
+    const size_t out_cap = (bgzf_bound(n) + 15) & ~(size_t)15;
+    JobBufs jb;
+    BgzfJob bj;
+    uint32_t *d_freq;
+    int rc;
+    if ((rc = members_reserve(jb, bj, nm, S, span, level, out_cap, kWrapBgzf, &d_freq)) != ZB_OK) return rc;
+    if ((rc = stage(sizeof(BgzfCtl) + 16)) != ZB_OK) return rc;
+    uint8_t *d_in = const_cast<uint8_t *>(jb.in);
+    const size_t mi_bytes = ((size_t)nm * sizeof(JobInfo) + 15) & ~(size_t)15;
+
+    CK(cudaEventRecord(ev0, st));
+    // staging: one pitched copy of the whole blocks, the short last one, zeros in the gaps and behind the last member
+    const cudaMemcpyKind kind = src_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+    const uint8_t *s8 = static_cast<const uint8_t *>(src);
+    if (nm > 1) {
+        CK(cudaMemcpy2DAsync(d_in, kBgzfStride, s8, kBgzfBlock, kBgzfBlock, nm - 1, kind, st));
+        CK(cudaMemset2DAsync(d_in + kBgzfBlock, kBgzfStride, 0, kBgzfStride - kBgzfBlock, nm - 1, st));
+    }
+    if (nm) CK(cudaMemcpyAsync(d_in + (size_t)(nm - 1) * kBgzfStride, s8 + (size_t)(nm - 1) * kBgzfBlock, S - (nm - 1) * kBgzfStride, kind, st));
+    CK(cudaMemsetAsync(d_in + S, 0, span - S + kPad + 16, st));
+    CK(cudaMemsetAsync(bj.minfo, 0, mi_bytes + sizeof(BgzfCtl), st));
+    CK(cudaMemsetAsync(jb.out, 0, out_cap, st));
+    k_bgzf_setup<<<nm / 256 + 1, 256, 0, st>>>(bj, (uint64_t)n);
+    CK(launch_crc32_segments(d_in, bj.moff, bj.mlen, nm, bj.mcheck, st));
+    CK(launch_crc32_join(bj.mcheck, bj.mlen, &bj.ctl->count, d_check, st));
+    launches += 3;
+    if ((rc = members_launch(jb, bj, level, d_freq)) != ZB_OK) return rc;
     BgzfCtl *h_ctl = static_cast<BgzfCtl *>(h_stage);
     uint32_t *h_crc = reinterpret_cast<uint32_t *>(h_ctl + 1);
     CK(cudaMemcpyAsync(h_ctl, bj.ctl, sizeof(BgzfCtl), cudaMemcpyDeviceToHost, st));
@@ -830,6 +847,123 @@ int Engine::deflate_bgzf(const void *src, size_t n, bool src_dev, void *dst, siz
     res->exact_parity = 1;
     res->gpu_ms = ms;
     res->bits_used = 8;
+    return ZB_OK;
+}
+
+// zb_deflate_batch (zb_bgzf.h, DESIGN.md §2i): item i is deflated alone and framed as its own zlib / gzip / raw stream, byte for
+// byte what zb_deflate gives for it.  The items are packed into the staged buffer by the host's member table and go through the
+// member core of BGZF; a call costs a fixed number of launches and two host syncs whatever the number and lengths of its items.
+int Engine::deflate_batch(const void *src, const uint64_t *src_off, size_t n_items, bool src_dev, void *dst, size_t dst_cap, bool dst_dev,
+                          int level, int strategy, int window_bits, uint32_t flags, uint64_t *dst_off, uint32_t *checks,
+                          zb_deflate_result *res)
+{
+    if (!res || !dst_off || (n_items && (!src_off || !dst))) { snprintf(g_err, sizeof g_err, "deflate_batch: null argument"); return ZB_E_PARAM; }
+    memset(res, 0, sizeof *res);
+    const uint32_t ml = (flags >> 8) & 15u;
+    uint32_t wrap;
+    if (window_bits == 15) wrap = 1;
+    else if (window_bits == 31) wrap = 2;
+    else if (window_bits == -15) wrap = 0;
+    else { snprintf(g_err, sizeof g_err, "deflate_batch takes window_bits 15, -15 or 31"); return ZB_E_PARAM; }
+    if ((flags & ~ZB_FLAG_MEMLEVEL(15)) || (ml && ml != 8) || strategy != 0 || level < -1 || level > 9) {
+        snprintf(g_err, sizeof g_err, "deflate_batch takes Z_DEFAULT_STRATEGY, level -1..9, memLevel 8 and no flag");
+        return ZB_E_PARAM;
+    }
+    if (n_items > kBatchMaxItems) { snprintf(g_err, sizeof g_err, "deflate_batch: %zu items (at most %llu)", n_items, (unsigned long long)kBatchMaxItems); return ZB_E_PARAM; }
+    // the member table, on the host: items at 64-byte aligned staged offsets with a zero gap behind each
+    const uint32_t nm = (uint32_t)n_items;
+    uint64_t span = 0, bound = 0;
+    for (uint32_t i = 0; i < nm; i++) {
+        if (src_off[i + 1] < src_off[i] || src_off[i + 1] - src_off[i] > kMemberMax) {
+            snprintf(g_err, sizeof g_err, "deflate_batch: item %u is not 0..%u bytes", i, kMemberMax);
+            return ZB_E_PARAM;
+        }
+        span = batch_stage_next(span, src_off[i + 1] - src_off[i]);
+        bound += stream_bound(src_off[i + 1] - src_off[i]);
+    }
+    const uint64_t total = nm ? src_off[nm] - src_off[0] : 0;
+    if (total > kBatchMaxBytes) { snprintf(g_err, sizeof g_err, "deflate_batch: %llu bytes in all (at most 2^31)", (unsigned long long)total); return ZB_E_PARAM; }
+    if (total && !src) { snprintf(g_err, sizeof g_err, "deflate_batch: null source"); return ZB_E_PARAM; }
+    if (level == -1) level = 6;
+    res->exact_parity = 1;
+    res->bits_used = 8;
+    dst_off[0] = 0;
+    if (nm == 0) return ZB_OK;
+    CK(cudaSetDevice(device));
+    launches = 0;
+    const uint32_t S = (uint32_t)span; // the link kernels run over the gaps too: their links are cut like any other crossing link
+    const size_t out_cap = (bound + 15) & ~(size_t)15;
+    JobBufs jb;
+    BgzfJob bj;
+    uint32_t *d_freq;
+    int rc;
+    if ((rc = members_reserve(jb, bj, nm, S, span, level, out_cap, wrap, &d_freq)) != ZB_OK) return rc;
+    // pinned staging: the member table up (moff | mlen | src_off), the control block, offsets and checks down
+    const size_t t_up = (size_t)nm * 8 + (size_t)nm * 4 + ((size_t)nm + 1) * 8, t_down = sizeof(BgzfCtl) + (size_t)nm * 12 + 16;
+    if ((rc = stage(t_up + t_down + 64)) != ZB_OK) return rc;
+    uint8_t *h = static_cast<uint8_t *>(h_stage);
+    uint64_t *h_moff = reinterpret_cast<uint64_t *>(h);
+    uint32_t *h_mlen = reinterpret_cast<uint32_t *>(h + (size_t)nm * 8);
+    uint64_t *h_soff = reinterpret_cast<uint64_t *>(h + (size_t)nm * 12);
+    BgzfCtl *h_ctl = reinterpret_cast<BgzfCtl *>(h + ((t_up + 15) & ~(size_t)15));
+    uint64_t *h_mout = reinterpret_cast<uint64_t *>(h_ctl + 1);
+    uint32_t *h_chk = reinterpret_cast<uint32_t *>(h_mout + nm);
+    uint64_t off = 0;
+    for (uint32_t i = 0; i < nm; i++) {
+        h_moff[i] = off;
+        h_mlen[i] = (uint32_t)(src_off[i + 1] - src_off[i]);
+        off = batch_stage_next(off, h_mlen[i]);
+    }
+    memcpy(h_soff, src_off, ((size_t)nm + 1) * 8);
+    void *p;
+    if ((rc = reserve(S_BATCH, ((size_t)nm + 1) * 8 + 64 + (src_dev ? 0 : total), &p)) != ZB_OK) return rc;
+    uint64_t *d_soff = static_cast<uint64_t *>(p);
+    const uint8_t *d_src = src_dev ? static_cast<const uint8_t *>(src) + src_off[0]
+                                   : static_cast<const uint8_t *>(p) + ((((size_t)nm + 1) * 8 + 63) & ~(size_t)63);
+    const size_t mi_bytes = ((size_t)nm * sizeof(JobInfo) + 15) & ~(size_t)15;
+
+    CK(cudaEventRecord(ev0, st));
+    CK(cudaMemcpyAsync(bj.moff, h_moff, (size_t)nm * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(bj.mlen, h_mlen, (size_t)nm * 4, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_soff, h_soff, ((size_t)nm + 1) * 8, cudaMemcpyHostToDevice, st));
+    // staging: one contiguous copy of a host source, then every item to its staged offset with the gap behind it zeroed
+    if (!src_dev && total) CK(cudaMemcpyAsync(const_cast<uint8_t *>(d_src), static_cast<const uint8_t *>(src) + src_off[0], total, cudaMemcpyHostToDevice, st));
+    k_batch_stage<<<nm, 256, 0, st>>>(d_src, d_soff, bj, const_cast<uint8_t *>(jb.in), span);
+    CK(cudaMemsetAsync(const_cast<uint8_t *>(jb.in) + span, 0, kPad + 16, st));
+    CK(cudaMemsetAsync(bj.minfo, 0, mi_bytes + sizeof(BgzfCtl), st));
+    CK(cudaMemsetAsync(jb.out, 0, out_cap, st));
+    launches++;
+    // the items' checks, as zb_deflate returns them
+    if (wrap == 1) CK(launch_adler32_segments(jb.in, bj.moff, bj.mlen, nm, bj.mcheck, st));
+    else if (wrap == 2) CK(launch_crc32_segments(jb.in, bj.moff, bj.mlen, nm, bj.mcheck, st));
+    else CK(cudaMemsetAsync(bj.mcheck, 0, (size_t)nm * 4, st));
+    if (wrap) launches++;
+    if ((rc = members_launch(jb, bj, level, d_freq)) != ZB_OK) return rc;
+    CK(cudaMemcpyAsync(h_ctl, bj.ctl, sizeof(BgzfCtl), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(h_mout, bj.mout, (size_t)nm * 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(h_chk, bj.mcheck, (size_t)nm * 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (h_ctl->error) { snprintf(g_err, sizeof g_err, "engine error flags 0x%x (batch)", h_ctl->error); return ZB_E_INTERNAL; }
+    const uint64_t out_bytes = h_ctl->out_bytes;
+    if (out_bytes > dst_cap) {
+        res->out_bytes = out_bytes;
+        return ZB_E_BUF;
+    }
+    CK(cudaMemcpyAsync(dst, jb.out, out_bytes, dst_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
+    CK(cudaEventRecord(ev1, st));
+    CK(cudaStreamSynchronize(st));
+    float ms = 0;
+    CK(cudaEventElapsedTime(&ms, ev0, ev1));
+    for (uint32_t i = 0; i < nm; i++) dst_off[i] = h_mout[i];
+    dst_off[nm] = out_bytes;
+    if (checks) memcpy(checks, h_chk, (size_t)nm * 4);
+    res->out_bytes = out_bytes;
+    res->data_type = (int32_t)h_ctl->data_type;
+    res->iterations = level > 0 ? 1 : 0;
+    res->n_symbols = h_ctl->n_syms;
+    res->n_blocks = h_ctl->n_blocks;
+    res->gpu_launches = launches;
+    res->gpu_ms = ms;
     return ZB_OK;
 }
 
@@ -926,6 +1060,31 @@ int zb_deflate_ex(zb_engine *z, const void *src, size_t n, int src_dev, void *ds
 size_t zb_deflate_bound(size_t n) { return zb::deflate_bound(n); }
 
 size_t zb_bgzf_bound(size_t n) { return (size_t)zb::bgzf_bound(n); }
+
+int zb_deflate_batch(zb_engine *z, const void *src, const uint64_t *src_off, size_t n_items, int src_dev, void *dst, size_t cap,
+                     int dst_dev, int level, int strategy, int window_bits, uint32_t flags, uint64_t *dst_off, uint32_t *checks,
+                     zb_deflate_result *res)
+{
+    if (!z) return ZB_E_NODEVICE;
+    z->e.shard.phase = 0; // a range job in progress is gone (its buffers are reused)
+    return z->e.deflate_batch(src, src_off, n_items, src_dev != 0, dst, cap, dst_dev != 0, level, strategy, window_bits, flags, dst_off,
+                              checks, res);
+}
+
+size_t zb_deflate_batch_bound(const uint64_t *src_off, size_t n_items)
+{
+    size_t b = 0;
+    for (size_t i = 0; i < n_items; i++) b += (size_t)zb::stream_bound(src_off[i + 1] - src_off[i]);
+    return b;
+}
+
+int zb_inflate_batch(zb_engine *z, const void *src, const uint64_t *src_off, size_t n_items, int src_dev, void *dst, const uint64_t *dst_off,
+                     int dst_dev, int window_bits, zb_inflate_result *items)
+{
+    if (!z) return ZB_E_NODEVICE;
+    z->e.shard.phase = 0; // a range job in progress is gone (its buffers are reused)
+    return z->e.inflate_batch(src, src_off, n_items, src_dev != 0, dst, dst_off, dst_dev != 0, window_bits, items);
+}
 
 int zb_inflate(zb_engine *z, const void *src, size_t n, int src_dev, void *dst, size_t cap, int dst_dev, int window_bits,
                zb_inflate_result *res)

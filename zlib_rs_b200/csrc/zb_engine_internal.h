@@ -15,7 +15,8 @@ size_t deflate_bound(size_t n);
 enum { S_IN, S_L, S_HOLES, S_HOLESN, S_M, S_NXT, S_PEXIT, S_PCNT, S_SYMIDX, S_TENTRY, S_TSYMB, S_TDIRTY, S_SYMS, S_SYMB,
        S_BLOCKS, S_SCRATCH, S_FREQ, S_OUT, S_CK, S_INF0, S_INF1, S_PHEAD, S_SK, S_MARKN, S_LLIST, S_LCNT, S_BMAP, S_HDIFF, S_HCOARSE, S_CSTATE, S_LISTS, S_LR, S_LLAST, S_BBASE, S_MCHG, S_GFN, S_KEYS, S_SHARD,
        S_MEMT, S_MEMC, // multi-member gzip: tile counts and control block; candidate and member tables
-       S_BGZF,         // BGZF writing: member tables and control block
+       S_BGZF,         // BGZF writing and deflate batches: member tables and control block
+       S_BATCH,        // batches: the caller's offsets, a host source's bytes (deflate), item tables and results (inflate)
        S_COUNT };
 
 // A range job of chunk-sharded deflate (zb_shard_*, zb_shard.cu) between its four calls.
@@ -32,7 +33,7 @@ struct ShardState {
 };
 
 struct Engine {
-    static constexpr int kSlots = 41;
+    static constexpr int kSlots = 42;
     struct Buf { void *p = nullptr; size_t cap = 0; };
     int device = -1;
     cudaStream_t st = nullptr, st2 = nullptr; // st2: the serial tail runs beside k_emit
@@ -67,11 +68,18 @@ struct Engine {
     int deflate(const void *src, size_t n, bool src_dev, void *dst, size_t dst_cap, bool dst_dev, int level, int strategy,
                 int window_bits, uint32_t flags, zb_deflate_result *res, const void *dict = nullptr, size_t dict_len = 0);
     int deflate_bgzf(const void *src, size_t n, bool src_dev, void *dst, size_t dst_cap, bool dst_dev, int level, zb_deflate_result *res);
+    int deflate_batch(const void *src, const uint64_t *src_off, size_t n_items, bool src_dev, void *dst, size_t dst_cap, bool dst_dev,
+                      int level, int strategy, int window_bits, uint32_t flags, uint64_t *dst_off, uint32_t *checks, zb_deflate_result *res);
+    int members_reserve(JobBufs &jb, BgzfJob &bj, uint32_t nm, uint32_t S, size_t span, int level, size_t out_cap, uint32_t wrap,
+                        uint32_t **d_freq);
+    int members_launch(JobBufs &jb, BgzfJob &bj, int level, uint32_t *d_freq);
     int inflate(const void *src, size_t n, bool src_dev, void *dst, size_t dst_cap, bool dst_dev, int window_bits,
                 zb_inflate_result *res, uint32_t flags = 0);
     int inflate_stream(const uint8_t *d_src, size_t n, uint8_t *d_dst, size_t dst_cap, int window_bits, uint32_t flags,
                        zb_inflate_result *res);
     int inflate_members(const uint8_t *d_src, size_t n, uint8_t *d_dst, size_t dst_cap, int window_bits, zb_inflate_result *res);
+    int inflate_batch(const void *src, const uint64_t *src_off, size_t n_items, bool src_dev, void *dst, const uint64_t *dst_off,
+                      bool dst_dev, int window_bits, zb_inflate_result *items);
     int inflate_blocks(const void *src, size_t n, uint64_t start_bit, const void *dict, size_t dict_len, void *dst, size_t dst_cap,
                        int check_kind, uint32_t check_start, zb_inflate_seg *out);
     int checksum(bool crc, uint32_t start, const void *buf, size_t len, bool on_dev, uint32_t *out, float *ms);

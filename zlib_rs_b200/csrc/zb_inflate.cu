@@ -28,7 +28,8 @@ struct ICode { uint8_t op, bits; uint16_t val; };
 enum InfErr {
     IE_OK = 0, IE_HEADER_CHECK, IE_METHOD, IE_WINDOW, IE_BLOCK_TYPE, IE_STORED_LEN, IE_TOO_MANY, IE_CODE_LENS, IE_REPEAT,
     IE_NO_EOB, IE_LITLEN_SET, IE_DIST_SET, IE_LITLEN_CODE, IE_DIST_CODE, IE_TOO_FAR, IE_TRUNCATED, IE_OUTPUT_FULL, IE_GZ_FLAGS,
-    IE_HCRC, IE_NEED_DICT
+    IE_HCRC, IE_NEED_DICT,
+    IE_DATA_CHECK, IE_LENGTH_CHECK // the trailer disagrees with the output (decided after the decode: inflate_stream, k_batch_verdict)
 };
 
 struct InfState { // device result block
@@ -1390,6 +1391,57 @@ __global__ void __launch_bounds__(1024) k_mem_verdict(const InfState *mst, const
     }
 }
 
+// ================================================================================================
+// Batch inflate (zb_inflate_batch, DESIGN.md §2i): every item is an independent stream with its own output slot.
+//   k_batch_members                 the decoder of k_inflate on every item, one warp each, from the caller's table;
+//   k_crc_segments, k_adler_segments  the check of each item's output, by the framing its header turned out to have;
+//   k_batch_verdict                 one status per item: the decoder's, or the trailer check inflate_stream makes.
+// The launch count does not depend on the number or the lengths of the items.
+// ================================================================================================
+struct BatchItem {     // the caller's table, relative to the staged source and destination
+    uint64_t in_off, in_len, out_off, out_cap;
+};
+struct BatchResult {   // what comes back to the host per item
+    uint64_t out_bytes, in_bytes;
+    uint32_t check, err; // err: InfErr, IE_OUTPUT_FULL is ZB_E_BUF
+};
+
+__global__ void __launch_bounds__(32) k_batch_members(const uint8_t *__restrict__ src, const BatchItem *items, uint8_t *__restrict__ dst,
+                                                      int window_bits, InfState *ist, uint64_t *out_off, uint32_t *crc_len,
+                                                      uint32_t *adler_len)
+{
+    extern __shared__ __align__(16) uint8_t smem_raw[];
+    const uint32_t i = blockIdx.x;
+    const BatchItem it = items[i];
+    inflate_warp(*reinterpret_cast<InfShared *>(smem_raw), src + it.in_off, it.in_len, dst + it.out_off, it.out_cap, window_bits, ist + i,
+                 InfSeg{0, nullptr, 0, 0});
+    __syncwarp();
+    if (threadIdx.x == 0) {
+        // inflate_stream checks what was produced unless the output did not fit; an item's slots hold below 4 GiB (host check)
+        const InfState &r = ist[i];
+        const uint32_t n = r.err == IE_OUTPUT_FULL ? 0u : (uint32_t)r.out_bytes;
+        out_off[i] = it.out_off;
+        crc_len[i] = r.kind == 2 ? n : 0u;
+        adler_len[i] = r.kind == 1 ? n : 0u;
+    }
+}
+
+// One thread per item: the status inflate_stream gives for it alone (the decoder's error, else the trailer checks) and its check.
+__global__ void __launch_bounds__(256) k_batch_verdict(const InfState *ist, const uint32_t *crc, const uint32_t *adler, uint32_t n,
+                                                       BatchResult *out)
+{
+    const uint32_t i = blockIdx.x * 256 + threadIdx.x;
+    if (i >= n) return;
+    const InfState &r = ist[i];
+    const uint32_t check = r.kind == 2 ? crc[i] : r.kind == 1 ? adler[i] : 1u; // a raw stream has no check: adler32's start value
+    uint32_t err = r.err;
+    if (err == IE_OK && r.kind != 0) {
+        if (check != r.trailer_check) err = IE_DATA_CHECK;
+        else if (r.kind == 2 && (uint32_t)r.out_bytes != r.trailer_len) err = IE_LENGTH_CHECK;
+    }
+    out[i] = BatchResult{r.out_bytes, r.in_bytes, check, err};
+}
+
 static const char *inf_msg(uint32_t e)
 {
     switch (e) {
@@ -1411,6 +1463,8 @@ static const char *inf_msg(uint32_t e)
     case IE_HCRC: return "header crc mismatch";
     case IE_NEED_DICT: return "need dictionary";
     case IE_TRUNCATED: return "unexpected end of input";
+    case IE_DATA_CHECK: return "incorrect data check";
+    case IE_LENGTH_CHECK: return "incorrect length check";
     default: return "";
     }
 }
@@ -1421,6 +1475,8 @@ int Engine::inflate_init()
     if (e != cudaSuccess) { snprintf(g_err, sizeof g_err, "k_inflate attr: %s", cudaGetErrorString(e)); return ZB_E_CUDA; }
     e = cudaFuncSetAttribute(k_members, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(InfShared));
     if (e != cudaSuccess) { snprintf(g_err, sizeof g_err, "k_members attr: %s", cudaGetErrorString(e)); return ZB_E_CUDA; }
+    e = cudaFuncSetAttribute(k_batch_members, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(InfShared));
+    if (e != cudaSuccess) { snprintf(g_err, sizeof g_err, "k_batch_members attr: %s", cudaGetErrorString(e)); return ZB_E_CUDA; }
     if (cudaMalloc(&d_inf_state, sizeof(InfState)) != cudaSuccess) return ZB_E_MEM;
     if (cudaMallocHost(&h_inf_state, sizeof(InfState)) != cudaSuccess) return ZB_E_MEM;
     return ZB_OK;
@@ -1703,8 +1759,93 @@ int Engine::inflate_stream(const uint8_t *d_src, size_t n, uint8_t *d_dst, size_
     }
     res->check = check;
     if (status == ZB_OK && his->kind != 0) {
-        if (check != his->trailer_check) { status = ZB_E_DATA; snprintf(res->msg, sizeof res->msg, "incorrect data check"); }
-        else if (his->kind == 2 && (uint32_t)his->out_bytes != his->trailer_len) { status = ZB_E_DATA; snprintf(res->msg, sizeof res->msg, "incorrect length check"); }
+        if (check != his->trailer_check) { status = ZB_E_DATA; snprintf(res->msg, sizeof res->msg, "%s", inf_msg(IE_DATA_CHECK)); }
+        else if (his->kind == 2 && (uint32_t)his->out_bytes != his->trailer_len) { status = ZB_E_DATA; snprintf(res->msg, sizeof res->msg, "%s", inf_msg(IE_LENGTH_CHECK)); }
+    }
+    return status;
+}
+
+// zb_inflate_batch: item i of src[src_off[i], src_off[i+1]) into dst[dst_off[i], dst_off[i+1]), each as zb_inflate_ex decodes it
+// alone.  Fixed launches (k_batch_members, the two checksum kernels, k_batch_verdict) and one host sync.
+int Engine::inflate_batch(const void *src, const uint64_t *src_off, size_t n_items, bool src_dev, void *dst, const uint64_t *dst_off,
+                          bool dst_dev, int window_bits, zb_inflate_result *items)
+{
+    if (n_items && (!src_off || !dst_off || !items)) { snprintf(g_err, sizeof g_err, "inflate_batch: null argument"); return ZB_E_PARAM; }
+    if (window_bits < 0) { if (window_bits < -15 || window_bits > -8) return ZB_E_PARAM; }
+    else if (window_bits != 0 && ((window_bits & 15) < 8)) return ZB_E_PARAM;
+    if (window_bits > 47) return ZB_E_PARAM;
+    if (n_items > kBatchMaxInflateItems) {
+        snprintf(g_err, sizeof g_err, "inflate_batch: %zu items (at most %llu)", n_items, (unsigned long long)kBatchMaxInflateItems);
+        return ZB_E_PARAM;
+    }
+    const uint32_t nm = (uint32_t)n_items;
+    for (uint32_t i = 0; i < nm; i++) {
+        if (src_off[i + 1] < src_off[i] || dst_off[i + 1] < dst_off[i]) { snprintf(g_err, sizeof g_err, "inflate_batch: offsets of item %u decrease", i); return ZB_E_PARAM; }
+        if (dst_off[i + 1] - dst_off[i] > 0xffffffffull) { snprintf(g_err, sizeof g_err, "inflate_batch: slot of item %u is 4 GiB or more", i); return ZB_E_PARAM; }
+    }
+    const uint64_t in_total = nm ? src_off[nm] - src_off[0] : 0, out_total = nm ? dst_off[nm] - dst_off[0] : 0;
+    if ((in_total && !src) || (out_total && !dst)) { snprintf(g_err, sizeof g_err, "inflate_batch: null buffer"); return ZB_E_PARAM; }
+    for (uint32_t i = 0; i < nm; i++) memset(&items[i], 0, sizeof items[i]);
+    if (nm == 0) return ZB_OK;
+    CKI(cudaSetDevice(device));
+    launches = 0;
+    int rc;
+    void *p;
+    // S_BATCH: item table | results | output offsets | the two checksum length tables and their checks | decoder states
+    const size_t a_items = ((size_t)nm * sizeof(BatchItem) + 63) & ~(size_t)63, a_res = ((size_t)nm * sizeof(BatchResult) + 63) & ~(size_t)63;
+    const size_t a4 = ((size_t)nm * 4 + 63) & ~(size_t)63, a8 = ((size_t)nm * 8 + 63) & ~(size_t)63;
+    if ((rc = reserve(S_BATCH, a_items + a_res + a8 + 4 * a4 + (size_t)nm * sizeof(InfState), &p)) != ZB_OK) return rc;
+    uint8_t *t = static_cast<uint8_t *>(p);
+    BatchItem *d_items = reinterpret_cast<BatchItem *>(t);
+    BatchResult *d_res = reinterpret_cast<BatchResult *>(t + a_items);
+    uint64_t *d_ooff = reinterpret_cast<uint64_t *>(t + a_items + a_res);
+    uint32_t *d_clen = reinterpret_cast<uint32_t *>(t + a_items + a_res + a8), *d_alen = d_clen + a4 / 4;
+    uint32_t *d_crc = d_alen + a4 / 4, *d_adler = d_crc + a4 / 4;
+    InfState *d_ist = reinterpret_cast<InfState *>(d_adler + a4 / 4);
+    if ((rc = stage(a_items + a_res + 64)) != ZB_OK) return rc;
+    BatchItem *h_items = static_cast<BatchItem *>(h_stage);
+    BatchResult *h_res = reinterpret_cast<BatchResult *>(static_cast<uint8_t *>(h_stage) + a_items);
+    for (uint32_t i = 0; i < nm; i++)
+        h_items[i] = BatchItem{src_off[i] - src_off[0], src_off[i + 1] - src_off[i], dst_off[i] - dst_off[0], dst_off[i + 1] - dst_off[i]};
+    // the item offsets index the caller's buffers: a host buffer is copied (or staged) as one range
+    const uint8_t *d_src = static_cast<const uint8_t *>(src) + (nm ? src_off[0] : 0);
+    uint8_t *d_dst = static_cast<uint8_t *>(dst) + dst_off[0];
+    CKI(cudaEventRecord(ev0, st));
+    if (!src_dev) {
+        if ((rc = reserve(S_INF0, in_total + 64, &p)) != ZB_OK) return rc;
+        if (in_total) CKI(cudaMemcpyAsync(p, d_src, in_total, cudaMemcpyHostToDevice, st));
+        d_src = static_cast<const uint8_t *>(p);
+    }
+    if (!dst_dev) {
+        if ((rc = reserve(S_INF1, out_total + 64, &p)) != ZB_OK) return rc;
+        d_dst = static_cast<uint8_t *>(p);
+        CKI(cudaMemsetAsync(d_dst, 0, out_total, st)); // the slots go back whole: what lies behind an item's output is zeros
+    }
+    CKI(cudaMemcpyAsync(d_items, h_items, (size_t)nm * sizeof(BatchItem), cudaMemcpyHostToDevice, st));
+    k_batch_members<<<nm, 32, sizeof(InfShared), st>>>(d_src, d_items, d_dst, window_bits, d_ist, d_ooff, d_clen, d_alen);
+    CKI(launch_crc32_segments(d_dst, d_ooff, d_clen, nm, d_crc, st));
+    CKI(launch_adler32_segments(d_dst, d_ooff, d_alen, nm, d_adler, st));
+    k_batch_verdict<<<(nm + 255) / 256, 256, 0, st>>>(d_ist, d_crc, d_adler, nm, d_res);
+    launches += 4;
+    CKI(cudaMemcpyAsync(h_res, d_res, (size_t)nm * sizeof(BatchResult), cudaMemcpyDeviceToHost, st));
+    if (!dst_dev && out_total) CKI(cudaMemcpyAsync(static_cast<uint8_t *>(dst) + dst_off[0], d_dst, out_total, cudaMemcpyDeviceToHost, st));
+    CKI(cudaEventRecord(ev1, st));
+    CKI(cudaStreamSynchronize(st));
+    CKI(cudaGetLastError());
+    float ms = 0;
+    CKI(cudaEventElapsedTime(&ms, ev0, ev1));
+    int status = ZB_OK;
+    for (uint32_t i = 0; i < nm; i++) {
+        zb_inflate_result &r = items[i];
+        const BatchResult &b = h_res[i];
+        r.out_bytes = b.out_bytes;
+        r.in_bytes = b.in_bytes;
+        r.check = b.check;
+        r.status = b.err == IE_OK ? ZB_OK : b.err == IE_OUTPUT_FULL ? ZB_E_BUF : ZB_E_DATA;
+        if (r.status == ZB_E_DATA) snprintf(r.msg, sizeof r.msg, "%s", inf_msg(b.err));
+        r.gpu_launches = launches;
+        r.gpu_ms = ms;
+        if (status == ZB_OK) status = r.status;
     }
     return status;
 }

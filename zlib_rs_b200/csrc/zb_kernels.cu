@@ -1733,19 +1733,7 @@ __global__ void __launch_bounds__(256) k_scan_blocks(JobBufs jb)
     jb.info->out_bytes = bytes;
     jb.info->data_type = jb.blocks[0].sym_count ? jb.blocks[0].data_type : 2u;
     if (bytes > jb.out_cap) { atomicOr(&jb.info->error, 8u); return; }
-    if (jb.wrap == 1) {
-        // zlib header (deflate.rs:1572-1601)
-        // level_flags (deflate.rs:1591-1601): strategy >= HuffmanOnly or level < 2 -> 0
-        const uint32_t lf = (jb.huffman_only || jb.strategy_fixed || jb.level < 2) ? 0 : jb.level < 6 ? 1 : jb.level == 6 ? 2 : 3;
-        uint32_t h = ((8u + (jb.cinfo << 4)) << 8) | (lf << 6);
-        h += 31 - (h % 31);
-        jb.out[0] = (uint8_t)(h >> 8);
-        jb.out[1] = (uint8_t)h;
-    } else if (jb.wrap == 2) {
-        // gzip header without gz_header (deflate.rs:2574-2599): 1f 8b 08 00 mtime(0) xfl os(3 = unix)
-        const uint8_t g[10] = {31, 139, 8, 0, 0, 0, 0, 0, (uint8_t)jb.xfl, 3};
-        for (int i = 0; i < 10; i++) jb.out[i] = g[i];
-    }
+    stream_header(jb.out, jb.wrap, zlib_level_flags(jb.level, jb.huffman_only || jb.strategy_fixed), jb.cinfo, jb.xfl);
 }
 
 // Bit packing of one block at bd.bit_base of the zeroed output, one CTA of 1024 threads; a body of other than body_bits bits sets
@@ -1860,8 +1848,8 @@ __global__ void __launch_bounds__(1024) k_encode(JobBufs jb)
 }
 
 // ------------------------------------------------------------------------------------------------
-// BGZF members (zb_bgzf.h, zb_bgzf.cu): the block kernels above over every member at once, one CTA per block slot
-// m * kBgzfMaxBlocks + k.  Positions and symbols are member-relative; in_start and sym_begin point into the staged buffers.
+// Members of a BGZF file or a batch (zb_bgzf.h, zb_bgzf.cu): the block kernels above over every member at once, one CTA per block
+// slot m * kBgzfMaxBlocks + k.  Positions and symbols are member-relative; in_start and sym_begin point into the staged buffers.
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) k_bgzf_hist(JobBufs jb, BgzfJob bj, uint32_t *freq)
 {
@@ -1869,7 +1857,7 @@ __global__ void __launch_bounds__(256) k_bgzf_hist(JobBufs jb, BgzfJob bj, uint3
     const JobInfo &mi = bj.minfo[m];
     const uint32_t nsyms = mi.n_syms, nblocks = mi.n_blocks;
     if (k >= nblocks) return;
-    const uint32_t base = m * kBgzfStride, len = bj.mlen[m];
+    const uint32_t base = (uint32_t)bj.moff[m], len = bj.mlen[m];
     const Sym *syms = jb.syms + base;
     const uint32_t begin = k * jb.block_syms;
     const uint32_t count = k + 1 < nblocks ? jb.block_syms : nsyms - begin;
@@ -1915,15 +1903,7 @@ __global__ void k_finish(JobBufs jb, const uint32_t *check)
     const uint64_t p = (jb.info->total_bits + 7) >> 3;
     const uint32_t a = *check;
     if (jb.not_last && jb.end_mode == 0) { jb.out[jb.info->marker_byte + 2] = 0xff; jb.out[jb.info->marker_byte + 3] = 0xff; }
-    if (jb.wrap == 1) { // adler32, big endian (deflate.rs:2786-2789)
-        jb.out[p] = (uint8_t)(a >> 24);
-        jb.out[p + 1] = (uint8_t)(a >> 16);
-        jb.out[p + 2] = (uint8_t)(a >> 8);
-        jb.out[p + 3] = (uint8_t)a;
-    } else if (jb.wrap == 2) { // crc32 + isize, little endian (deflate.rs:2773-2785)
-        for (int i = 0; i < 4; i++) jb.out[p + i] = (uint8_t)(a >> (8 * i));
-        for (int i = 0; i < 4; i++) jb.out[p + 4 + i] = (uint8_t)((jb.N - jb.start) >> (8 * i));
-    }
+    stream_trailer(jb.out + p, jb.wrap, a, jb.N - jb.start);
     jb.info->adler = a;
 }
 
@@ -1957,32 +1937,19 @@ __global__ void __launch_bounds__(256) k_literal_syms(JobBufs jb)
 __global__ void __launch_bounds__(256) k_stored(JobBufs jb)
 {
     const uint32_t N = jb.N - jb.start; // a dictionary does not enter stored blocks
-    const uint32_t nb = N == 0 ? 1 : (N + 65534) / 65535;
+    const uint32_t nb = (uint32_t)stored_blocks(N);
     const uint32_t b = blockIdx.x;
     if (b >= nb) return;
-    const uint32_t start = b * 65535u;
-    const uint32_t len = min(65535u, N - start);
-    uint8_t *o = jb.out + jb.hdr_len + (uint64_t)b * (65535u + 5u);
+    const uint32_t start = b * kStoredMax;
+    const uint32_t len = min(kStoredMax, N - start);
+    uint8_t *o = jb.out + jb.hdr_len + (uint64_t)b * (kStoredMax + 5u);
     if (threadIdx.x == 0) {
-        o[0] = b + 1 == nb ? 1 : 0;
-        o[1] = (uint8_t)len;
-        o[2] = (uint8_t)(len >> 8);
-        o[3] = (uint8_t)~len;
-        o[4] = (uint8_t)((~len) >> 8);
+        stored_header(o, len, b + 1 == nb);
         if (b == 0) {
-            jb.info->total_bits = 8ull * (jb.hdr_len + (uint64_t)N + 5ull * nb);
-            jb.info->out_bytes = jb.hdr_len + (uint64_t)N + 5ull * nb + (jb.wrap == 1 ? 4 : jb.wrap == 2 ? 8 : 0);
+            jb.info->total_bits = 8ull * (jb.hdr_len + stored_payload(N));
+            jb.info->out_bytes = jb.hdr_len + stored_payload(N) + stream_trailer_len(jb.wrap);
             jb.info->data_type = 2;
-            if (jb.wrap == 1) {
-                uint32_t h = (8u + (jb.cinfo << 4)) << 8; // level_flags 0 (deflate.rs:1572-1601)
-                h += 31 - (h % 31);
-                jb.out[0] = (uint8_t)(h >> 8);
-                jb.out[1] = (uint8_t)h;
-            }
-            else if (jb.wrap == 2) {
-                const uint8_t g[10] = {31, 139, 8, 0, 0, 0, 0, 0, 4, 3};
-                for (int i = 0; i < 10; i++) jb.out[i] = g[i];
-            }
+            stream_header(jb.out, jb.wrap, 0, jb.cinfo, 4); // level 0: FLEVEL 0, XFL 4
         }
     }
     for (uint32_t i = threadIdx.x; i < len; i += blockDim.x) o[5 + i] = jb.in[jb.start + start + i];

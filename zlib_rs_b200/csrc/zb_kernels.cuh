@@ -115,9 +115,9 @@ struct JobBufs {
     uint32_t cinfo;           // zlib header CINFO = windowBits - 8 (7 unless the whole input fits a smaller window's match range)
 };
 
-// One BGZF call (ZB_FLAG_BGZF, zb_bgzf.h): member m is staged at m * kBgzfStride of JobBufs::in, its symbols start at
-// syms[m * kBgzfStride], its deflate blocks are blocks[m * kBgzfMaxBlocks + k] and the window bases of their flushes
-// block_base[m * kBgzfMaxBlocks + k].
+// One member call (zb_bgzf.h): a BGZF file (ZB_FLAG_BGZF) or a batch of streams (zb_deflate_batch).  Member m is staged at
+// moff[m] of JobBufs::in, its symbols start at syms[moff[m]], its deflate blocks are blocks[m * kBgzfMaxBlocks + k] and the
+// window bases of their flushes block_base[m * kBgzfMaxBlocks + k].
 struct BgzfCtl {
     uint32_t count;     // members (k_crc_join)
     uint32_t error;     // non-zero: internal invariant violated
@@ -125,16 +125,17 @@ struct BgzfCtl {
     uint32_t n_syms;    // symbols of the compressed members
     uint32_t data_type; // of the first block, as a single-stream job reports it
     uint32_t pad;
-    uint64_t out_bytes; // file length
+    uint64_t out_bytes; // file length (BGZF) or the batch's total output
 };
 struct BgzfJob {
     uint32_t nm;        // members
+    uint32_t wrap;      // framing of every member: kWrapBgzf, or 0 raw / 1 zlib / 2 gzip (batch items)
     uint64_t *moff;     // staged offset of member m
     uint32_t *mlen;     // its input bytes
-    uint32_t *mcrc;     // its crc32
-    uint32_t *mbytes;   // its length in the file
-    uint64_t *mout;     // its offset in the file
-    uint32_t *mstored;  // 1: written as one stored block (level 0, or the payload does not fit 64 KiB)
+    uint32_t *mcheck;   // its check: crc32 (BGZF, gzip), adler32 (zlib), 0 (raw)
+    uint32_t *mbytes;   // its length in the output
+    uint64_t *mout;     // its offset in the output
+    uint32_t *mstored;  // 1: written as stored blocks (level 0, or a BGZF payload that does not fit 64 KiB)
     JobInfo *minfo;     // n_syms, n_blocks and final_base of its parse, as a single-stream parse reports them
     BgzfCtl *ctl;
 };
@@ -149,5 +150,8 @@ cudaError_t launch_crc32(const uint8_t *d_buf, uint64_t len, uint32_t start, voi
 cudaError_t launch_crc32_segments(const uint8_t *d_buf, const uint64_t *d_off, const uint32_t *d_len, uint32_t nseg, uint32_t *d_crc,
                                   cudaStream_t st);
 cudaError_t launch_crc32_join(const uint32_t *d_crc, const uint32_t *d_len, const uint32_t *d_count, uint32_t *d_out, cudaStream_t st);
+// adler32 of every segment [off[s], off[s] + len[s]) of d_buf (batch items, zb_bgzf.cu / zb_inflate.cu)
+cudaError_t launch_adler32_segments(const uint8_t *d_buf, const uint64_t *d_off, const uint32_t *d_len, uint32_t nseg, uint32_t *d_adler,
+                                    cudaStream_t st);
 
 } // namespace zb

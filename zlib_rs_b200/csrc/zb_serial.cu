@@ -94,12 +94,14 @@ __global__ void __launch_bounds__(32) k_serial_low(JobBufs jb)
     else serial_low_body<kRingFast, true>(jb, smem);
 }
 
-// BGZF (zb_bgzf.h): one CTA per member, each parsing its block alone as k_serial_low parses a stream.  At level 1 the 64 KiB ring
-// holds the whole member.
+// BGZF and batches (zb_bgzf.h): one CTA per member, each parsing its member alone as k_serial_low parses a stream.  At level 1 the
+// 64 KiB ring holds a whole member of up to kMemberMax bytes; its refills read 16-byte rows, the last one into the zero gap
+// behind the member.
+static_assert(kRingQuick >= kMemberMax, "level-1 ring");
 __global__ void __launch_bounds__(32) k_serial_low_members(JobBufs jb, BgzfJob bj)
 {
     extern __shared__ __align__(16) uint8_t smem[];
-    const uint32_t m = blockIdx.x, base = m * kBgzfStride;
+    const uint32_t m = blockIdx.x, base = (uint32_t)bj.moff[m];
     JobBufs mj = jb;
     mj.in = jb.in + base;
     mj.N = bj.mlen[m];
