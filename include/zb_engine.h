@@ -123,6 +123,22 @@ ZB_API int zb_deflate_batch(zb_engine *e, const void *src, const uint64_t *src_o
                             uint32_t *checks, zb_deflate_result *res);
 ZB_API size_t zb_deflate_batch_bound(const uint64_t *src_off, size_t n_items); /* sum of zb_deflate_bound(len_i) */
 
+/* zb_deflate_batch_dict: zb_deflate_batch with one preset dictionary for every item (DESIGN.md §2j).  Item i's stream is byte for
+ * byte what deflateInit2(level, Z_DEFLATED, window_bits, 8, Z_DEFAULT_STRATEGY) + deflateSetDictionary(dict, dict_len) +
+ * deflate(Z_FINISH) writes for it alone.  dict is a host pointer, or a device pointer with src_on_device (as zb_deflate_dict).
+ *   window_bits 15: a non-empty dictionary gives the header FDICT and DICTID = the adler32 of the whole dictionary; the trailer
+ *                   and checks[i] are the adler32 of the item alone.  dict_len 0 gives exactly zb_deflate_batch's bytes.
+ *   window_bits -15: the payload only, checks[i] = 0.  window_bits 31 (gzip) takes no dictionary: ZB_E_PARAM.
+ * A dictionary of 65536 bytes or more puts only its last 32768 bytes in the window (DICTID still covers all of it).  Levels -1, 0
+ * and 3..9; levels 1 and 2 give ZB_E_PARAM (no exact parser with a dictionary), so res->exact_parity is 1 on every accepted call.
+ * The other limits are zb_deflate_batch's, and the staged bytes -- every item behind its own copy of the dictionary's window bytes,
+ * 64-byte aligned with a 64-byte gap -- are at most 2^31.  zb_deflate_batch_bound is enough for the output.  Launches: those of
+ * zb_deflate_batch, one more for DICTID (window_bits 15, dict_len > 0) and one more at levels 3..8 when the window holds at least
+ * 3 dictionary bytes. */
+ZB_API int zb_deflate_batch_dict(zb_engine *e, const void *dict, size_t dict_len, const void *src, const uint64_t *src_off,
+                                 size_t n_items, int src_on_device, void *dst, size_t dst_cap, int dst_on_device, int level, int strategy,
+                                 int window_bits, uint32_t flags, uint64_t *dst_off, uint32_t *checks, zb_deflate_result *res);
+
 typedef struct zb_inflate_result {
     uint64_t out_bytes;
     uint64_t in_bytes;   /* compressed bytes consumed */
@@ -166,6 +182,16 @@ ZB_API int zb_inflate_ex(zb_engine *e, const void *src, size_t src_len, int src_
  * ZB_E_PARAM).  Each item is decoded by one warp: a single large stream decodes faster through zb_inflate_ex. */
 ZB_API int zb_inflate_batch(zb_engine *e, const void *src, const uint64_t *src_off, size_t n_items, int src_on_device, void *dst,
                             const uint64_t *dst_off, int dst_on_device, int window_bits, zb_inflate_result *items);
+/* zb_inflate_batch_dict: zb_inflate_batch with one preset dictionary (DESIGN.md §2j).  items[i] gets what inflateInit2(window_bits),
+ * inflateSetDictionary(dict) up front for a raw stream or after inflate() returned Z_NEED_DICT, and inflate(Z_FINISH) give for
+ * that item alone: a raw item decodes with the dictionary as its window, a zlib item with FDICT when its DICTID equals
+ * adler32(dict) (1 for an empty dictionary).  An FDICT item naming another dictionary keeps "need dictionary"; zlib items without
+ * FDICT and gzip items decode as with zb_inflate_batch.  The window holds the last 32 KiB of the dictionary; out_bytes, the slot and
+ * check cover the item's own output.  dict is a host pointer, or a device pointer with src_on_device.  One launch more than
+ * zb_inflate_batch (the dictionary's adler32). */
+ZB_API int zb_inflate_batch_dict(zb_engine *e, const void *dict, size_t dict_len, const void *src, const uint64_t *src_off,
+                                 size_t n_items, int src_on_device, void *dst, const uint64_t *dst_off, int dst_on_device, int window_bits,
+                                 zb_inflate_result *items);
 
 /* Streaming building block (what inflate() of the zlib ABI runs on, zlib-rs/src/inflate.rs:2376-2457): decode the COMPLETE deflate
  * blocks of a raw deflate segment.  src/dict/dst are host buffers; decoding starts at bit `start_bit` of src with the last

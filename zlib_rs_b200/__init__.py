@@ -139,6 +139,9 @@ def lib():
                                            ctypes.POINTER(DeflateResult)]
             L.zb_deflate_batch_bound.argtypes, L.zb_deflate_batch_bound.restype = [u64p, sz], sz
             L.zb_inflate_batch.argtypes = [vp, vp, u64p, sz, ci, vp, u64p, ci, ci, ctypes.POINTER(InflateResult)]
+        if hasattr(L, "zb_deflate_batch_dict"):
+            L.zb_deflate_batch_dict.argtypes = [vp, vp, sz] + L.zb_deflate_batch.argtypes[1:]
+            L.zb_inflate_batch_dict.argtypes = [vp, vp, sz] + L.zb_inflate_batch.argtypes[1:]
         L.zb_adler32.argtypes = [vp, u32, vp, sz, ci, ctypes.POINTER(u32), ctypes.POINTER(ctypes.c_float)]
         L.zb_crc32.argtypes = [vp, u32, vp, sz, ci, ctypes.POINTER(u32), ctypes.POINTER(ctypes.c_float)]
         L.zb_engine_set_profile.argtypes = [vp, ci]
@@ -183,6 +186,16 @@ def _gather(items):
     items = [bytes(x) for x in items]
     data = b"".join(items)
     return (ctypes.c_char * max(len(data), 1)).from_buffer_copy(data or b"\0"), _offsets([len(x) for x in items])
+
+
+def _dictionary(dictionary, on_device):
+    """(pointer, length, keep-alive) of a preset dictionary: bytes-like on the host, (device pointer, length) with on_device."""
+    if on_device:
+        ptr, n = dictionary
+        return ptr, n, None
+    data = bytes(dictionary)
+    keep = (ctypes.c_char * max(len(data), 1)).from_buffer_copy(data or b"\0")
+    return ctypes.addressof(keep), len(data), keep
 
 
 def deflate_batch_bound(lengths):
@@ -423,12 +436,14 @@ class Engine:
         return rc, (own.raw[: res.out_bytes] if own is not None else None), res
 
     def deflate_batch(self, items, level=-1, window_bits=15, strategy=0, mem_level=8, flags=0, src_on_device=False, src_off=None,
-                      dst=None, dst_cap=0, dst_on_device=False):
+                      dst=None, dst_cap=0, dst_on_device=False, dictionary=None):
         """Deflate every item as its own stream in one call (zb_deflate_batch): item i's stream is byte for byte what
         Engine.deflate gives for it alone.  Host `items`: a list of bytes-like objects; device `items`: a pointer, with `src_off`
         (n + 1 offsets into it).  Returns (list of bytes or None, offsets (n + 1), checks, DeflateResult); with a caller's `dst`
         the streams are packed back to back there and the first element is None.  Raises ZlibError (.needed: the size a too
-        small dst_cap would have to be)."""
+        small dst_cap would have to be).
+        With a `dictionary` (bytes-like, or (device pointer, length) with src_on_device) every item is deflated after
+        deflateSetDictionary(dictionary) (zb_deflate_batch_dict): zlib items carry FDICT and its adler32 as DICTID."""
         res = DeflateResult()
         flags |= (mem_level & 15) << 8
         keep = None
@@ -447,8 +462,13 @@ class Engine:
             dst_on_device = False
         dst_off = (ctypes.c_uint64 * (n + 1))()
         checks = (ctypes.c_uint32 * max(n, 1))()
-        rc = lib().zb_deflate_batch(self.h, src, off, n, int(src_on_device), dst, dst_cap, int(dst_on_device), level, strategy,
-                                    window_bits, flags, dst_off, checks, ctypes.byref(res))
+        args = (src, off, n, int(src_on_device), dst, dst_cap, int(dst_on_device), level, strategy, window_bits, flags, dst_off, checks,
+                ctypes.byref(res))
+        if dictionary is None:
+            rc = lib().zb_deflate_batch(self.h, *args)
+        else:
+            dptr, dlen, dkeep = _dictionary(dictionary, src_on_device)
+            rc = lib().zb_deflate_batch_dict(self.h, dptr, dlen, *args)
         if rc != 0:
             e = ZlibError(rc, lib().zb_last_error().decode())
             e.needed = res.out_bytes
@@ -459,11 +479,13 @@ class Engine:
         return outs, offs, list(checks)[:n], res
 
     def inflate_batch(self, items, out_caps, window_bits=15, src_on_device=False, src_off=None, dst=None, dst_off=None,
-                      dst_on_device=False):
+                      dst_on_device=False, dictionary=None):
         """Inflate every item into its own slot in one call (zb_inflate_batch).  Host `items`: a list of bytes-like objects and
         `out_caps` the slot length of each; device `items`: a pointer with `src_off`.  A caller's `dst` takes `dst_off` (n + 1
         offsets) instead of out_caps.  Returns (rc, list of bytes or None, list of InflateResult): each result is what
-        Engine.inflate gives for that item alone."""
+        Engine.inflate gives for that item alone.
+        With a `dictionary` (bytes-like, or (device pointer, length) with src_on_device; zb_inflate_batch_dict) raw items decode
+        with it as their window, and zlib items whose FDICT header names its adler32 too."""
         keep = None
         if src_on_device:
             off = (ctypes.c_uint64 * len(src_off))(*src_off)
@@ -481,7 +503,12 @@ class Engine:
         else:
             doff = (ctypes.c_uint64 * len(dst_off))(*dst_off)
         res = (InflateResult * max(n, 1))()
-        rc = lib().zb_inflate_batch(self.h, src, off, n, int(src_on_device), dst, doff, int(dst_on_device), window_bits, res)
+        args = (src, off, n, int(src_on_device), dst, doff, int(dst_on_device), window_bits, res)
+        if dictionary is None:
+            rc = lib().zb_inflate_batch(self.h, *args)
+        else:
+            dptr, dlen, dkeep = _dictionary(dictionary, src_on_device)
+            rc = lib().zb_inflate_batch_dict(self.h, dptr, dlen, *args)
         results = list(res)[:n]
         outs = None
         if own is not None:

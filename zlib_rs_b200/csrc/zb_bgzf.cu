@@ -17,25 +17,55 @@ __global__ void __launch_bounds__(256) k_bgzf_setup(BgzfJob bj, uint64_t n)
 }
 
 // Batch staging: item m of the contiguous source `src` (item m at src[soff[m] - soff[0]], the member table filled by the host) goes
-// to its staged offset, and the gap behind it up to the next item's offset (or `span`) is zeroed.  One CTA per item.
-__global__ void __launch_bounds__(256) k_batch_stage(const uint8_t *__restrict__ src, const uint64_t *__restrict__ soff, BgzfJob bj,
-                                                     uint8_t *__restrict__ in, uint64_t span)
+// to its staged offset behind its own copy of the dictionary's window bytes dict[0, bj.pstart), and the gap behind it up to the next
+// item's offset (or `span`) is zeroed.  One CTA per item.
+__global__ void __launch_bounds__(256) k_batch_stage(const uint8_t *__restrict__ src, const uint64_t *__restrict__ soff,
+                                                     const uint8_t *__restrict__ dict, BgzfJob bj, uint8_t *__restrict__ in, uint64_t span)
 {
-    const uint32_t m = blockIdx.x;
+    const uint32_t m = blockIdx.x, D = bj.pstart;
     const uint8_t *s = src + (soff[m] - soff[0]);
     uint8_t *d = in + bj.moff[m];
     const uint32_t len = bj.mlen[m];
     const uint64_t end = (m + 1 < bj.nm ? bj.moff[m + 1] : span) - bj.moff[m];
-    for (uint32_t i = threadIdx.x; i < end; i += 256) d[i] = i < len ? s[i] : 0;
+    for (uint32_t i = threadIdx.x; i < end; i += 256) d[i] = i < D ? dict[i] : i - D < len ? s[i - D] : 0;
+}
+
+// The stale head entry deflateSetDictionary leaves behind (k_links_dict_ghost), per member of a batch with a dictionary: the last
+// string the dictionary inserts, g = D' - 3, was hashed with a zero in place of the item's first byte, and the first later position
+// of that bucket K0 links to g.  One CTA per member scans the candidates g + 1 .. in rounds of 256 and stops at the first round
+// with a hit; candidates end where the member's hash reads end (its own bytes), so the work is bounded by the item's length.
+__global__ void __launch_bounds__(256) k_batch_dict_ghost(JobBufs jb, BgzfJob bj)
+{
+    __shared__ uint32_t first;
+    const uint32_t m = blockIdx.x, D = bj.pstart, N = D + bj.mlen[m];
+    if (D < 3 || N == D) return;
+    const uint8_t *d = jb.in + bj.moff[m];
+    const uint32_t g = D - 3;
+    const uint32_t k0 = hash_u32((uint32_t)d[g] | ((uint32_t)d[g + 1] << 8) | ((uint32_t)d[g + 2] << 16));
+    const uint32_t kt = hash_u32((uint32_t)d[g] | ((uint32_t)d[g + 1] << 8) | ((uint32_t)d[g + 2] << 16) | ((uint32_t)d[g + 3] << 24));
+    if (k0 == kt) return;
+    if (threadIdx.x == 0) first = 0xffffffffu;
+    __syncthreads();
+    const uint32_t last = min(g + kMaxDist, N - 4); // N >= D + 1 = g + 4
+    for (uint32_t r = g + 1; r <= last; r += 256) {
+        const uint32_t x = r + threadIdx.x;
+        bool hit = false;
+        if (x <= last) hit = hash_u32((uint32_t)d[x] | ((uint32_t)d[x + 1] << 8) | ((uint32_t)d[x + 2] << 16) | ((uint32_t)d[x + 3] << 24)) == k0;
+        if (hit) atomicMin(&first, x);
+        if (__syncthreads_or(hit)) break;
+    }
+    if (threadIdx.x == 0 && first != 0xffffffffu) jb.L[bj.moff[m] + first] = (uint16_t)(first - g);
 }
 
 // Levels 3..6: lane 0 runs the exact serial simulator over the whole member, as k_tail does over a short stream.  There are no
-// holes to iterate on: the simulator keeps its own inserted-positions bitmap (in shared memory, one bit per position of a member).
+// holes to iterate on: the simulator keeps its own inserted-positions bitmap (in shared memory, one bit per position from the parse
+// start on: an item has at most kMemberMax of them).  The dictionary's positions in front of the parse start count as inserted
+// (BgzfAcc::inserted), as deflateSetDictionary inserts every one of them.
 __global__ void __launch_bounds__(32) k_bgzf_medium(JobBufs jb, BgzfJob bj)
 {
     __shared__ uint32_t ins[kMemberMax / 32];
     if (threadIdx.x != 0) return;
-    const uint32_t m = blockIdx.x, base = (uint32_t)bj.moff[m], len = bj.mlen[m], bs = jb.block_syms;
+    const uint32_t m = blockIdx.x, base = (uint32_t)bj.moff[m], p0 = bj.pstart, len = p0 + bj.mlen[m], bs = jb.block_syms;
     const BgzfAcc a{jb.in + base, jb.L + base, len, 4u};
     Sym *syms = jb.syms + base;
     uint32_t *bb = jb.block_base + m * kBgzfMaxBlocks;
@@ -44,7 +74,7 @@ __global__ void __launch_bounds__(32) k_bgzf_medium(JobBufs jb, BgzfJob bj)
         syms[k++] = s;
         if (--left == 0) { bb[blk++] = B; left = bs; } // the window base when this symbol fills the block (k_block_hist's sym_base)
     };
-    const uint32_t fb = serial_medium(a, len, 0, ins, kMemberMax / 32, jb.lp, emit);
+    const uint32_t fb = serial_medium(a, len, p0, ins, kMemberMax / 32, jb.lp, emit);
     JobInfo &mi = bj.minfo[m];
     mi.n_syms = k;
     mi.final_base = fb;
@@ -52,13 +82,14 @@ __global__ void __launch_bounds__(32) k_bgzf_medium(JobBufs jb, BgzfJob bj)
 }
 
 // Levels 7..9: deflate_slow has no holes, so the macro step from a fresh loop-top is a function of its position (zb_slow.h).  One
-// thread per position of a member evaluates it through the member-relative accessor: kMemberMax / 256 CTAs per member.
+// thread per item position of a member (from the parse start on) evaluates it through the member-relative accessor: kMemberMax / 256
+// CTAs per member.
 __global__ void __launch_bounds__(256) k_bgzf_slow_steps(JobBufs jb, BgzfJob bj)
 {
-    const uint32_t m = blockIdx.x / (kMemberMax / 256), y = (blockIdx.x % (kMemberMax / 256)) * 256 + threadIdx.x;
+    const uint32_t m = blockIdx.x / (kMemberMax / 256), i = (blockIdx.x % (kMemberMax / 256)) * 256 + threadIdx.x;
     if (m >= bj.nm) return;
-    const uint32_t len = bj.mlen[m];
-    if (y >= len) return;
+    if (i >= bj.mlen[m]) return;
+    const uint32_t y = bj.pstart + i, len = bj.pstart + bj.mlen[m];
     const uint32_t base = (uint32_t)bj.moff[m], x = base + y;
     const BgzfAcc a{jb.in + base, jb.L + base, len, jb.sp.slow ? 3u : 4u};
     const SlowStep s = slow_step(a, y, len, jb.sp);
@@ -66,17 +97,18 @@ __global__ void __launch_bounds__(256) k_bgzf_slow_steps(JobBufs jb, BgzfJob bj)
     jb.nxt[x] = s.next;
 }
 
-// ... and one thread per member walks the steps from position 0 and writes the symbols (k_emit_slow + k_tail_slow of one member).
+// ... and one thread per member walks the steps from the parse start and writes the symbols (k_emit_slow + k_tail_slow of one
+// member).  `len` is the member's end in its own coordinates: the dictionary's bytes and the item's.
 __global__ void __launch_bounds__(32) k_bgzf_slow_walk(JobBufs jb, BgzfJob bj)
 {
     const uint32_t m = blockIdx.x * 32 + threadIdx.x;
     if (m >= bj.nm) return;
-    const uint32_t base = (uint32_t)bj.moff[m], len = bj.mlen[m], bs = jb.block_syms;
+    const uint32_t base = (uint32_t)bj.moff[m], len = bj.pstart + bj.mlen[m], bs = jb.block_syms;
     const uint8_t *d = jb.in + base;
     const uint32_t *M = jb.M + base, *nxt = jb.nxt + base;
     Sym *syms = jb.syms + base;
     uint32_t n = 0;
-    for (uint32_t p = 0; p < len;) {
+    for (uint32_t p = bj.pstart; p < len;) {
         const uint32_t v = M[p], nlit = v >> 24;
         for (uint32_t i = 0; i < nlit; i++) syms[n++] = Sym{0, d[p + i], p + i};
         if (v & 0x8000u) syms[n++] = Sym{(uint16_t)((v & 0x7fffu) + 1u), (uint16_t)((v >> 16) & 0xffu), p + nlit};
@@ -120,7 +152,7 @@ __global__ void __launch_bounds__(256) k_bgzf_size(JobBufs jb, BgzfJob bj)
     if (stored) { payload = stored_payload(len); nb = (uint32_t)stored_blocks(len); } // one block for a BGZF member
     atomicAdd(&bj.ctl->n_blocks, nb);
     bj.mstored[m] = stored;
-    bj.mbytes[m] = member_header_len(bj.wrap) + (uint32_t)payload + member_trailer_len(bj.wrap);
+    bj.mbytes[m] = member_header_len(bj.wrap, bj.fdict) + (uint32_t)payload + member_trailer_len(bj.wrap);
 }
 
 // One CTA: the members' offsets in the output (exclusive scan of their lengths), the blocks' absolute bit positions, the output
@@ -142,7 +174,7 @@ __global__ void __launch_bounds__(1024) k_bgzf_scan(JobBufs jb, BgzfJob bj)
         __syncthreads();
     }
     uint64_t off = part[tid] - s;
-    const uint32_t hl = member_header_len(bj.wrap);
+    const uint32_t hl = member_header_len(bj.wrap, bj.fdict);
     for (uint32_t i = beg; i < end; i++) {
         bj.mout[i] = off;
         if (!bj.mstored[i]) {
@@ -155,7 +187,7 @@ __global__ void __launch_bounds__(1024) k_bgzf_scan(JobBufs jb, BgzfJob bj)
     if (tid == 0) bj.ctl->data_type = (n && !bj.mstored[0] && jb.blocks[0].sym_count) ? jb.blocks[0].data_type : 2u;
 }
 
-// One CTA per member: header (BGZF's with BSIZE, or the item's zlib / gzip header), trailer, and the stored blocks of a member
+// One CTA per member: header (BGZF's with BSIZE, or the item's zlib / gzip header, with FDICT and DICTID behind a dictionary), trailer, and the stored blocks of a member
 // written stored; with BGZF the last CTA writes the end-of-file member.  Runs behind k_bgzf_encode (the payload bits are OR-ed
 // into the zeroed output).
 __global__ void __launch_bounds__(256) k_bgzf_frame(JobBufs jb, BgzfJob bj)
@@ -167,18 +199,19 @@ __global__ void __launch_bounds__(256) k_bgzf_frame(JobBufs jb, BgzfJob bj)
         return;
     }
     uint8_t *o = jb.out + bj.mout[m];
-    const uint32_t len = bj.mlen[m], bytes = bj.mbytes[m], hl = member_header_len(bj.wrap);
+    const uint32_t len = bj.mlen[m], bytes = bj.mbytes[m], hl = member_header_len(bj.wrap, bj.fdict);
     const bool stored = bj.mstored[m] != 0;
     if (tid == 0) {
         if (bj.wrap == kWrapBgzf) bgzf_header(o, bytes);
-        else stream_header(o, bj.wrap, zlib_level_flags(jb.level, false), 7, gzip_xfl((int)jb.level, 0));
+        else stream_header(o, bj.wrap, zlib_level_flags(jb.level, false), 7, gzip_xfl((int)jb.level, 0), bj.fdict != 0,
+                           bj.fdict ? *bj.dictid : 0u);
         const uint32_t tw = bj.wrap == kWrapBgzf ? 2u : bj.wrap; // BGZF's trailer is gzip's
         stream_trailer(o + bytes - member_trailer_len(bj.wrap), tw, bj.mcheck[m], len);
     }
     if (stored) {
         const uint32_t nb = (uint32_t)stored_blocks(len);
         if (tid < nb) stored_header(o + hl + tid * (kStoredMax + 5), min(kStoredMax, len - tid * kStoredMax), tid + 1 == nb);
-        const uint8_t *src = jb.in + bj.moff[m];
+        const uint8_t *src = jb.in + bj.moff[m] + bj.pstart; // the item's bytes only
         for (uint32_t i = tid; i < len; i += 256) o[hl + 5 * (i / kStoredMax + 1) + i] = src[i];
     }
 }

@@ -3,7 +3,7 @@
 //
 // Like zb_members.h this is `__host__ __device__`: the kernels of zb_bgzf.cu follow these rules, and tests/bgzfmodel and
 // tests/batchmodel compile the same source, so the CPU tests check the member-relative parse against the oracle and the framing
-// against Python's gzip and zlib.
+// against Python's gzip and zlib; tests/batchdictmodel does the same for batches with a preset dictionary.
 //
 // BGZF.  The input is cut into blocks of kBgzfBlock bytes (htslib's BGZF_BLOCK_SIZE; the last may be shorter, an empty input has
 // none).  Block m becomes one gzip member: the 18-byte header below, the raw deflate stream the reference writes for that block
@@ -18,8 +18,15 @@
 // the reference), and level 0 cuts stored blocks at 65535 bytes as the single-stream writer does (stored_blocks in zb_core.h), so a
 // 65536-byte item has two.  The items' streams are packed back to back in input order.
 //
+// Batch with a preset dictionary (zb_deflate_batch_dict, DESIGN.md §2j).  Item i becomes what the reference writes after
+// deflateSetDictionary(dict): the single-stream rule of a dictionary (Engine::deflate) applied to every member.  The window holds
+// D' bytes of the dictionary (all of it, or its last 32 KiB when it is 64 KiB or longer, deflate.rs:517-531), so member m is staged
+// as D' ++ item and its parse starts at the parse start D' (BgzfJob::pstart, one value per call).  A zlib item gets the 6-byte
+// header with FDICT and DICTID (adler32 of the whole dictionary) whenever D' > 0; its trailer and checks[i] cover the item alone.
+// Level 0 writes stored blocks of the item bytes only (a dictionary does not enter stored blocks).
+//
 // Staging.  Member m is staged at moff[m] of the engine's input buffer with at least kMemberGap zero bytes behind it: BGZF at
-// m * kBgzfStride, a batch packed by batch_stage_next().  The link kernels of the single-stream path run over the whole staged
+// m * kBgzfStride, a batch packed by batch_stage_next() (with a dictionary, the member is its dictionary copy and the item).  The link kernels of the single-stream path run over the whole staged
 // buffer unchanged, as if it were one stream; BgzfAcc then reads member m in its own coordinates.  That is exact whatever lies
 // in front of or behind the member:
 //   - a link is the nearest earlier position with the same hash.  If that position lies in front of the member's start, no
@@ -27,8 +34,14 @@
 //   - the hash of a position whose `need` bytes reach past the member's end reads bytes that are not the member's: no link, as a
 //     one-shot input of that length never inserts it;
 //   - bytes behind the member are never read from the staged buffer (BgzfAcc::byte gives the reference's window contents);
-//     only the 16-byte refills of the level-1/2 input ring (RingAcc, zb_serial.h) load them, and read the zero gap.
-// The symbols, M and nxt entries of member m live at the same offset moff[m] of their buffers (at most one per input byte).
+//     only the 16-byte refills of the level-1/2 input ring (RingAcc, zb_serial.h) load them, and read the zero gap;
+//   - with a dictionary the member's coordinates include its own dictionary copy: a link into [0, D') is the one the window of
+//     the item alone has, as in the single stream with a dictionary, and a link farther back leaves the member and is cut as
+//     above.  What deflateSetDictionary leaves in the hash table beyond the positions' own links is the one stale head entry of
+//     the single-stream case (k_links_dict_ghost): k_batch_dict_ghost restates it per member, looking for the first position
+//     of its bucket among the member's own positions only (the next member's dictionary copy follows the gap).
+// The symbols, M and nxt entries of member m live at the same offset moff[m] of their buffers (at most one per input byte: the
+// parse writes its symbols from syms[moff[m]] and its steps at the item's own positions).
 #pragma once
 #include "zb_core.h"
 
@@ -50,7 +63,7 @@ constexpr uint32_t kWrapBgzf = 3;            // BgzfJob::wrap of a BGZF file; 0 
 
 // batch limits (zb_deflate_batch): staged offsets and symbol indices are 32-bit
 constexpr uint64_t kBatchMaxItems = 65535;
-constexpr uint64_t kBatchMaxBytes = 1ull << 31;
+constexpr uint64_t kBatchMaxBytes = 1ull << 31;   // input bytes; with a dictionary the staged bytes (dictionary copies included)
 constexpr uint64_t kBatchMaxInflateItems = 1ull << 20;
 
 ZB_HD uint64_t bgzf_members(uint64_t n) { return (n + kBgzfBlock - 1) / kBgzfBlock; }
@@ -81,21 +94,23 @@ ZB_HD uint8_t bgzf_eof(uint32_t i)
 }
 
 // Framing of a member: BGZF (the trailer is gzip's), or the stream of a batch item.
-ZB_HD uint32_t member_header_len(uint32_t wrap) { return wrap == kWrapBgzf ? kBgzfHeader : stream_header_len(wrap); }
+ZB_HD uint32_t member_header_len(uint32_t wrap, bool fdict = false) { return wrap == kWrapBgzf ? kBgzfHeader : stream_header_len(wrap, fdict); }
 ZB_HD uint32_t member_trailer_len(uint32_t wrap) { return wrap == kWrapBgzf ? kBgzfTrailer : stream_trailer_len(wrap); }
 
 // Where batch item i is staged: each item at a 64-byte aligned offset with at least kMemberGap zero bytes behind it.  off(0) = 0;
-// off(i + 1) = batch_stage_next(off(i), len(i)).
+// off(i + 1) = batch_stage_next(off(i), D' + len(i)), D' = 0 without a dictionary.
 ZB_HD uint64_t batch_stage_next(uint64_t off, uint64_t len) { return (off + len + kMemberGap + 63) & ~63ull; }
 // Largest stream zb_deflate writes for n bytes (zb_deflate_bound; zb_deflate_batch_bound is the sum over the items): the
 // conservative bound of the reference (deflate.rs:3193-3205: n + (n+7)/8 + (n+63)/64 + 5 + wrapper).  deflate_quick has no stored
 // fallback and codes a literal in up to 9 bits (deflate_quick_overhead, :3169-3176); every other path of the engine stays below
-// stored + framing, which this covers for every memLevel.
+// stored + framing, which this covers for every memLevel.  With a dictionary the zlib header grows by the 4 bytes of DICTID: the 18 +
+// 64 bytes of slack beyond stored + 6 + 4 still cover it, so zb_deflate_batch_bound bounds zb_deflate_batch_dict too.
 ZB_HD uint64_t stream_bound(uint64_t n) { return n + ((n + 7) >> 3) + ((n + 63) >> 6) + 5 + 18 + 64; }
 
 // Member m of a staged input, in its own coordinates: position y reads in[moff[m] + y].  Behind the member's `n` bytes it
 // reads what the reference's window buffer holds behind a one-shot input of n bytes (zeros up to 64 KiB, then the bytes one window
-// earlier, cf. GAcc: a member of kMemberMax bytes slides the window once), so it never reads the staged buffer behind the member.
+// earlier, cf. GAcc: the rule holds for any n, and a member with a dictionary has n = D' + len < 2 * kMemberMax), so it never reads
+// the staged buffer behind the member.
 // A link that reaches farther back than y crosses the member's start: "no link".  `need` is the span of the hash (4 bytes, 3 for
 // the rolling hash of level 9): a position whose hash reaches past the end has no link.  Every position counts as inserted:
 // serial_medium keeps its own bitmap, and deflate_slow inserts every position.

@@ -54,16 +54,21 @@ ZB_HD uint32_t zlib_level_flags(uint32_t level, bool plain_strategy)
 }
 // gzip XFL (deflate.rs:2574-2599)
 ZB_HD uint32_t gzip_xfl(int level, int strategy) { return level == 9 ? 2u : (strategy >= 2 || level < 2) ? 4u : 0u; }
-ZB_HD uint32_t stream_header_len(uint32_t wrap) { return wrap == 1 ? 2u : wrap == 2 ? 10u : 0u; }
+// fdict: a zlib header with FDICT and DICTID (6 bytes), written behind a preset dictionary (deflate.rs:1572-1587, 2747-2753)
+ZB_HD uint32_t stream_header_len(uint32_t wrap, bool fdict = false) { return wrap == 1 ? (fdict ? 6u : 2u) : wrap == 2 ? 10u : 0u; }
 ZB_HD uint32_t stream_trailer_len(uint32_t wrap) { return wrap == 1 ? 4u : wrap == 2 ? 8u : 0u; }
-// zlib: CMF/FLG with the window's CINFO and FCHECK (deflate.rs:1572-1601); gzip: 1f 8b 08 00, MTIME 0, XFL, OS 3 (unix)
-ZB_HD void stream_header(uint8_t *h, uint32_t wrap, uint32_t level_flags, uint32_t cinfo, uint32_t xfl)
+// zlib: CMF/FLG with the window's CINFO and FCHECK (deflate.rs:1572-1601), with fdict the FDICT bit and the big-endian DICTID
+// behind them; gzip: 1f 8b 08 00, MTIME 0, XFL, OS 3 (unix)
+ZB_HD void stream_header(uint8_t *h, uint32_t wrap, uint32_t level_flags, uint32_t cinfo, uint32_t xfl, bool fdict = false,
+                         uint32_t dictid = 0)
 {
     if (wrap == 1) {
-        uint32_t v = ((8u + (cinfo << 4)) << 8) | (level_flags << 6);
+        uint32_t v = ((8u + (cinfo << 4)) << 8) | (level_flags << 6) | (fdict ? 0x20u : 0u);
         v += 31 - (v % 31);
         h[0] = (uint8_t)(v >> 8);
         h[1] = (uint8_t)v;
+        if (fdict)
+            for (int i = 0; i < 4; i++) h[2 + i] = (uint8_t)(dictid >> (24 - 8 * i));
     } else if (wrap == 2) {
         const uint8_t g[10] = {31, 139, 8, 0, 0, 0, 0, 0, (uint8_t)xfl, 3};
         for (int i = 0; i < 10; i++) h[i] = g[i];

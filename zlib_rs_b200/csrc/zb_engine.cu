@@ -72,7 +72,8 @@ __global__ void k_bgzf_size(JobBufs, BgzfJob);
 __global__ void k_bgzf_scan(JobBufs, BgzfJob);
 __global__ void k_bgzf_encode(JobBufs, BgzfJob);
 __global__ void k_bgzf_frame(JobBufs, BgzfJob);
-__global__ void k_batch_stage(const uint8_t *, const uint64_t *, BgzfJob, uint8_t *, uint64_t);
+__global__ void k_batch_stage(const uint8_t *, const uint64_t *, const uint8_t *, BgzfJob, uint8_t *, uint64_t);
+__global__ void k_batch_dict_ghost(JobBufs, BgzfJob);
 
 constexpr uint32_t kMatchSmemBytes = (kWSize + kMatchSub + 512) + (kWSize + kMatchSub) * 2 + ((kWSize + kMatchSub) / 32 + 1) * 4 * 4 + 8192;
 constexpr uint32_t kPathSmemBytes = kPathTile * 4 * 3;
@@ -724,6 +725,9 @@ int Engine::members_reserve(JobBufs &jb, BgzfJob &bj, uint32_t nm, uint32_t S, s
     uint8_t *t = static_cast<uint8_t *>(p);
     bj.nm = nm;
     bj.wrap = wrap;
+    bj.pstart = 0;
+    bj.fdict = 0;
+    bj.dictid = nullptr;
     bj.moff = reinterpret_cast<uint64_t *>(t);
     bj.mout = reinterpret_cast<uint64_t *>(t + m8);
     bj.mlen = reinterpret_cast<uint32_t *>(t + 2 * m8);
@@ -748,6 +752,7 @@ int Engine::members_launch(JobBufs &jb, BgzfJob &bj, int level, uint32_t *d_freq
             } else {
                 k_links2_std<<<nmt, 1024, kLinks2SmemBytes, st>>>(jb, 0);
                 k_links_fix_std<<<S / 256 + 1, 256, 0, st>>>(jb);
+                if (bj.pstart >= 3) { k_batch_dict_ghost<<<nm, 256, 0, st>>>(jb, bj); launches++; } // zb_bgzf.cu
             }
             launches += 2;
         }
@@ -853,24 +858,39 @@ int Engine::deflate_bgzf(const void *src, size_t n, bool src_dev, void *dst, siz
 // zb_deflate_batch (zb_bgzf.h, DESIGN.md §2i): item i is deflated alone and framed as its own zlib / gzip / raw stream, byte for
 // byte what zb_deflate gives for it.  The items are packed into the staged buffer by the host's member table and go through the
 // member core of BGZF; a call costs a fixed number of launches and two host syncs whatever the number and lengths of its items.
-int Engine::deflate_batch(const void *src, const uint64_t *src_off, size_t n_items, bool src_dev, void *dst, size_t dst_cap, bool dst_dev,
-                          int level, int strategy, int window_bits, uint32_t flags, uint64_t *dst_off, uint32_t *checks,
-                          zb_deflate_result *res)
+// With a preset dictionary (zb_deflate_batch_dict, DESIGN.md §2j) every item is staged behind its own copy of the dictionary's
+// window bytes and parsed from there: item i is what deflateSetDictionary(dict) + deflate(Z_FINISH) writes for it.  `dict` is
+// nullptr for zb_deflate_batch.
+int Engine::deflate_batch(const void *dict, size_t dict_len, const void *src, const uint64_t *src_off, size_t n_items, bool src_dev,
+                          void *dst, size_t dst_cap, bool dst_dev, int level, int strategy, int window_bits, uint32_t flags,
+                          uint64_t *dst_off, uint32_t *checks, zb_deflate_result *res)
 {
     if (!res || !dst_off || (n_items && (!src_off || !dst))) { snprintf(g_err, sizeof g_err, "deflate_batch: null argument"); return ZB_E_PARAM; }
     memset(res, 0, sizeof *res);
+    const bool with_dict = dict != nullptr || dict_len != 0;
     const uint32_t ml = (flags >> 8) & 15u;
     uint32_t wrap;
     if (window_bits == 15) wrap = 1;
-    else if (window_bits == 31) wrap = 2;
+    else if (window_bits == 31 && !with_dict) wrap = 2;
     else if (window_bits == -15) wrap = 0;
+    else if (window_bits == 31) { snprintf(g_err, sizeof g_err, "deflate_batch_dict: a gzip stream takes no dictionary"); return ZB_E_PARAM; }
     else { snprintf(g_err, sizeof g_err, "deflate_batch takes window_bits 15, -15 or 31"); return ZB_E_PARAM; }
     if ((flags & ~ZB_FLAG_MEMLEVEL(15)) || (ml && ml != 8) || strategy != 0 || level < -1 || level > 9) {
         snprintf(g_err, sizeof g_err, "deflate_batch takes Z_DEFAULT_STRATEGY, level -1..9, memLevel 8 and no flag");
         return ZB_E_PARAM;
     }
+    if (with_dict && (level == 1 || level == 2)) {
+        // the one-warp parsers of levels 1/2 take no dictionary (zb_deflate_dict runs the level-3 kernels there, not the reference's
+        // bytes); a batch returns the reference's bytes or nothing
+        snprintf(g_err, sizeof g_err, "deflate_batch_dict: levels 1 and 2 have no exact parser with a dictionary (use 0 or 3..9)");
+        return ZB_E_PARAM;
+    }
+    if (with_dict && !dict) { snprintf(g_err, sizeof g_err, "deflate_batch_dict: null dictionary of %zu bytes", dict_len); return ZB_E_PARAM; }
+    if (dict_len > 0xffffffffull) { snprintf(g_err, sizeof g_err, "deflate_batch_dict: dictionary of 4 GiB or more"); return ZB_E_PARAM; }
+    // the window's part of the dictionary (deflate.rs:517-531): all of it, or its last w_size bytes when it would fill the window
+    const uint32_t D = dict_len >= 2 * (size_t)kWSize ? kWSize : (uint32_t)dict_len;
     if (n_items > kBatchMaxItems) { snprintf(g_err, sizeof g_err, "deflate_batch: %zu items (at most %llu)", n_items, (unsigned long long)kBatchMaxItems); return ZB_E_PARAM; }
-    // the member table, on the host: items at 64-byte aligned staged offsets with a zero gap behind each
+    // the member table, on the host: items at 64-byte aligned staged offsets, each behind its dictionary copy, with a zero gap behind
     const uint32_t nm = (uint32_t)n_items;
     uint64_t span = 0, bound = 0;
     for (uint32_t i = 0; i < nm; i++) {
@@ -878,11 +898,15 @@ int Engine::deflate_batch(const void *src, const uint64_t *src_off, size_t n_ite
             snprintf(g_err, sizeof g_err, "deflate_batch: item %u is not 0..%u bytes", i, kMemberMax);
             return ZB_E_PARAM;
         }
-        span = batch_stage_next(span, src_off[i + 1] - src_off[i]);
+        span = batch_stage_next(span, D + (src_off[i + 1] - src_off[i]));
         bound += stream_bound(src_off[i + 1] - src_off[i]);
     }
     const uint64_t total = nm ? src_off[nm] - src_off[0] : 0;
     if (total > kBatchMaxBytes) { snprintf(g_err, sizeof g_err, "deflate_batch: %llu bytes in all (at most 2^31)", (unsigned long long)total); return ZB_E_PARAM; }
+    if (D && span > kBatchMaxBytes) {
+        snprintf(g_err, sizeof g_err, "deflate_batch_dict: %llu staged bytes with the dictionary copies (at most 2^31)", (unsigned long long)span);
+        return ZB_E_PARAM;
+    }
     if (total && !src) { snprintf(g_err, sizeof g_err, "deflate_batch: null source"); return ZB_E_PARAM; }
     if (level == -1) level = 6;
     res->exact_parity = 1;
@@ -898,13 +922,17 @@ int Engine::deflate_batch(const void *src, const uint64_t *src_off, size_t n_ite
     uint32_t *d_freq;
     int rc;
     if ((rc = members_reserve(jb, bj, nm, S, span, level, out_cap, wrap, &d_freq)) != ZB_OK) return rc;
-    // pinned staging: the member table up (moff | mlen | src_off), the control block, offsets and checks down
-    const size_t t_up = (size_t)nm * 8 + (size_t)nm * 4 + ((size_t)nm + 1) * 8, t_down = sizeof(BgzfCtl) + (size_t)nm * 12 + 16;
+    bj.pstart = D;
+    bj.fdict = wrap == 1 && D > 0; // FDICT whenever the dictionary put bytes in the window (deflate.rs:1578-1581)
+    // pinned staging: the member table up (moff | mlen | src_off | the dictionary's offset and length for its adler32), the control
+    // block, offsets and checks down
+    const size_t t_up = (size_t)nm * 8 + (size_t)nm * 4 + ((size_t)nm + 1) * 8 + 16, t_down = sizeof(BgzfCtl) + (size_t)nm * 12 + 16;
     if ((rc = stage(t_up + t_down + 64)) != ZB_OK) return rc;
     uint8_t *h = static_cast<uint8_t *>(h_stage);
     uint64_t *h_moff = reinterpret_cast<uint64_t *>(h);
     uint32_t *h_mlen = reinterpret_cast<uint32_t *>(h + (size_t)nm * 8);
     uint64_t *h_soff = reinterpret_cast<uint64_t *>(h + (size_t)nm * 12);
+    uint64_t *h_dseg = h_soff + nm + 1; // offset 0, then the dictionary's length
     BgzfCtl *h_ctl = reinterpret_cast<BgzfCtl *>(h + ((t_up + 15) & ~(size_t)15));
     uint64_t *h_mout = reinterpret_cast<uint64_t *>(h_ctl + 1);
     uint32_t *h_chk = reinterpret_cast<uint32_t *>(h_mout + nm);
@@ -912,32 +940,50 @@ int Engine::deflate_batch(const void *src, const uint64_t *src_off, size_t n_ite
     for (uint32_t i = 0; i < nm; i++) {
         h_moff[i] = off;
         h_mlen[i] = (uint32_t)(src_off[i + 1] - src_off[i]);
-        off = batch_stage_next(off, h_mlen[i]);
+        off = batch_stage_next(off, D + h_mlen[i]);
     }
     memcpy(h_soff, src_off, ((size_t)nm + 1) * 8);
+    h_dseg[0] = 0;
+    h_dseg[1] = dict_len;
+    // S_BATCH: the caller's offsets | the dictionary segment (offset, length, its adler32) | a host dictionary | a host source
+    const size_t a_soff = ((((size_t)nm + 1) * 8 + 63) & ~(size_t)63), a_dseg = 64;
+    const size_t a_dict = src_dev ? 0 : ((dict_len + 63) & ~(size_t)63);
     void *p;
-    if ((rc = reserve(S_BATCH, ((size_t)nm + 1) * 8 + 64 + (src_dev ? 0 : total), &p)) != ZB_OK) return rc;
-    uint64_t *d_soff = static_cast<uint64_t *>(p);
-    const uint8_t *d_src = src_dev ? static_cast<const uint8_t *>(src) + src_off[0]
-                                   : static_cast<const uint8_t *>(p) + ((((size_t)nm + 1) * 8 + 63) & ~(size_t)63);
+    if ((rc = reserve(S_BATCH, a_soff + a_dseg + a_dict + (src_dev ? 0 : total), &p)) != ZB_OK) return rc;
+    uint8_t *t = static_cast<uint8_t *>(p);
+    uint64_t *d_soff = reinterpret_cast<uint64_t *>(t);
+    uint64_t *d_dseg = reinterpret_cast<uint64_t *>(t + a_soff);
+    uint32_t *d_dictid = reinterpret_cast<uint32_t *>(t + a_soff + 32);
+    const uint8_t *d_dict = src_dev ? static_cast<const uint8_t *>(dict) : t + a_soff + a_dseg;
+    const uint8_t *d_src = src_dev ? static_cast<const uint8_t *>(src) + src_off[0] : t + a_soff + a_dseg + a_dict;
     const size_t mi_bytes = ((size_t)nm * sizeof(JobInfo) + 15) & ~(size_t)15;
+    bj.dictid = d_dictid;
 
     CK(cudaEventRecord(ev0, st));
     CK(cudaMemcpyAsync(bj.moff, h_moff, (size_t)nm * 8, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(bj.mlen, h_mlen, (size_t)nm * 4, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_soff, h_soff, ((size_t)nm + 1) * 8, cudaMemcpyHostToDevice, st));
-    // staging: one contiguous copy of a host source, then every item to its staged offset with the gap behind it zeroed
+    if (bj.fdict) CK(cudaMemcpyAsync(d_dseg, h_dseg, 16, cudaMemcpyHostToDevice, st));
+    // staging: one contiguous copy of a host source (and dictionary), then every item to its staged offset behind its dictionary copy,
+    // with the gap behind it zeroed
+    if (!src_dev && dict_len) CK(cudaMemcpyAsync(const_cast<uint8_t *>(d_dict), dict, dict_len, cudaMemcpyHostToDevice, st));
     if (!src_dev && total) CK(cudaMemcpyAsync(const_cast<uint8_t *>(d_src), static_cast<const uint8_t *>(src) + src_off[0], total, cudaMemcpyHostToDevice, st));
-    k_batch_stage<<<nm, 256, 0, st>>>(d_src, d_soff, bj, const_cast<uint8_t *>(jb.in), span);
+    k_batch_stage<<<nm, 256, 0, st>>>(d_src, d_soff, D ? d_dict + (dict_len - D) : nullptr, bj, const_cast<uint8_t *>(jb.in), span);
     CK(cudaMemsetAsync(const_cast<uint8_t *>(jb.in) + span, 0, kPad + 16, st));
     CK(cudaMemsetAsync(bj.minfo, 0, mi_bytes + sizeof(BgzfCtl), st));
     CK(cudaMemsetAsync(jb.out, 0, out_cap, st));
     launches++;
-    // the items' checks, as zb_deflate returns them
-    if (wrap == 1) CK(launch_adler32_segments(jb.in, bj.moff, bj.mlen, nm, bj.mcheck, st));
+    // the items' checks, as zb_deflate returns them (the item's bytes only, behind its dictionary copy), and DICTID: the adler32 of
+    // the whole dictionary as passed (deflate.rs:507-510)
+    if (wrap == 1) CK(launch_adler32_segments(jb.in + D, bj.moff, bj.mlen, nm, bj.mcheck, st));
     else if (wrap == 2) CK(launch_crc32_segments(jb.in, bj.moff, bj.mlen, nm, bj.mcheck, st));
     else CK(cudaMemsetAsync(bj.mcheck, 0, (size_t)nm * 4, st));
     if (wrap) launches++;
+    if (bj.fdict) {
+        // one segment: [0, dict_len) of the dictionary, its length as a 32-bit word (the low half of h_dseg[1], little-endian)
+        CK(launch_adler32_segments(d_dict, d_dseg, reinterpret_cast<const uint32_t *>(d_dseg + 1), 1, d_dictid, st));
+        launches++;
+    }
     if ((rc = members_launch(jb, bj, level, d_freq)) != ZB_OK) return rc;
     CK(cudaMemcpyAsync(h_ctl, bj.ctl, sizeof(BgzfCtl), cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(h_mout, bj.mout, (size_t)nm * 8, cudaMemcpyDeviceToHost, st));
@@ -1061,14 +1107,27 @@ size_t zb_deflate_bound(size_t n) { return zb::deflate_bound(n); }
 
 size_t zb_bgzf_bound(size_t n) { return (size_t)zb::bgzf_bound(n); }
 
+int zb_deflate_batch_dict(zb_engine *z, const void *dict, size_t dict_len, const void *src, const uint64_t *src_off, size_t n_items,
+                          int src_dev, void *dst, size_t cap, int dst_dev, int level, int strategy, int window_bits, uint32_t flags,
+                          uint64_t *dst_off, uint32_t *checks, zb_deflate_result *res)
+{
+    if (!z) return ZB_E_NODEVICE;
+    if (!dict && dict_len) { snprintf(zb::g_err, sizeof zb::g_err, "deflate_batch_dict: null dictionary of %zu bytes", dict_len); return ZB_E_PARAM; }
+    z->e.shard.phase = 0; // a range job in progress is gone (its buffers are reused)
+    // an empty dictionary still makes this the dictionary call (its rules on levels and framing), with the bytes of zb_deflate_batch
+    static const uint8_t none = 0;
+    return z->e.deflate_batch(dict ? dict : &none, dict_len, src, src_off, n_items, src_dev != 0, dst, cap, dst_dev != 0, level, strategy,
+                              window_bits, flags, dst_off, checks, res);
+}
+
 int zb_deflate_batch(zb_engine *z, const void *src, const uint64_t *src_off, size_t n_items, int src_dev, void *dst, size_t cap,
                      int dst_dev, int level, int strategy, int window_bits, uint32_t flags, uint64_t *dst_off, uint32_t *checks,
                      zb_deflate_result *res)
 {
     if (!z) return ZB_E_NODEVICE;
     z->e.shard.phase = 0; // a range job in progress is gone (its buffers are reused)
-    return z->e.deflate_batch(src, src_off, n_items, src_dev != 0, dst, cap, dst_dev != 0, level, strategy, window_bits, flags, dst_off,
-                              checks, res);
+    return z->e.deflate_batch(nullptr, 0, src, src_off, n_items, src_dev != 0, dst, cap, dst_dev != 0, level, strategy, window_bits, flags,
+                              dst_off, checks, res);
 }
 
 size_t zb_deflate_batch_bound(const uint64_t *src_off, size_t n_items)
@@ -1078,12 +1137,23 @@ size_t zb_deflate_batch_bound(const uint64_t *src_off, size_t n_items)
     return b;
 }
 
+int zb_inflate_batch_dict(zb_engine *z, const void *dict, size_t dict_len, const void *src, const uint64_t *src_off, size_t n_items,
+                          int src_dev, void *dst, const uint64_t *dst_off, int dst_dev, int window_bits, zb_inflate_result *items)
+{
+    if (!z) return ZB_E_NODEVICE;
+    if (!dict && dict_len) { snprintf(zb::g_err, sizeof zb::g_err, "inflate_batch_dict: null dictionary of %zu bytes", dict_len); return ZB_E_PARAM; }
+    z->e.shard.phase = 0; // a range job in progress is gone (its buffers are reused)
+    static const uint8_t none = 0; // an empty dictionary (id 1) is still a dictionary
+    return z->e.inflate_batch(dict ? dict : &none, dict_len, src, src_off, n_items, src_dev != 0, dst, dst_off, dst_dev != 0, window_bits,
+                              items);
+}
+
 int zb_inflate_batch(zb_engine *z, const void *src, const uint64_t *src_off, size_t n_items, int src_dev, void *dst, const uint64_t *dst_off,
                      int dst_dev, int window_bits, zb_inflate_result *items)
 {
     if (!z) return ZB_E_NODEVICE;
     z->e.shard.phase = 0; // a range job in progress is gone (its buffers are reused)
-    return z->e.inflate_batch(src, src_off, n_items, src_dev != 0, dst, dst_off, dst_dev != 0, window_bits, items);
+    return z->e.inflate_batch(nullptr, 0, src, src_off, n_items, src_dev != 0, dst, dst_off, dst_dev != 0, window_bits, items);
 }
 
 int zb_inflate(zb_engine *z, const void *src, size_t n, int src_dev, void *dst, size_t cap, int dst_dev, int window_bits,

@@ -68,8 +68,9 @@ struct Engine {
     int deflate(const void *src, size_t n, bool src_dev, void *dst, size_t dst_cap, bool dst_dev, int level, int strategy,
                 int window_bits, uint32_t flags, zb_deflate_result *res, const void *dict = nullptr, size_t dict_len = 0);
     int deflate_bgzf(const void *src, size_t n, bool src_dev, void *dst, size_t dst_cap, bool dst_dev, int level, zb_deflate_result *res);
-    int deflate_batch(const void *src, const uint64_t *src_off, size_t n_items, bool src_dev, void *dst, size_t dst_cap, bool dst_dev,
-                      int level, int strategy, int window_bits, uint32_t flags, uint64_t *dst_off, uint32_t *checks, zb_deflate_result *res);
+    int deflate_batch(const void *dict, size_t dict_len, const void *src, const uint64_t *src_off, size_t n_items, bool src_dev, void *dst,
+                      size_t dst_cap, bool dst_dev, int level, int strategy, int window_bits, uint32_t flags, uint64_t *dst_off,
+                      uint32_t *checks, zb_deflate_result *res);
     int members_reserve(JobBufs &jb, BgzfJob &bj, uint32_t nm, uint32_t S, size_t span, int level, size_t out_cap, uint32_t wrap,
                         uint32_t **d_freq);
     int members_launch(JobBufs &jb, BgzfJob &bj, int level, uint32_t *d_freq);
@@ -78,8 +79,8 @@ struct Engine {
     int inflate_stream(const uint8_t *d_src, size_t n, uint8_t *d_dst, size_t dst_cap, int window_bits, uint32_t flags,
                        zb_inflate_result *res);
     int inflate_members(const uint8_t *d_src, size_t n, uint8_t *d_dst, size_t dst_cap, int window_bits, zb_inflate_result *res);
-    int inflate_batch(const void *src, const uint64_t *src_off, size_t n_items, bool src_dev, void *dst, const uint64_t *dst_off,
-                      bool dst_dev, int window_bits, zb_inflate_result *items);
+    int inflate_batch(const void *dict, size_t dict_len, const void *src, const uint64_t *src_off, size_t n_items, bool src_dev, void *dst,
+                      const uint64_t *dst_off, bool dst_dev, int window_bits, zb_inflate_result *items);
     int inflate_blocks(const void *src, size_t n, uint64_t start_bit, const void *dict, size_t dict_len, void *dst, size_t dst_cap,
                        int check_kind, uint32_t check_start, zb_inflate_seg *out);
     int checksum(bool crc, uint32_t start, const void *buf, size_t len, bool on_dev, uint32_t *out, float *ms);

@@ -52,6 +52,15 @@ struct InfSeg {
     uint32_t dict_len;
     uint32_t on; // 0: whole stream with header and trailer (one-shot)
 };
+// A one-shot stream with a preset dictionary (zb_inflate_batch_dict): `win` holds the last `len` (<= 32 KiB) bytes of the dictionary
+// and *id its adler32.  A raw stream decodes with them as its window, a zlib stream whose FDICT header names *id too
+// (inflateSetDictionary, inflate.rs:2605-2640); any other stream decodes as without it.
+struct InfDict {
+    const uint8_t *win;
+    const uint32_t *id;
+    uint32_t len;
+    uint32_t on;
+};
 
 __device__ static const uint16_t d_lbase[31] = {3, 4, 5, 6, 7, 8, 9, 10, 11, 13, 15, 17, 19, 23, 27, 31, 35, 43, 51, 59, 67, 83, 99, 115, 131, 163, 195, 227, 258, 0, 0};
 __device__ static const uint8_t d_lext[31] = {16, 16, 16, 16, 16, 16, 16, 16, 17, 17, 17, 17, 18, 18, 18, 18, 19, 19, 19, 19, 20, 20, 20, 20, 21, 21, 21, 21, 16, 77, 202};
@@ -141,7 +150,7 @@ enum Cmd { C_NONE = 0, C_REFILL, C_FLUSH, C_COPY, C_DONE };
 // The one-warp decoder: a whole stream (header, blocks, trailer) or, in segment mode, raw blocks from a bit position.  Output goes to
 // dst[0, cap) only.  k_inflate runs it on one stream, k_members on one gzip member per warp.
 __device__ __forceinline__ void inflate_warp(InfShared &S, const uint8_t *__restrict__ src, uint64_t n, uint8_t *__restrict__ dst,
-                                             uint64_t cap, int window_bits, InfState *res, InfSeg seg)
+                                             uint64_t cap, int window_bits, InfState *res, InfSeg seg, InfDict pd = InfDict{nullptr, nullptr, 0, 0})
 {
     const uint32_t lane = threadIdx.x;
     // shared between lanes through shuffles from lane 0
@@ -161,8 +170,10 @@ __device__ __forceinline__ void inflate_warp(InfShared &S, const uint8_t *__rest
     uint32_t copy_len = 0, copy_dist = 0;
     uint32_t gz_fl = 0, gz_xl = 0;
 
-    // segment mode: the window in front of the segment occupies ring positions [0, D0); output position D0 + i is dst[i]
-    const uint64_t D0 = seg.on ? seg.dict_len : 0;
+    // segment mode: the window in front of the segment occupies ring positions [0, D0); output position D0 + i is dst[i].  A preset
+    // dictionary is loaded there too: D0 is its length from the start for a raw stream, from the end of the header for a zlib stream
+    // that asks for it (lane 0 sets it, the others take it with the next command), and stays 0 for any other stream.
+    uint64_t D0 = seg.on ? seg.dict_len : 0;
     uint64_t blk_bit = seg.start_bit, blk_out = D0;
     uint32_t final_done = 0, stored_wait = 0;
     if (seg.on) {
@@ -175,6 +186,11 @@ __device__ __forceinline__ void inflate_warp(InfShared &S, const uint8_t *__rest
         mode = 1;
         kind = 0;
     }
+    if (pd.on) {
+        for (uint32_t i = lane; i < pd.len; i += 32) S.out[i] = pd.win[i];
+        if (window_bits < 0) { D0 = pd.len; oflush = opos = blk_out = D0; }
+    }
+    const uint32_t dict_id = pd.on ? *pd.id : 0u;
     if (lane == 0) {
         uint32_t root;
         uint32_t sym = 0;
@@ -233,7 +249,17 @@ __device__ __forceinline__ void inflate_warp(InfShared &S, const uint8_t *__rest
                     const uint32_t wb = ((h >> 4) & 0xf) + 8;
                     const uint32_t want = (uint32_t)(window_bits & 15);
                     if (wb > 15 || (want != 0 && wb > want)) { FAIL(IE_WINDOW); continue; }
-                    if (h & 0x2000) { FAIL(IE_NEED_DICT); continue; }
+                    if (h & 0x2000) { // FDICT: DICTID follows, big-endian (inflate.rs:1006-1017)
+                        if (!pd.on) { FAIL(IE_NEED_DICT); continue; }
+                        NEED(48);
+                        if (!REAL(48)) { FAIL(IE_TRUNCATED); continue; }
+                        if (__byte_perm((uint32_t)(hold >> 16), 0, 0x0123) != dict_id) { FAIL(IE_NEED_DICT); continue; }
+                        DROP(48);
+                        D0 = pd.len;
+                        opos = oflush = blk_out = D0; // lane 0's flush trigger counts from here; the other lanes take it with D0
+                        mode = 1;
+                        continue;
+                    }
                     DROP(16);
                     mode = 1;
                     continue;
@@ -395,6 +421,10 @@ __device__ __forceinline__ void inflate_warp(InfShared &S, const uint8_t *__rest
             }
         }
         cmd = __shfl_sync(0xffffffffu, cmd, 0);
+        if (pd.on) { // a zlib header may have just moved the output start behind the dictionary (nothing was flushed yet)
+            D0 = __shfl_sync(0xffffffffu, D0, 0);
+            if (oflush < D0) oflush = D0;
+        }
         if (cmd == C_REFILL) {
             const uint64_t ipos0 = __shfl_sync(0xffffffffu, ipos, 0);
             // fill up to the ring size, never overwriting unread bytes
@@ -1408,13 +1438,13 @@ struct BatchResult {   // what comes back to the host per item
 
 __global__ void __launch_bounds__(32) k_batch_members(const uint8_t *__restrict__ src, const BatchItem *items, uint8_t *__restrict__ dst,
                                                       int window_bits, InfState *ist, uint64_t *out_off, uint32_t *crc_len,
-                                                      uint32_t *adler_len)
+                                                      uint32_t *adler_len, InfDict pd)
 {
     extern __shared__ __align__(16) uint8_t smem_raw[];
     const uint32_t i = blockIdx.x;
     const BatchItem it = items[i];
     inflate_warp(*reinterpret_cast<InfShared *>(smem_raw), src + it.in_off, it.in_len, dst + it.out_off, it.out_cap, window_bits, ist + i,
-                 InfSeg{0, nullptr, 0, 0});
+                 InfSeg{0, nullptr, 0, 0}, pd);
     __syncwarp();
     if (threadIdx.x == 0) {
         // inflate_stream checks what was produced unless the output did not fit; an item's slots hold below 4 GiB (host check)
@@ -1766,11 +1796,14 @@ int Engine::inflate_stream(const uint8_t *d_src, size_t n, uint8_t *d_dst, size_
 }
 
 // zb_inflate_batch: item i of src[src_off[i], src_off[i+1]) into dst[dst_off[i], dst_off[i+1]), each as zb_inflate_ex decodes it
-// alone.  Fixed launches (k_batch_members, the two checksum kernels, k_batch_verdict) and one host sync.
-int Engine::inflate_batch(const void *src, const uint64_t *src_off, size_t n_items, bool src_dev, void *dst, const uint64_t *dst_off,
-                          bool dst_dev, int window_bits, zb_inflate_result *items)
+// alone.  Fixed launches (k_batch_members, the two checksum kernels, k_batch_verdict) and one host sync.  With a preset dictionary
+// (zb_inflate_batch_dict, `dict` not nullptr) one more launch gives its adler32, the id an FDICT header must name; the decoder
+// preloads the dictionary's last 32 KiB as the window of the raw items and of the zlib items that name it.
+int Engine::inflate_batch(const void *dict, size_t dict_len, const void *src, const uint64_t *src_off, size_t n_items, bool src_dev,
+                          void *dst, const uint64_t *dst_off, bool dst_dev, int window_bits, zb_inflate_result *items)
 {
     if (n_items && (!src_off || !dst_off || !items)) { snprintf(g_err, sizeof g_err, "inflate_batch: null argument"); return ZB_E_PARAM; }
+    if (dict_len > 0xffffffffull) { snprintf(g_err, sizeof g_err, "inflate_batch_dict: dictionary of 4 GiB or more"); return ZB_E_PARAM; }
     if (window_bits < 0) { if (window_bits < -15 || window_bits > -8) return ZB_E_PARAM; }
     else if (window_bits != 0 && ((window_bits & 15) < 8)) return ZB_E_PARAM;
     if (window_bits > 47) return ZB_E_PARAM;
@@ -1794,7 +1827,9 @@ int Engine::inflate_batch(const void *src, const uint64_t *src_off, size_t n_ite
     // S_BATCH: item table | results | output offsets | the two checksum length tables and their checks | decoder states
     const size_t a_items = ((size_t)nm * sizeof(BatchItem) + 63) & ~(size_t)63, a_res = ((size_t)nm * sizeof(BatchResult) + 63) & ~(size_t)63;
     const size_t a4 = ((size_t)nm * 4 + 63) & ~(size_t)63, a8 = ((size_t)nm * 8 + 63) & ~(size_t)63;
-    if ((rc = reserve(S_BATCH, a_items + a_res + a8 + 4 * a4 + (size_t)nm * sizeof(InfState), &p)) != ZB_OK) return rc;
+    // ... | the dictionary segment (offset, length, id) | a host dictionary
+    const size_t a_ist = ((size_t)nm * sizeof(InfState) + 63) & ~(size_t)63, a_dict = (dict && !src_dev) ? ((dict_len + 63) & ~(size_t)63) : 0;
+    if ((rc = reserve(S_BATCH, a_items + a_res + a8 + 4 * a4 + a_ist + 64 + a_dict, &p)) != ZB_OK) return rc;
     uint8_t *t = static_cast<uint8_t *>(p);
     BatchItem *d_items = reinterpret_cast<BatchItem *>(t);
     BatchResult *d_res = reinterpret_cast<BatchResult *>(t + a_items);
@@ -1802,9 +1837,15 @@ int Engine::inflate_batch(const void *src, const uint64_t *src_off, size_t n_ite
     uint32_t *d_clen = reinterpret_cast<uint32_t *>(t + a_items + a_res + a8), *d_alen = d_clen + a4 / 4;
     uint32_t *d_crc = d_alen + a4 / 4, *d_adler = d_crc + a4 / 4;
     InfState *d_ist = reinterpret_cast<InfState *>(d_adler + a4 / 4);
-    if ((rc = stage(a_items + a_res + 64)) != ZB_OK) return rc;
+    uint64_t *d_dseg = reinterpret_cast<uint64_t *>(reinterpret_cast<uint8_t *>(d_ist) + a_ist);
+    uint32_t *d_dictid = reinterpret_cast<uint32_t *>(d_dseg + 2);
+    const uint8_t *d_dict = src_dev ? static_cast<const uint8_t *>(dict) : reinterpret_cast<const uint8_t *>(d_dseg) + 64;
+    if ((rc = stage(a_items + a_res + 64 + 16)) != ZB_OK) return rc;
     BatchItem *h_items = static_cast<BatchItem *>(h_stage);
     BatchResult *h_res = reinterpret_cast<BatchResult *>(static_cast<uint8_t *>(h_stage) + a_items);
+    uint64_t *h_dseg = reinterpret_cast<uint64_t *>(static_cast<uint8_t *>(h_stage) + a_items + a_res + 64);
+    h_dseg[0] = 0;
+    h_dseg[1] = dict_len;
     for (uint32_t i = 0; i < nm; i++)
         h_items[i] = BatchItem{src_off[i] - src_off[0], src_off[i + 1] - src_off[i], dst_off[i] - dst_off[0], dst_off[i + 1] - dst_off[i]};
     // the item offsets index the caller's buffers: a host buffer is copied (or staged) as one range
@@ -1822,7 +1863,17 @@ int Engine::inflate_batch(const void *src, const uint64_t *src_off, size_t n_ite
         CKI(cudaMemsetAsync(d_dst, 0, out_total, st)); // the slots go back whole: what lies behind an item's output is zeros
     }
     CKI(cudaMemcpyAsync(d_items, h_items, (size_t)nm * sizeof(BatchItem), cudaMemcpyHostToDevice, st));
-    k_batch_members<<<nm, 32, sizeof(InfShared), st>>>(d_src, d_items, d_dst, window_bits, d_ist, d_ooff, d_clen, d_alen);
+    InfDict pd{nullptr, nullptr, 0, 0};
+    if (dict) {
+        // the dictionary's id: the adler32 of all of it (an empty one has id 1), as inflateSetDictionary checks it
+        CKI(cudaMemcpyAsync(d_dseg, h_dseg, 16, cudaMemcpyHostToDevice, st));
+        if (!src_dev && dict_len) CKI(cudaMemcpyAsync(const_cast<uint8_t *>(d_dict), dict, dict_len, cudaMemcpyHostToDevice, st));
+        CKI(launch_adler32_segments(d_dict, d_dseg, reinterpret_cast<const uint32_t *>(d_dseg + 1), 1, d_dictid, st));
+        launches++;
+        const uint32_t w = dict_len > kWSize ? kWSize : (uint32_t)dict_len; // the window keeps the dictionary's last 32 KiB
+        pd = InfDict{d_dict + (dict_len - w), d_dictid, w, 1};
+    }
+    k_batch_members<<<nm, 32, sizeof(InfShared), st>>>(d_src, d_items, d_dst, window_bits, d_ist, d_ooff, d_clen, d_alen, pd);
     CKI(launch_crc32_segments(d_dst, d_ooff, d_clen, nm, d_crc, st));
     CKI(launch_adler32_segments(d_dst, d_ooff, d_alen, nm, d_adler, st));
     k_batch_verdict<<<(nm + 255) / 256, 256, 0, st>>>(d_ist, d_crc, d_adler, nm, d_res);

@@ -1849,7 +1849,8 @@ __global__ void __launch_bounds__(1024) k_encode(JobBufs jb)
 
 // ------------------------------------------------------------------------------------------------
 // Members of a BGZF file or a batch (zb_bgzf.h, zb_bgzf.cu): the block kernels above over every member at once, one CTA per block
-// slot m * kBgzfMaxBlocks + k.  Positions and symbols are member-relative; in_start and sym_begin point into the staged buffers.
+// slot m * kBgzfMaxBlocks + k.  Positions and symbols are member-relative (a dictionary's bytes included, so block_start and
+// have_window see the window as the single stream with a dictionary does); in_start and sym_begin point into the staged buffers.
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) k_bgzf_hist(JobBufs jb, BgzfJob bj, uint32_t *freq)
 {
@@ -1857,7 +1858,7 @@ __global__ void __launch_bounds__(256) k_bgzf_hist(JobBufs jb, BgzfJob bj, uint3
     const JobInfo &mi = bj.minfo[m];
     const uint32_t nsyms = mi.n_syms, nblocks = mi.n_blocks;
     if (k >= nblocks) return;
-    const uint32_t base = (uint32_t)bj.moff[m], len = bj.mlen[m];
+    const uint32_t base = (uint32_t)bj.moff[m], len = bj.pstart + bj.mlen[m]; // the member's end: dictionary and item
     const Sym *syms = jb.syms + base;
     const uint32_t begin = k * jb.block_syms;
     const uint32_t count = k + 1 < nblocks ? jb.block_syms : nsyms - begin;
@@ -1868,7 +1869,7 @@ __global__ void __launch_bounds__(256) k_bgzf_hist(JobBufs jb, BgzfJob bj, uint3
         bd.sym_begin = base + begin;
         bd.sym_count = count;
         bd.last = last;
-        const uint32_t start = begin == 0 ? 0 : sym_end(syms[begin - 1]);
+        const uint32_t start = begin == 0 ? bj.pstart : sym_end(syms[begin - 1]);
         const uint32_t end = last ? len : sym_end(syms[begin + count - 1]);
         bd.in_start = base + start;
         bd.in_len = end - start;

@@ -138,6 +138,9 @@ struct BgzfJob {
     uint32_t *mstored;  // 1: written as stored blocks (level 0, or a BGZF payload that does not fit 64 KiB)
     JobInfo *minfo;     // n_syms, n_blocks and final_base of its parse, as a single-stream parse reports them
     BgzfCtl *ctl;
+    uint32_t pstart;    // parse start of every member: the dictionary's bytes D' staged in front of each item (0: none)
+    uint32_t fdict;     // zlib items get FDICT and DICTID = *dictid (a batch with a preset dictionary)
+    const uint32_t *dictid;
 };
 
 cudaError_t upload_tables();
