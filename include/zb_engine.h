@@ -217,6 +217,60 @@ typedef struct zb_inflate_seg {
 ZB_API int zb_inflate_blocks(zb_engine *e, const void *src, size_t src_len, uint64_t start_bit, const void *dict, size_t dict_len,
                              void *dst, size_t dst_cap, int check_kind, uint32_t check_start, zb_inflate_seg *out);
 
+/* Random access into deflate, zlib and gzip streams (DESIGN.md §2k).  An index lists access points: bits of the compressed input
+ * where raw-block decoding can resume given the 32 KiB of output in front of them -- a block's header, or the start of a literal or
+ * length symbol inside a fixed-code or dynamic block.  For a span S it holds the first block of every member (window empty) and,
+ * for every k >= 1 with k * S < total output, the first access point in stream order whose offset in the whole output is >= k * S
+ * (once).  The points are a function of the stream and S alone; from any output offset x the last point at or before x lies less
+ * than S + 65535 bytes behind x.  Each point has its window: the min(32768, out_off - member's output start) bytes in front of it.
+ *
+ * zb_index_build: zb_inflate_ex plus an index.  For the same arguments it returns the same code, the same res (gpu_launches and
+ *   gpu_ms aside: they include the index kernels) and the same bytes in dst, every error included; only on ZB_OK it also returns
+ *   the index in *out (else *out = NULL).  flags: those of zb_inflate_ex except ZB_INF_NO_SERIAL (ZB_E_PARAM); with ZB_INF_MEMBERS
+ *   every member is indexed.  span: 32768 <= S <= 2^32, else ZB_E_PARAM.  A stream with a preset dictionary gives "need dictionary".
+ * zb_index_extract: range i is the output bytes [offsets[i], offsets[i] + slot_i) of the indexed stream, slot_i = dst_off[i+1] -
+ *   dst_off[i] (host arrays, n_ranges + 1 offsets into dst); they go to the range's slot.  items[i].out_bytes = min(slot_i,
+ *   total_out - offsets[i]), 0 past the end; status ZB_OK, or ZB_E_DATA with the decoder's message when the input the range needs
+ *   turns out to be damaged.  One bad range never changes another's result.  With a host dst the rest of each slot is zeroed.
+ *   src is the indexed stream (host, or device with src_on_device); src_len below the index's in_bytes gives ZB_E_PARAM, as do more
+ *   than 2^20 ranges and slots of 4 GiB or more.  A host src is not uploaded whole: a range needs only the input from its point up
+ *   to the first point at or after its end (or its member's end), and the dynamic header of its point's block (at most 288 bytes).
+ *   One kernel launch and one host sync whatever n_ranges; a range is decoded by one warp per member it touches, at most
+ *   S + 65535 + its length bytes of decoding each.  Returns ZB_OK, or the status of the first range that failed.
+ * zb_index_serialize: buf NULL gives the length only; cap below it gives ZB_E_BUF.  Layout (little-endian):
+ *     header   u32 magic "ZBIX" (0x5849425a), u32 version 1, u64 span, u64 total_out, u64 in_bytes, u32 check, i32 window_bits,
+ *              u64 n_members, u64 n_points, u64 win_bytes                                              (64 bytes)
+ *     members  n_members x {u64 in_start, in_end, out_start, out_end}: input (header and trailer included) and output (32 bytes)
+ *     points   n_points x {u64 out_off, bit, hdr_bit; u32 member, btype, window_len, 0}, sorted by (out_off, bit)  (40 bytes)
+ *     windows  the window_len bytes of every point, in point order
+ * zb_index_deserialize: validates every field (magic, version, lengths, order, bits below 8 * in_bytes, members, btype, window
+ *   lengths) and gives ZB_E_DATA for a malformed blob, never reading outside buf[0, len).
+ * An index is host memory, independent of the engine that built it, and read-only: several threads may extract through one index
+ * with an engine each. */
+typedef struct zb_index zb_index;
+typedef struct zb_index_info {
+    uint64_t span, total_out, in_bytes, n_points, n_members;
+    uint32_t check;      /* res->check of the build */
+    int32_t window_bits; /* as passed to the build */
+} zb_index_info;
+typedef struct zb_index_point {
+    uint64_t out_off;       /* offset in the whole output */
+    uint64_t bit;           /* absolute bit offset in the input */
+    uint64_t hdr_bit;       /* header bit of the block it sits in (== bit for a block header) */
+    uint32_t member, btype; /* index of its member; block type 0 stored, 1 fixed, 2 dynamic */
+    uint32_t window_len;
+    const uint8_t *window;  /* window_len bytes: the output in front of out_off, valid as long as the index */
+} zb_index_point;
+ZB_API int zb_index_build(zb_engine *e, const void *src, size_t src_len, int src_on_device, void *dst, size_t dst_cap, int dst_on_device,
+                          int window_bits, uint32_t flags, uint64_t span, zb_inflate_result *res, zb_index **out);
+ZB_API int zb_index_extract(zb_engine *e, const zb_index *idx, const void *src, size_t src_len, int src_on_device, const uint64_t *offsets,
+                            size_t n_ranges, void *dst, const uint64_t *dst_off, int dst_on_device, zb_inflate_result *items);
+ZB_API int zb_index_serialize(const zb_index *idx, void *buf, size_t cap, size_t *len);
+ZB_API int zb_index_deserialize(const void *buf, size_t len, zb_index **out);
+ZB_API int zb_index_get_info(const zb_index *idx, zb_index_info *info);
+ZB_API int zb_index_get_point(const zb_index *idx, size_t i, zb_index_point *p);
+ZB_API void zb_index_free(zb_index *idx);
+
 /* Chunk-sharded deflate with the one-stream bytes (levels 7..9; see DESIGN.md §5).  One input of total_len bytes is cut into
  * contiguous ranges [S_r, E_r), one per rank (every range but the last >= 64 KiB); each rank runs the four calls below on its
  * own engine, and the caller moves the small records between them (the library has no transport):

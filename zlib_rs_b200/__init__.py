@@ -74,6 +74,16 @@ class ShardSpan(ctypes.Structure):
                 ("reserved", ctypes.c_uint32)]
 
 
+class IndexInfo(ctypes.Structure):
+    _fields_ = [("span", ctypes.c_uint64), ("total_out", ctypes.c_uint64), ("in_bytes", ctypes.c_uint64), ("n_points", ctypes.c_uint64),
+                ("n_members", ctypes.c_uint64), ("check", ctypes.c_uint32), ("window_bits", ctypes.c_int32)]
+
+
+class IndexPoint(ctypes.Structure):
+    _fields_ = [("out_off", ctypes.c_uint64), ("bit", ctypes.c_uint64), ("hdr_bit", ctypes.c_uint64), ("member", ctypes.c_uint32),
+                ("btype", ctypes.c_uint32), ("window_len", ctypes.c_uint32), ("window", ctypes.c_void_p)]
+
+
 class ZlibError(Exception):
     def __init__(self, code, msg=""):
         super().__init__("zlib error %d %s" % (code, msg))
@@ -139,6 +149,15 @@ def lib():
                                            ctypes.POINTER(DeflateResult)]
             L.zb_deflate_batch_bound.argtypes, L.zb_deflate_batch_bound.restype = [u64p, sz], sz
             L.zb_inflate_batch.argtypes = [vp, vp, u64p, sz, ci, vp, u64p, ci, ci, ctypes.POINTER(InflateResult)]
+        if hasattr(L, "zb_index_build"):
+            u64p = ctypes.POINTER(u64)
+            L.zb_index_build.argtypes = [vp, vp, sz, ci, vp, sz, ci, ci, u32, u64, ctypes.POINTER(InflateResult), ctypes.POINTER(vp)]
+            L.zb_index_extract.argtypes = [vp, vp, vp, sz, ci, u64p, sz, vp, u64p, ci, ctypes.POINTER(InflateResult)]
+            L.zb_index_serialize.argtypes = [vp, vp, sz, ctypes.POINTER(sz)]
+            L.zb_index_deserialize.argtypes = [vp, sz, ctypes.POINTER(vp)]
+            L.zb_index_get_info.argtypes = [vp, ctypes.POINTER(IndexInfo)]
+            L.zb_index_get_point.argtypes = [vp, sz, ctypes.POINTER(IndexPoint)]
+            L.zb_index_free.argtypes, L.zb_index_free.restype = [vp], None
         if hasattr(L, "zb_deflate_batch_dict"):
             L.zb_deflate_batch_dict.argtypes = [vp, vp, sz] + L.zb_deflate_batch.argtypes[1:]
             L.zb_inflate_batch_dict.argtypes = [vp, vp, sz] + L.zb_inflate_batch.argtypes[1:]
@@ -186,6 +205,18 @@ def _gather(items):
     items = [bytes(x) for x in items]
     data = b"".join(items)
     return (ctypes.c_char * max(len(data), 1)).from_buffer_copy(data or b"\0"), _offsets([len(x) for x in items])
+
+
+def _host_view(src):
+    """(address, length, keep-alive) of a host buffer without copying it: bytes, or any writable contiguous buffer (bytearray,
+    mmap, numpy array).  Other read-only buffers are copied once."""
+    if not isinstance(src, bytes):
+        mv = memoryview(src).cast("B")
+        if mv.readonly or len(mv) == 0:
+            return _host_view(bytes(mv))
+        arr = (ctypes.c_char * len(mv)).from_buffer(mv)
+        return ctypes.addressof(arr), len(mv), (arr, mv)
+    return ctypes.cast(ctypes.c_char_p(src), ctypes.c_void_p).value, len(src), src
 
 
 def _dictionary(dictionary, on_device):
@@ -356,6 +387,61 @@ class Inflate:
             pass
 
 
+# ---------------------------------------------------------------- access-point index (zb_index_*)
+class Index:
+    """An access-point index of one stream (zb_index_build): host memory, independent of the engine that built it.
+    .info: IndexInfo; .points: list of dicts (out_off, bit, hdr_bit, member, btype, window_len, window bytes)."""
+
+    def __init__(self, handle):
+        self.h = handle
+
+    @classmethod
+    def from_bytes(cls, blob):
+        """The index of a serialized blob (validated: a malformed one raises ZlibError(ZB_E_DATA))."""
+        data, keep = _buf(blob)
+        h = ctypes.c_void_p()
+        rc = lib().zb_index_deserialize(keep, len(data), ctypes.byref(h))
+        if rc != 0:
+            raise ZlibError(rc, lib().zb_last_error().decode())
+        return cls(h.value)
+
+    def to_bytes(self):
+        n = ctypes.c_size_t(0)
+        lib().zb_index_serialize(self.h, None, 0, ctypes.byref(n))
+        buf = ctypes.create_string_buffer(max(n.value, 1))
+        rc = lib().zb_index_serialize(self.h, buf, n.value, ctypes.byref(n))
+        if rc != 0:
+            raise ZlibError(rc)
+        return buf.raw[: n.value]
+
+    @property
+    def info(self):
+        i = IndexInfo()
+        lib().zb_index_get_info(self.h, ctypes.byref(i))
+        return i
+
+    @property
+    def points(self):
+        out = []
+        p = IndexPoint()
+        for i in range(self.info.n_points):
+            lib().zb_index_get_point(self.h, i, ctypes.byref(p))
+            out.append(dict(out_off=p.out_off, bit=p.bit, hdr_bit=p.hdr_bit, member=p.member, btype=p.btype, window_len=p.window_len,
+                            window=ctypes.string_at(p.window, p.window_len) if p.window_len else b""))
+        return out
+
+    def close(self):
+        if self.h:
+            lib().zb_index_free(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 # ---------------------------------------------------------------- low-level engine (device-resident buffers)
 class Engine:
     def __init__(self, device=0):
@@ -514,6 +600,53 @@ class Engine:
         if own is not None:
             raw = own.raw
             outs = [raw[doff[i]:doff[i] + results[i].out_bytes] for i in range(n)]
+        return rc, outs, results
+
+    def build_index(self, src, out_cap, span=1 << 20, window_bits=15, flags=0, n=None, src_on_device=False, dst=None,
+                    dst_on_device=False):
+        """Inflate `src` as Engine.inflate does and index it (zb_index_build): access points every `span` output bytes.
+        Returns (rc, bytes or None, InflateResult, Index or None): the first three are what Engine.inflate returns for the same
+        arguments; the Index only with rc == 0."""
+        res = InflateResult()
+        keep = None
+        if not src_on_device:
+            data, keep = _buf(src)
+            n = len(data)
+            src = ctypes.addressof(keep)
+        own = None
+        if dst is None:
+            own = ctypes.create_string_buffer(max(out_cap, 1))
+            dst = ctypes.addressof(own)
+        h = ctypes.c_void_p()
+        rc = lib().zb_index_build(self.h, src, n, int(src_on_device), dst, out_cap, int(dst_on_device), window_bits, flags, span,
+                                  ctypes.byref(res), ctypes.byref(h))
+        return rc, (own.raw[: res.out_bytes] if own is not None else None), res, (Index(h.value) if rc == 0 and h.value else None)
+
+    def extract(self, src, index, ranges, n=None, src_on_device=False, dst=None, dst_off=None, dst_on_device=False):
+        """Extract byte ranges of an indexed stream in one call (zb_index_extract).  `ranges`: a list of (offset, length); a
+        caller's `dst` takes `dst_off` (len(ranges) + 1 offsets) and then only the offsets of `ranges` count.  Host `src` may be
+        bytes or any writable buffer (bytearray, mmap, numpy array), which is not copied: only the input the ranges need is read;
+        device `src` is a pointer + n.  Returns (rc, list of bytes or None, list of InflateResult)."""
+        keep = None
+        if not src_on_device:
+            src, n, keep = _host_view(src)
+        nr = len(ranges)
+        offs = (ctypes.c_uint64 * max(nr, 1))(*[r[0] for r in ranges])
+        own = None
+        if dst is None:
+            doff = _offsets([r[1] for r in ranges])
+            own = ctypes.create_string_buffer(max(doff[nr], 1))
+            dst = ctypes.addressof(own)
+            dst_on_device = False
+        else:
+            doff = (ctypes.c_uint64 * len(dst_off))(*dst_off)
+        res = (InflateResult * max(nr, 1))()
+        rc = lib().zb_index_extract(self.h, index.h, src, n, int(src_on_device), offs, nr, dst, doff, int(dst_on_device), res)
+        results = list(res)[:nr]
+        outs = None
+        if own is not None:
+            raw = own.raw
+            outs = [raw[doff[i]:doff[i] + results[i].out_bytes] for i in range(nr)]
         return rc, outs, results
 
     def adler32(self, buf, n=None, start=1, on_device=False):

@@ -1180,6 +1180,102 @@ int zb_inflate_blocks(zb_engine *z, const void *src, size_t n, uint64_t start_bi
     return z->e.inflate_blocks(src, n, start_bit, dict, dict_len, dst, cap, check_kind, check_start, out);
 }
 
+int zb_index_build(zb_engine *z, const void *src, size_t src_len, int src_dev, void *dst, size_t cap, int dst_dev, int window_bits,
+                   uint32_t flags, uint64_t span, zb_inflate_result *res, zb_index **out)
+{
+    if (!z) return ZB_E_NODEVICE;
+    if (!out) return ZB_E_PARAM;
+    *out = nullptr;
+    if (flags & ZB_INF_NO_SERIAL) { snprintf(zb::g_err, sizeof zb::g_err, "index_build: ZB_INF_NO_SERIAL is not accepted"); return ZB_E_PARAM; }
+    if (span < zb::kIdxMinSpan || span > zb::kIdxMaxSpan) { snprintf(zb::g_err, sizeof zb::g_err, "index_build: span %llu outside [32768, 2^32]", (unsigned long long)span); return ZB_E_PARAM; }
+    z->e.shard.phase = 0; // a range job in progress is gone (its buffers are reused)
+    zb::IdxBuild ib;
+    ib.span = span;
+    ib.out = new (std::nothrow) zb_index;
+    if (!ib.out) return ZB_E_MEM;
+    int rc;
+    try {
+        rc = z->e.inflate(src, src_len, src_dev != 0, dst, cap, dst_dev != 0, window_bits, res, flags, &ib);
+    } catch (const std::bad_alloc &) {
+        rc = ZB_E_MEM;
+    }
+    if (rc == ZB_OK) *out = ib.out;
+    else delete ib.out;
+    return rc;
+}
+
+int zb_index_extract(zb_engine *z, const zb_index *idx, const void *src, size_t src_len, int src_dev, const uint64_t *offsets,
+                     size_t n_ranges, void *dst, const uint64_t *dst_off, int dst_dev, zb_inflate_result *items)
+{
+    if (!z) return ZB_E_NODEVICE;
+    z->e.shard.phase = 0; // a range job in progress is gone (its buffers are reused)
+    try {
+        return z->e.index_extract(idx, src, src_len, src_dev != 0, offsets, n_ranges, dst, dst_off, dst_dev != 0, items);
+    } catch (const std::bad_alloc &) {
+        return ZB_E_MEM;
+    }
+}
+
+int zb_index_serialize(const zb_index *x, void *buf, size_t cap, size_t *len)
+{
+    if (!x || !len) return ZB_E_PARAM;
+    const size_t hb = sizeof x->h, mb = x->m.size() * sizeof(zb::IdxMember), pb = x->p.size() * sizeof(zb::IdxPoint);
+    *len = hb + mb + pb + x->win.size();
+    if (!buf) return ZB_OK;
+    if (cap < *len) return ZB_E_BUF;
+    uint8_t *o = static_cast<uint8_t *>(buf);
+    memcpy(o, &x->h, hb);
+    if (mb) memcpy(o + hb, x->m.data(), mb);
+    if (pb) memcpy(o + hb + mb, x->p.data(), pb);
+    if (!x->win.empty()) memcpy(o + hb + mb + pb, x->win.data(), x->win.size());
+    return ZB_OK;
+}
+
+int zb_index_deserialize(const void *buf, size_t len, zb_index **out)
+{
+    if (!out) return ZB_E_PARAM;
+    *out = nullptr;
+    zb::IdxHeader h;
+    const uint8_t *b = static_cast<const uint8_t *>(buf);
+    if (zb::zbi_validate(b, len, &h) != 0) { snprintf(zb::g_err, sizeof zb::g_err, "index_deserialize: malformed index"); return ZB_E_DATA; }
+    zb_index *x = new (std::nothrow) zb_index;
+    if (!x) return ZB_E_MEM;
+    try {
+        x->h = h;
+        const uint8_t *mp = b + sizeof h, *pp = mp + h.n_members * sizeof(zb::IdxMember), *wp = pp + h.n_points * sizeof(zb::IdxPoint);
+        x->m.resize(h.n_members);
+        memcpy(x->m.data(), mp, h.n_members * sizeof(zb::IdxMember));
+        x->p.resize(h.n_points);
+        memcpy(x->p.data(), pp, h.n_points * sizeof(zb::IdxPoint));
+        x->win.assign(wp, wp + h.win_bytes);
+        x->woff.resize(h.n_points);
+        uint64_t w = 0;
+        for (size_t i = 0; i < x->p.size(); i++) { x->woff[i] = w; w += x->p[i].window_len; }
+    } catch (const std::bad_alloc &) {
+        delete x;
+        return ZB_E_MEM;
+    }
+    *out = x;
+    return ZB_OK;
+}
+
+int zb_index_get_info(const zb_index *x, zb_index_info *info)
+{
+    if (!x || !info) return ZB_E_PARAM;
+    *info = zb_index_info{x->h.span, x->h.total_out, x->h.in_bytes, x->h.n_points, x->h.n_members, x->h.check, x->h.window_bits};
+    return ZB_OK;
+}
+
+int zb_index_get_point(const zb_index *x, size_t i, zb_index_point *p)
+{
+    if (!x || !p || i >= x->p.size()) return ZB_E_PARAM;
+    const zb::IdxPoint &q = x->p[i];
+    *p = zb_index_point{q.out_off, q.bit, q.hdr_bit, q.member, q.btype, q.window_len, x->win.data() + x->woff[i]};
+    return ZB_OK;
+}
+
+void zb_index_free(zb_index *x) { delete x; }
+
 int zb_adler32(zb_engine *z, uint32_t start, const void *buf, size_t len, int on_dev, uint32_t *out, float *ms)
 {
     if (!z) return ZB_E_NODEVICE;

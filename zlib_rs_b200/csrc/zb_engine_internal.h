@@ -3,7 +3,9 @@
 #include <cuda_runtime.h>
 #include <stddef.h>
 #include <stdint.h>
+#include <vector>
 #include "../../include/zb_engine.h"
+#include "zb_index.h"
 #include "zb_kernels.cuh"
 
 namespace zb {
@@ -17,6 +19,8 @@ enum { S_IN, S_L, S_HOLES, S_HOLESN, S_M, S_NXT, S_PEXIT, S_PCNT, S_SYMIDX, S_TE
        S_MEMT, S_MEMC, // multi-member gzip: tile counts and control block; candidate and member tables
        S_BGZF,         // BGZF writing and deflate batches: member tables and control block
        S_BATCH,        // batches: the caller's offsets, a host source's bytes (deflate), item tables and results (inflate)
+       S_INDEX,        // index build: jobs, hits and points; extract: pieces, decoder states, windows and staged input
+       S_INDEXW,       // index build: the windows of the points
        S_COUNT };
 
 // A range job of chunk-sharded deflate (zb_shard_*, zb_shard.cu) between its four calls.
@@ -32,8 +36,29 @@ struct ShardState {
     zb_shard_span span;
 };
 
+// What an inflate call tells the index build (zb_index_build): where each member lies and, for each member that the block-parallel
+// path decoded, its block table (input bits from the member's first byte, output from the member's start).
+struct IdxBlock {
+    uint64_t start_bit, out_off;
+    uint32_t out_len, type;
+};
+struct TraceMember {
+    IdxMember m;
+    std::vector<IdxBlock> blocks; // empty when k_inflate or k_members decoded the member
+};
+struct InfTrace {
+    std::vector<TraceMember> members;
+    std::vector<IdxBlock> blocks; // the table of the last inflate_stream call
+    uint32_t kind = 0;            // 0 raw, 1 zlib, 2 gzip (every member of ZB_INF_MEMBERS)
+};
+struct IdxBuild {
+    uint64_t span = 0;
+    InfTrace tr;
+    zb_index *out = nullptr;
+};
+
 struct Engine {
-    static constexpr int kSlots = 42;
+    static constexpr int kSlots = 44;
     struct Buf { void *p = nullptr; size_t cap = 0; };
     int device = -1;
     cudaStream_t st = nullptr, st2 = nullptr; // st2: the serial tail runs beside k_emit
@@ -75,10 +100,14 @@ struct Engine {
                         uint32_t **d_freq);
     int members_launch(JobBufs &jb, BgzfJob &bj, int level, uint32_t *d_freq);
     int inflate(const void *src, size_t n, bool src_dev, void *dst, size_t dst_cap, bool dst_dev, int window_bits,
-                zb_inflate_result *res, uint32_t flags = 0);
+                zb_inflate_result *res, uint32_t flags = 0, IdxBuild *ib = nullptr);
     int inflate_stream(const uint8_t *d_src, size_t n, uint8_t *d_dst, size_t dst_cap, int window_bits, uint32_t flags,
-                       zb_inflate_result *res);
-    int inflate_members(const uint8_t *d_src, size_t n, uint8_t *d_dst, size_t dst_cap, int window_bits, zb_inflate_result *res);
+                       zb_inflate_result *res, InfTrace *tr = nullptr);
+    int inflate_members(const uint8_t *d_src, size_t n, uint8_t *d_dst, size_t dst_cap, int window_bits, zb_inflate_result *res,
+                        InfTrace *tr = nullptr);
+    int index_points(const uint8_t *d_src, const uint8_t *d_dst, const zb_inflate_result *res, int window_bits, IdxBuild *ib);
+    int index_extract(const zb_index *x, const void *src, size_t src_len, bool src_dev, const uint64_t *offsets, size_t n_ranges,
+                      void *dst, const uint64_t *dst_off, bool dst_dev, zb_inflate_result *items);
     int inflate_batch(const void *dict, size_t dict_len, const void *src, const uint64_t *src_off, size_t n_items, bool src_dev, void *dst,
                       const uint64_t *dst_off, bool dst_dev, int window_bits, zb_inflate_result *items);
     int inflate_blocks(const void *src, size_t n, uint64_t start_bit, const void *dict, size_t dict_len, void *dst, size_t dst_cap,
@@ -95,3 +124,13 @@ struct Engine {
 static_assert(S_COUNT <= Engine::kSlots, "slots");
 
 } // namespace zb
+
+// An access-point index (zb_index_* in zb_engine.h): host memory, read-only once built or loaded.  woff[i] is where point i's window
+// starts in win.
+struct zb_index {
+    zb::IdxHeader h;
+    std::vector<zb::IdxMember> m;
+    std::vector<zb::IdxPoint> p;
+    std::vector<uint64_t> woff;
+    std::vector<uint8_t> win;
+};

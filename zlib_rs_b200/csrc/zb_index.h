@@ -1,0 +1,173 @@
+// zb_index.h -- random access into deflate, zlib and gzip streams: the access-point rule, the serialized index, its validation,
+// the lookup from an output offset to its point and the input a range needs (zb_index_* in zb_engine.h, DESIGN.md §2k).
+//
+// Like zb_members.h this is `__host__ __device__`: the index kernels of zb_inflate.cu use it, the host code of the engine uses it,
+// and tests/indexmodel compiles the same source for the CPU (with AddressSanitizer and UBSan) so the CPU tests check it.
+//
+// An access point is a position in the compressed input where raw-block decoding can resume, given the 32 KiB of output in front
+// of it: the bit where a block's 3 header bits start (any block type), or the bit where a literal or length symbol starts inside a
+// fixed-code or dynamic block (never the end-of-block code, never inside a stored block's payload).  Along the stream the output
+// offsets of the access points never decrease, so "in stream order" and "sorted by (out_off, bit)" are the same order.
+//
+// For a span S the index holds exactly:
+//   - the header of the first block of every member (its window is empty);
+//   - for every k >= 1 with k * S < total output, the first access point in stream order whose output offset (in the whole output)
+//     is >= k * S, unless it is already in the list.
+// So the points are a function of the stream and S alone, and for any output offset x the last point at or before x lies less than
+// S + 65535 bytes behind x (S + 258 inside Huffman blocks).
+//
+// Serialized layout (little-endian, as the structs below lay it out):
+//   IdxHeader                      64 bytes
+//   IdxMember  x n_members         32 bytes each
+//   IdxPoint   x n_points          40 bytes each
+//   windows                        the window_len bytes of every point, in point order (win_bytes in all)
+#pragma once
+#include <string.h>
+#include "zb_core.h"
+
+namespace zb {
+
+constexpr uint32_t kIdxMagic = 0x5849425au; // "ZBIX"
+constexpr uint32_t kIdxVersion = 1;
+constexpr uint32_t kIdxWindow = 32768;
+constexpr uint64_t kIdxMinSpan = 32768, kIdxMaxSpan = 1ull << 32;
+constexpr uint64_t kIdxMaxRanges = 1ull << 20;
+constexpr uint32_t kIdxDynHeaderBytes = 288; // 74 header bits + at most 316 code-length codes of 7 bits, from any bit of a byte
+
+struct IdxHeader {
+    uint32_t magic, version;
+    uint64_t span, total_out, in_bytes;
+    uint32_t check;
+    int32_t window_bits;
+    uint64_t n_members, n_points, win_bytes;
+};
+struct IdxMember {           // member m: input bytes [in_start, in_end) (header and trailer included), output [out_start, out_end)
+    uint64_t in_start, in_end, out_start, out_end;
+};
+struct IdxPoint {
+    uint64_t out_off, bit, hdr_bit; // bit: absolute input bit of the point; hdr_bit: of its block's header (== bit for a header)
+    uint32_t member, btype, window_len, reserved;
+};
+static_assert(sizeof(IdxHeader) == 64 && sizeof(IdxMember) == 32 && sizeof(IdxPoint) == 40, "serialized layout");
+
+// number of targets k * S (k >= 1) below the total output
+ZB_HD uint64_t zbi_targets(uint64_t total_out, uint64_t span) { return total_out ? (total_out - 1) / span : 0; }
+
+ZB_HD uint32_t zbi_window_len(uint64_t out_off, uint64_t member_out_start)
+{
+    const uint64_t w = out_off - member_out_start;
+    return w < kIdxWindow ? (uint32_t)w : kIdxWindow;
+}
+
+// First i in [0, n) with pred(i) true, for a predicate that is false then true along i; n when it never holds.
+template <typename F>
+ZB_HD uint64_t zbi_first(uint64_t n, F pred)
+{
+    uint64_t lo = 0, hi = n;
+    while (lo < hi) {
+        const uint64_t mid = lo + (hi - lo) / 2;
+        if (pred(mid)) hi = mid;
+        else lo = mid + 1;
+    }
+    return lo;
+}
+
+// The unit (member, or block of one stream) in which the first access point at or after output offset T lies, for units in stream
+// order with output ranges [start, end): the first one that either starts at or after T (then its first header is the point) or
+// ends after T (then the point is inside it or, when its last symbol starts before T, the next unit's first header).
+// `units` has start(u) and end(u).
+template <typename Units>
+ZB_HD uint64_t zbi_unit_of(const Units &units, uint64_t n, uint64_t T)
+{
+    return zbi_first(n, [&](uint64_t u) { return units.end(u) > T || units.start(u) >= T; });
+}
+
+// Index of the last point with out_off <= off (points sorted); n_points when there is none.
+ZB_HD uint64_t zbi_lookup(const IdxPoint *p, uint64_t n_points, uint64_t off)
+{
+    const uint64_t i = zbi_first(n_points, [&](uint64_t k) { return p[k].out_off > off; });
+    return i ? i - 1 : n_points;
+}
+
+// The member whose output holds offset off: the first member with out_end > off; n_members past the end.
+ZB_HD uint64_t zbi_member_at(const IdxMember *m, uint64_t n_members, uint64_t off)
+{
+    return zbi_first(n_members, [&](uint64_t k) { return m[k].out_end > off; });
+}
+
+// The input a piece needs: the output [a, b) of one member (a < b), decoded from point pi = zbi_lookup(a).
+//   hdr   the dynamic header of the point's block (at most 288 bytes from hdr_bit), or the byte holding BFINAL of a fixed block;
+//         empty when the point is a block header;
+//   body  from the byte holding the point's bit up to and including the byte holding the bit of the first point at or after b in
+//         the same member, else up to the member's end.
+struct IdxSpan { uint64_t hdr_lo, hdr_hi, body_lo, body_hi; };
+ZB_HD IdxSpan zbi_piece_span(const IdxPoint *p, uint64_t n_points, const IdxMember *m, uint64_t pi, uint64_t b)
+{
+    const IdxPoint &pt = p[pi];
+    const IdxMember &mb = m[pt.member];
+    IdxSpan s;
+    s.hdr_lo = s.hdr_hi = pt.hdr_bit >> 3;
+    if (pt.bit != pt.hdr_bit) {
+        const uint64_t want = pt.btype == 2 ? kIdxDynHeaderBytes : 1;
+        s.hdr_hi = s.hdr_lo + want < mb.in_end ? s.hdr_lo + want : mb.in_end;
+    }
+    s.body_lo = pt.bit >> 3;
+    const uint64_t q = pi + zbi_first(n_points - pi, [&](uint64_t k) { return p[pi + k].out_off >= b; });
+    s.body_hi = (q < n_points && p[q].member == pt.member) ? (p[q].bit >> 3) + 1 : mb.in_end;
+    return s;
+}
+
+// Validation of a serialized index (it may come from outside the program): 0 when every field is consistent, else -1.  Nothing
+// outside buf[0, len) is read.  Checked: magic, version, lengths and counts (no overflow); members contiguous in the output and
+// ordered in the input within in_bytes; points sorted by (out_off, bit) with strictly increasing bits below 8 * in_bytes, each inside
+// its member's input and output, members in order with a point at every member's start; btype 0..2 (a stored point is a header);
+// window_len = min(32768, the output in front of the point in its member); win_bytes the sum of the window lengths.
+ZB_HD int zbi_validate(const uint8_t *buf, uint64_t len, IdxHeader *out)
+{
+    IdxHeader h;
+    if (!buf || len < sizeof h) return -1;
+    memcpy(&h, buf, sizeof h);
+    if (h.magic != kIdxMagic || h.version != kIdxVersion) return -1;
+    if (h.span < kIdxMinSpan || h.span > kIdxMaxSpan) return -1;
+    const uint64_t rest = len - sizeof h;
+    if (h.n_members == 0 || h.n_members > rest / sizeof(IdxMember)) return -1;
+    const uint64_t after_m = rest - h.n_members * sizeof(IdxMember);
+    if (h.n_points < h.n_members || h.n_points > after_m / sizeof(IdxPoint)) return -1;
+    if (h.win_bytes != after_m - h.n_points * sizeof(IdxPoint)) return -1;
+    if (h.in_bytes > (~0ull >> 4)) return -1;
+    const uint8_t *mp = buf + sizeof h, *pp = mp + h.n_members * sizeof(IdxMember);
+    IdxMember prev{0, 0, 0, 0};
+    for (uint64_t i = 0; i < h.n_members; i++) {
+        IdxMember m;
+        memcpy(&m, mp + i * sizeof m, sizeof m);
+        if (m.in_start > m.in_end || m.in_end > h.in_bytes || m.out_start > m.out_end) return -1;
+        if (m.out_start != prev.out_end || (i && m.in_start < prev.in_end)) return -1;
+        prev = m;
+    }
+    if (prev.out_end != h.total_out) return -1;
+    uint64_t win = 0, cur = 0;
+    IdxPoint last{0, 0, 0, 0, 0, 0, 0};
+    for (uint64_t i = 0; i < h.n_points; i++) {
+        IdxPoint p;
+        memcpy(&p, pp + i * sizeof p, sizeof p);
+        if (p.member >= h.n_members || p.btype > 2 || p.reserved != 0) return -1;
+        if (i && (p.out_off < last.out_off || p.bit <= last.bit || p.member < last.member)) return -1;
+        if (i == 0 ? p.member != 0 : (p.member != last.member && p.member != last.member + 1)) return -1;
+        IdxMember m;
+        memcpy(&m, mp + (uint64_t)p.member * sizeof m, sizeof m);
+        const bool first = i == 0 || p.member != last.member;
+        if (first && p.out_off != m.out_start) return -1;
+        if (p.out_off < m.out_start || p.out_off > m.out_end) return -1;
+        if (p.hdr_bit > p.bit || p.hdr_bit < 8 * m.in_start || p.bit >= 8 * m.in_end) return -1;
+        if (p.btype == 0 && p.bit != p.hdr_bit) return -1;
+        if (p.window_len != zbi_window_len(p.out_off, m.out_start)) return -1;
+        win += p.window_len;
+        cur = p.member;
+        last = p;
+    }
+    if (cur != h.n_members - 1 || win != h.win_bytes) return -1;
+    if (out) *out = h;
+    return 0;
+}
+
+} // namespace zb

@@ -17,6 +17,7 @@
 #include "zb_engine_internal.h"
 #include "zb_inflate_core.h"
 #include "zb_members.h"
+#include "zb_index.h"
 
 namespace zb {
 
@@ -147,10 +148,23 @@ struct InfShared {
 
 enum Cmd { C_NONE = 0, C_REFILL, C_FLUSH, C_COPY, C_DONE };
 
+// A range of an indexed stream (zb_index_extract, kRange = true, always in segment mode): the segment starts at an access point.
+// When that point is inside a block (resume), the block's tables come from its header at bit hdr_bit of hdr[0, hdr_n) -- a dynamic
+// header, or for a fixed block just its BFINAL bit -- and decoding goes on at the segment's start bit.  The first `skip` bytes of
+// output are discarded, the next `want` go to dst[0, want), and decoding stops as soon as they are complete.
+struct InfRange {
+    const uint8_t *hdr;
+    uint64_t hdr_n, hdr_bit, skip, want;
+    uint32_t btype, resume;
+};
+
 // The one-warp decoder: a whole stream (header, blocks, trailer) or, in segment mode, raw blocks from a bit position.  Output goes to
-// dst[0, cap) only.  k_inflate runs it on one stream, k_members on one gzip member per warp.
+// dst[0, cap) only.  k_inflate runs it on one stream, k_members on one gzip member per warp, k_index_extract (kRange) on one piece
+// of a range; the kRange additions compile away in the others.
+template <bool kRange = false>
 __device__ __forceinline__ void inflate_warp(InfShared &S, const uint8_t *__restrict__ src, uint64_t n, uint8_t *__restrict__ dst,
-                                             uint64_t cap, int window_bits, InfState *res, InfSeg seg, InfDict pd = InfDict{nullptr, nullptr, 0, 0})
+                                             uint64_t cap, int window_bits, InfState *res, InfSeg seg, InfDict pd = InfDict{nullptr, nullptr, 0, 0},
+                                             InfRange rg = InfRange{})
 {
     const uint32_t lane = threadIdx.x;
     // shared between lanes through shuffles from lane 0
@@ -201,8 +215,25 @@ __device__ __forceinline__ void inflate_warp(InfShared &S, const uint8_t *__rest
         inflate_table(1, S.lens, 288, S.lenfix, 9, S.work, &root);
         for (sym = 0; sym < 32; sym++) S.lens[sym] = 5;
         inflate_table(2, S.lens, 32, S.distfix, 5, S.work, &root);
+        if constexpr (kRange) {
+            if (rg.resume && rg.btype == 2) {
+                DynHeader h;
+                if (!parse_dynamic_header(BitSrc{rg.hdr, rg.hdr_n}, rg.hdr_bit, h, S.lens) ||
+                    inflate_table(1, S.lens, h.hlit, S.lencode, 10, S.work, &lenbits) ||
+                    inflate_table(2, S.lens + h.hlit, h.hdist, S.distcode, 9, S.work, &distbits)) {
+                    err = IE_CODE_LENS;
+                    mode = 5;
+                } else {
+                    lencode = S.lencode; distcode = S.distcode;
+                    last = (int)h.bfinal;
+                }
+            } else if (rg.resume) {
+                last = rg.hdr_n ? (rg.hdr[rg.hdr_bit >> 3] >> (rg.hdr_bit & 7)) & 1 : 0;
+            }
+        }
     }
     __syncwarp();
+    const uint64_t rstop = D0 + rg.skip + rg.want; // kRange: the output position where decoding stops
 
 #define NEED(nb) do { while (bits < (nb)) { hold |= (uint64_t)((ipos < n) ? S.in[ipos & (kInRing - 1)] : 0) << bits; ipos++; bits += 8; } } while (0)
 #define BITS(nb) ((uint32_t)(hold & ((1ull << (nb)) - 1)))
@@ -219,6 +250,7 @@ __device__ __forceinline__ void inflate_warp(InfShared &S, const uint8_t *__rest
             // run until a cooperative action is needed
             while (cmd == C_NONE) {
                 if (mode == 5) { cmd = C_DONE; break; }
+                if constexpr (kRange) { if (opos >= rstop) { mode = 5; continue; } }
                 if (ifill < n && ifill - ipos < 1024) { cmd = C_REFILL; break; }
                 if (opos - oflush >= kOutRing / 2 + 2048) { cmd = C_FLUSH; break; }
                 if (consumed_bits > 8 * n) { FAIL(IE_TRUNCATED); continue; }
@@ -282,6 +314,7 @@ __device__ __forceinline__ void inflate_warp(InfShared &S, const uint8_t *__rest
                 }
                 if (mode == 1) {
                     if (seg.on && consumed_bits < seg.start_bit) { const uint32_t k0 = (uint32_t)(seg.start_bit & 7); NEED(k0); DROP(k0); continue; }
+                    if constexpr (kRange) { if (rg.resume) { rg.resume = 0; mode = 3; continue; } } // inside the block: its tables are set
                     if (last) {
                         if (seg.on) { final_done = 1; blk_bit = consumed_bits; blk_out = opos; mode = 5; continue; } // the caller frames the trailer
                         DROP(bits & 7); mode = 4; continue;
@@ -349,6 +382,7 @@ __device__ __forceinline__ void inflate_warp(InfShared &S, const uint8_t *__rest
                 if (mode == 2) { // stored bytes (bit buffer is byte aligned here)
                     uint32_t k = 0;
                     while (stored_left && k < 4096) {
+                        if constexpr (kRange) { if (opos >= rstop) break; }
                         if (ifill < n && ifill - ipos < 16) break;
                         if (opos - D0 >= cap) { FAIL(IE_OUTPUT_FULL); break; }
                         NEED(8);
@@ -363,6 +397,7 @@ __device__ __forceinline__ void inflate_warp(InfShared &S, const uint8_t *__rest
                 if (mode == 3) { // literal/length/distance loop (inflate.rs:1918-2158)
                     uint32_t budget = 512;
                     while (budget--) {
+                        if constexpr (kRange) { if (opos >= rstop) break; }
                         if (ifill < n && ifill - ipos < 64) break;
                         if (opos - oflush >= kOutRing - 4096) break;
                         NEED(48);
@@ -437,7 +472,12 @@ __device__ __forceinline__ void inflate_warp(InfShared &S, const uint8_t *__rest
             const uint64_t opos0 = __shfl_sync(0xffffffffu, opos, 0);
             const uint64_t upto = cmd == C_DONE ? opos0 : oflush + kOutRing / 2; // the trigger guarantees opos0 >= upto
             const uint64_t end = upto - D0 > cap ? cap + D0 : upto;
-            for (uint64_t i = oflush + lane; i < end; i += 32) dst[i - D0] = S.out[i & (kOutRing - 1)];
+            if constexpr (kRange) { // only [D0 + skip, rstop) is written, to dst[0, want)
+                const uint64_t lo = oflush > D0 + rg.skip ? oflush : D0 + rg.skip, hi = end < rstop ? end : rstop;
+                for (uint64_t i = lo + lane; i < hi; i += 32) dst[i - D0 - rg.skip] = S.out[i & (kOutRing - 1)];
+            } else {
+                for (uint64_t i = oflush + lane; i < end; i += 32) dst[i - D0] = S.out[i & (kOutRing - 1)];
+            }
             if (end > oflush) oflush = end;
             __syncwarp();
             if (cmd == C_DONE) break;
@@ -1472,6 +1512,9 @@ __global__ void __launch_bounds__(256) k_batch_verdict(const InfState *ist, cons
     out[i] = BatchResult{r.out_bytes, r.in_bytes, check, err};
 }
 
+struct IdxPiece;
+__global__ void __launch_bounds__(32) k_index_extract(const IdxPiece *pieces, InfState *st);
+
 static const char *inf_msg(uint32_t e)
 {
     switch (e) {
@@ -1507,6 +1550,8 @@ int Engine::inflate_init()
     if (e != cudaSuccess) { snprintf(g_err, sizeof g_err, "k_members attr: %s", cudaGetErrorString(e)); return ZB_E_CUDA; }
     e = cudaFuncSetAttribute(k_batch_members, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(InfShared));
     if (e != cudaSuccess) { snprintf(g_err, sizeof g_err, "k_batch_members attr: %s", cudaGetErrorString(e)); return ZB_E_CUDA; }
+    e = cudaFuncSetAttribute(k_index_extract, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(InfShared));
+    if (e != cudaSuccess) { snprintf(g_err, sizeof g_err, "k_index_extract attr: %s", cudaGetErrorString(e)); return ZB_E_CUDA; }
     if (cudaMalloc(&d_inf_state, sizeof(InfState)) != cudaSuccess) return ZB_E_MEM;
     if (cudaMallocHost(&h_inf_state, sizeof(InfState)) != cudaSuccess) return ZB_E_MEM;
     return ZB_OK;
@@ -1519,7 +1564,7 @@ int Engine::inflate_init()
     } while (0)
 
 int Engine::inflate(const void *src, size_t n, bool src_dev, void *dst, size_t dst_cap, bool dst_dev, int window_bits,
-                    zb_inflate_result *res, uint32_t flags)
+                    zb_inflate_result *res, uint32_t flags, IdxBuild *ib)
 {
     if (!res || (!src && n) || (!dst && dst_cap)) return ZB_E_PARAM;
     memset(res, 0, sizeof *res);
@@ -1543,9 +1588,14 @@ int Engine::inflate(const void *src, size_t n, bool src_dev, void *dst, size_t d
         d_dst = static_cast<uint8_t *>(p);
     }
     launches = 0;
-    const int status = (flags & ZB_INF_MEMBERS) ? inflate_members(d_src, n, d_dst, dst_cap, window_bits, res)
-                                                : inflate_stream(d_src, n, d_dst, dst_cap, window_bits, flags, res);
+    InfTrace *tr = ib ? &ib->tr : nullptr;
+    const int status = (flags & ZB_INF_MEMBERS) ? inflate_members(d_src, n, d_dst, dst_cap, window_bits, res, tr)
+                                                : inflate_stream(d_src, n, d_dst, dst_cap, window_bits, flags, res, tr);
     if (status != ZB_OK && status != ZB_E_BUF && status != ZB_E_DATA && status != ZB_E_DECLINED) return status;
+    if (ib && status == ZB_OK) { // zb_index_build: the points and their windows, from the output while it is on the device
+        if (!(flags & ZB_INF_MEMBERS)) tr->members.assign(1, TraceMember{IdxMember{0, res->in_bytes, 0, res->out_bytes}, std::move(tr->blocks)});
+        if ((rc = index_points(d_src, d_dst, res, window_bits, ib)) != ZB_OK) return rc;
+    }
     if (!dst_dev && res->out_bytes) CKI(cudaMemcpyAsync(dst, d_dst, res->out_bytes, cudaMemcpyDeviceToHost, st));
     CKI(cudaEventRecord(ev1, st));
     CKI(cudaStreamSynchronize(st));
@@ -1559,7 +1609,8 @@ int Engine::inflate(const void *src, size_t n, bool src_dev, void *dst, size_t d
 // Runs of BGZF members go through the batch (k_mem_* / k_members); a member the batch hands back, and any other member, through
 // inflate_stream at the current offset.  The error of a member is the one inflate_stream gives for it alone; out_bytes / in_bytes
 // and check cover the members in front of it.
-int Engine::inflate_members(const uint8_t *d_src, size_t n, uint8_t *d_dst, size_t dst_cap, int window_bits, zb_inflate_result *res)
+int Engine::inflate_members(const uint8_t *d_src, size_t n, uint8_t *d_dst, size_t dst_cap, int window_bits, zb_inflate_result *res,
+                            InfTrace *tr)
 {
     int rc;
     void *p;
@@ -1611,6 +1662,7 @@ int Engine::inflate_members(const uint8_t *d_src, size_t n, uint8_t *d_dst, size
     uint64_t in = 0, out = 0;
     uint32_t check = 0;
     int status = ZB_OK;
+    if (tr) tr->kind = 2;
     for (bool first = true;; first = false) {
         if (!first) { // another member only behind 1f 8b (gz_look)
             if (n - in < 2) break;
@@ -1636,6 +1688,17 @@ int Engine::inflate_members(const uint8_t *d_src, size_t n, uint8_t *d_dst, size
                 CKI(cudaStreamSynchronize(st));
                 CKI(cudaGetLastError());
                 check = (uint32_t)crc32_combine64(check, h_ctl.good_crc, (z_off64_t)h_ctl.good_out);
+                if (tr && h_ctl.good) { // the index build records where each member of the run lies
+                    std::vector<uint64_t> mo(h_ctl.good), mu(h_ctl.good);
+                    std::vector<uint32_t> ml(h_ctl.good), mi(h_ctl.good);
+                    CKI(cudaMemcpyAsync(mo.data(), d_moff, 8 * (size_t)h_ctl.good, cudaMemcpyDeviceToHost, st));
+                    CKI(cudaMemcpyAsync(mu.data(), d_mout, 8 * (size_t)h_ctl.good, cudaMemcpyDeviceToHost, st));
+                    CKI(cudaMemcpyAsync(ml.data(), d_mlen, 4 * (size_t)h_ctl.good, cudaMemcpyDeviceToHost, st));
+                    CKI(cudaMemcpyAsync(mi.data(), d_misz, 4 * (size_t)h_ctl.good, cudaMemcpyDeviceToHost, st));
+                    CKI(cudaStreamSynchronize(st));
+                    for (uint32_t m = 0; m < h_ctl.good; m++)
+                        tr->members.push_back(TraceMember{IdxMember{mo[m], mo[m] + ml[m], out + mu[m], out + mu[m] + mi[m]}, {}});
+                }
                 out += h_ctl.good_out;
                 in += h_ctl.good_in;
                 if (h_ctl.good == h_ctl.count) continue;
@@ -1644,7 +1707,7 @@ int Engine::inflate_members(const uint8_t *d_src, size_t n, uint8_t *d_dst, size
         }
         zb_inflate_result r;
         memset(&r, 0, sizeof r);
-        const int st1 = inflate_stream(d_src + in, n - in, d_dst + out, dst_cap - out, window_bits, 0, &r);
+        const int st1 = inflate_stream(d_src + in, n - in, d_dst + out, dst_cap - out, window_bits, 0, &r, tr);
         if (st1 != ZB_OK) {
             if (st1 != ZB_E_BUF && st1 != ZB_E_DATA) return st1;
             status = st1;
@@ -1652,6 +1715,7 @@ int Engine::inflate_members(const uint8_t *d_src, size_t n, uint8_t *d_dst, size
             break;
         }
         check = (uint32_t)crc32_combine64(check, r.check, (z_off64_t)r.out_bytes);
+        if (tr) tr->members.push_back(TraceMember{IdxMember{in, in + r.in_bytes, out, out + r.out_bytes}, std::move(tr->blocks)});
         out += r.out_bytes;
         in += r.in_bytes;
     }
@@ -1663,12 +1727,13 @@ int Engine::inflate_members(const uint8_t *d_src, size_t n, uint8_t *d_dst, size
 
 // One stream at d_src[0, n) into d_dst[0, dst_cap): the block-parallel path, or k_inflate; then the check value and the trailer.
 int Engine::inflate_stream(const uint8_t *d_src, size_t n, uint8_t *d_dst, size_t dst_cap, int window_bits, uint32_t flags,
-                           zb_inflate_result *res)
+                           zb_inflate_result *res, InfTrace *tr)
 {
     int rc;
     void *p;
     InfState *dis = static_cast<InfState *>(d_inf_state), *his = static_cast<InfState *>(h_inf_state);
     bool done = false;
+    if (tr) tr->blocks.clear();
     const char *declined = "small"; // the stage of the block-parallel path that gave up (reported with ZB_INF_NO_SERIAL)
     if (n >= 65536) {
         // block-parallel path; anything it cannot follow falls through to the serial decoder below
@@ -1752,6 +1817,12 @@ int Engine::inflate_stream(const uint8_t *d_src, size_t n, uint8_t *d_dst, size_
                     his->trailer_len = hpar.trailer_len;
                     his->kind = hpar.kind;
                     done = true;
+                    if (tr) { // the index build scans from these blocks
+                        std::vector<InfBlock> hb(hpar.nblocks);
+                        CKI(cudaMemcpyAsync(hb.data(), dblk, sizeof(InfBlock) * hb.size(), cudaMemcpyDeviceToHost, st));
+                        CKI(cudaStreamSynchronize(st));
+                        for (const InfBlock &b : hb) tr->blocks.push_back(IdxBlock{b.start_bit, b.out_off, b.out_len, b.type});
+                    }
                 }
             }
         }
@@ -1769,6 +1840,7 @@ int Engine::inflate_stream(const uint8_t *d_src, size_t n, uint8_t *d_dst, size_
     }
     res->out_bytes = his->out_bytes;
     res->in_bytes = his->in_bytes;
+    if (tr) tr->kind = his->kind;
     int status = ZB_OK;
     if (his->err == IE_OUTPUT_FULL) status = ZB_E_BUF;
     else if (his->err != IE_OK) { status = ZB_E_DATA; snprintf(res->msg, sizeof res->msg, "%s", inf_msg(his->err)); }
@@ -1952,6 +2024,359 @@ int Engine::inflate_blocks(const void *src, size_t n, uint64_t start_bit, const 
     CKI(cudaStreamSynchronize(st));
     CKI(cudaEventElapsedTime(&out->gpu_ms, ev0, ev1));
     out->gpu_launches = launches;
+    return status;
+}
+
+// ================================================================================================
+// Access-point index (zb_index_build / zb_index_extract, zb_index.h, DESIGN.md §2k)
+//   k_index_scan     one warp per job: from a block header, decode symbols without output (crossing block headers) and take, for each
+//                    of the job's targets k * S, the first access point at or after it.  A job is a member (k_inflate streams,
+//                    members of ZB_INF_MEMBERS; it also finds the member's first block behind the zlib / gzip header) or, for a
+//                    stream of the block-parallel path, a block of the InfBlock table that holds targets.  Each job scans its own
+//                    range once, so the work is linear in the stream's symbols.
+//   k_index_windows  one CTA per point: its window out of the device-side output.
+//   k_index_extract  one warp per piece of a range (a piece never crosses a member): inflate_warp<true> from the piece's point.
+// ================================================================================================
+struct IdxJob {
+    uint64_t start_bit, in_start, in_end, out_start; // start_bit: absolute; the member's input is [in_start, in_end)
+    uint64_t k0, k1;                                 // targets k * S, k in [k0, k1)
+    uint32_t member, kind, auto_start, unit;         // auto_start: start at the member's first block (kind: 0 raw, 1 zlib, 2 gzip)
+};
+struct IdxHit { uint64_t out_off, bit, hdr_bit; uint32_t btype, found; }; // found: member + 1, 0 when the job ran out
+
+__global__ void __launch_bounds__(32) k_index_scan(const uint8_t *__restrict__ src, const IdxJob *jobs, uint64_t span, IdxHit *starts,
+                                                   IdxHit *hits)
+{
+    __shared__ DecShared S;
+    if (threadIdx.x != 0) return;
+    const IdxJob j = jobs[blockIdx.x];
+    const uint8_t *s = src + j.in_start;
+    const uint64_t n = j.in_end - j.in_start, base = 8 * j.in_start, nbits = 8 * n;
+    const BitSrc bs{s, n};
+    uint64_t pos = j.start_bit - base;
+    if (j.auto_start) {
+        const int64_t hl = j.kind == 2 ? zbm_header_len(s, n) : j.kind == 1 ? 2 : 0;
+        pos = hl < 0 ? 0 : 8 * (uint64_t)hl;
+        starts[blockIdx.x] = IdxHit{j.out_start, base + pos, base + pos, (bs.peek32(pos) >> 1) & 3u, j.member + 1};
+    }
+    uint64_t k = j.k0, out = j.out_start;
+    auto visit = [&](uint64_t bit, uint64_t hb, uint32_t bt) {
+        for (; k < j.k1 && k * span <= out; k++) hits[k - 1] = IdxHit{out, base + bit, base + hb, bt, j.member + 1};
+    };
+    bool fixed_ready = false; // S.lencode / S.distcode hold the fixed codes
+    while (k < j.k1 && pos + 3 <= nbits) {
+        const uint32_t w = bs.peek32(pos), last = w & 1u, type = (w >> 1) & 3u;
+        const uint64_t hb = pos;
+        visit(hb, hb, type);
+        if (k >= j.k1 || type == 3) break;
+        if (type == 0) {
+            const uint64_t p = (pos + 3 + 7) & ~7ull;
+            const uint32_t len = bs.peek32(p) & 0xffffu;
+            out += len;
+            pos = p + 32 + 8ull * len;
+        } else {
+            BitRd br;
+            uint32_t lb, db, bf;
+            if (type == 2) {
+                if (dec_setup(S, s, n, hb, br, lb, db, &bf)) break;
+                fixed_ready = false;
+            } else {
+                uint32_t sym = 0;
+                while (sym < 144) S.lens[sym++] = 8;
+                while (sym < 256) S.lens[sym++] = 9;
+                while (sym < 280) S.lens[sym++] = 7;
+                while (sym < 288) S.lens[sym++] = 8;
+                if (!fixed_ready) inflate_table(1, S.lens, 288, S.lencode, 9, S.work, &lb);
+                for (sym = 0; sym < 32; sym++) S.lens[sym] = 5;
+                if (!fixed_ready) inflate_table(2, S.lens, 32, S.distcode, 5, S.work, &db);
+                fixed_ready = true;
+                lb = 9; db = 5;
+                br.init(s, n, hb + 3);
+            }
+            const uint32_t lm = (1u << lb) - 1, dm = (1u << db) - 1;
+            int t = 0;
+            while (k < j.k1) {
+                const uint64_t sb = br.consumed();
+                if (sb > nbits) { t = -1; break; }
+                uint32_t v, d;
+                t = dec_symbol(S, br, lm, dm, v, d);
+                if (t != 0 && t != 1) break;
+                visit(sb, hb, type);  // a literal or length symbol starts here (the end-of-block code is no access point)
+                out += t == 0 ? 1u : v;
+            }
+            if (t != 2) break;        // all targets taken, or damage (the decode that ran before has vouched for the stream)
+            pos = br.consumed();
+        }
+        if (last) break;
+    }
+}
+
+__global__ void __launch_bounds__(256) k_index_windows(const uint8_t *__restrict__ out, const IdxPoint *pts, const uint64_t *woff,
+                                                       uint8_t *__restrict__ win)
+{
+    const IdxPoint p = pts[blockIdx.x];
+    const uint8_t *w = out + p.out_off - p.window_len;
+    uint8_t *d = win + woff[blockIdx.x];
+    for (uint32_t i = threadIdx.x; i < p.window_len; i += 256) d[i] = w[i];
+}
+
+// One piece: the output [a, b) of one member, from the point at or in front of a.  Every pointer is into the staged input (or the
+// caller's device input), the piece's window and its place in dst.
+struct IdxPiece {
+    const uint8_t *body, *hdr, *win;
+    uint8_t *dst;
+    uint64_t body_n, hdr_n, start_bit, hdr_bit, skip, want; // start_bit / hdr_bit: relative to body / hdr
+    uint32_t btype, resume, win_len, pad;
+};
+
+__global__ void __launch_bounds__(32) k_index_extract(const IdxPiece *pieces, InfState *st)
+{
+    extern __shared__ __align__(16) uint8_t smem_raw[];
+    const IdxPiece pc = pieces[blockIdx.x];
+    inflate_warp<true>(*reinterpret_cast<InfShared *>(smem_raw), pc.body, pc.body_n, pc.dst, 1ull << 62, -15, st + blockIdx.x,
+                       InfSeg{pc.start_bit, pc.win, pc.win_len, 1}, InfDict{nullptr, nullptr, 0, 0},
+                       InfRange{pc.hdr, pc.hdr_n, pc.hdr_bit, pc.skip, pc.want, pc.btype, pc.resume});
+}
+
+static size_t a64(size_t b) { return (b + 63) & ~(size_t)63; }
+
+// The points of zb_index_build over the decoded stream (d_dst holds its res->out_bytes bytes) and their windows.  ib->tr lists the
+// members and the block tables of those the block-parallel path decoded.  Each target k * S goes to the first member that ends after
+// it or starts at or after it (then the member's start is the point).  Inside a member with a block table it goes on to the first
+// block that ends after it or starts at or after it (then that block's header is the point), and a job scans from that block;
+// inside any other member the member's job scans for it.  Every member has a job, which also finds its first block.  A target a
+// job does not reach before its member ends goes to the next member's start.  Launches: k_index_scan and k_index_windows; host
+// syncs: one for the scan's results (the block tables came back with the decode).  The windows arrive with the caller's final sync.
+int Engine::index_points(const uint8_t *d_src, const uint8_t *d_dst, const zb_inflate_result *res, int window_bits, IdxBuild *ib)
+{
+    int rc;
+    void *p;
+    const InfTrace &tr = ib->tr;
+    const uint64_t nm = tr.members.size(), S = ib->span, total = res->out_bytes, K = zbi_targets(total, S);
+    std::vector<IdxMember> M(nm);
+    for (uint64_t m = 0; m < nm; m++) M[m] = tr.members[m].m;
+    struct MemberUnits {
+        const IdxMember *m;
+        ZB_HD uint64_t start(uint64_t u) const { return m[u].out_start; }
+        ZB_HD uint64_t end(uint64_t u) const { return m[u].out_end; }
+    };
+    struct BlockUnits {
+        const IdxBlock *b;
+        ZB_HD uint64_t start(uint64_t u) const { return b[u].out_off; }
+        ZB_HD uint64_t end(uint64_t u) const { return b[u].out_off + b[u].out_len; }
+    };
+    constexpr uint32_t kNoBlock = 0xffffffffu;
+    std::vector<IdxJob> jobs; // jobs[m]: member m
+    for (uint64_t m = 0; m < nm; m++)
+        jobs.push_back(IdxJob{0, M[m].in_start, M[m].in_end, M[m].out_start, 1, 1, (uint32_t)m, tr.kind, 1, kNoBlock});
+    std::vector<IdxHit> known(K);       // targets whose point (a block header) the table gives
+    std::vector<int64_t> start_of(K, -1); // ... or that is a member's start
+    std::vector<int64_t> job_of(K, -1);   // ... or that a job looks for
+    for (uint64_t k = 1; k <= K; k++) {
+        const uint64_t T = k * S, u = zbi_unit_of(MemberUnits{M.data()}, nm, T);
+        if (u == nm) continue;
+        if (M[u].out_start >= T) { start_of[k - 1] = (int64_t)u; continue; }
+        const std::vector<IdxBlock> &B = tr.members[u].blocks;
+        const uint64_t Tr = T - M[u].out_start, b = B.empty() ? 0 : zbi_unit_of(BlockUnits{B.data()}, B.size(), Tr);
+        if (b < B.size()) {
+            const uint64_t hb = 8 * M[u].in_start + B[b].start_bit;
+            if (B[b].out_off >= Tr) { known[k - 1] = IdxHit{M[u].out_start + B[b].out_off, hb, hb, B[b].type, (uint32_t)u + 1}; continue; }
+            if (jobs.back().member != u || jobs.back().unit != b)
+                jobs.push_back(IdxJob{hb, M[u].in_start, M[u].in_end, M[u].out_start + B[b].out_off, k, k, (uint32_t)u, tr.kind, 0, (uint32_t)b});
+            jobs.back().k1 = k + 1;
+            job_of[k - 1] = (int64_t)jobs.size() - 1;
+            continue;
+        }
+        if (jobs[u].k0 == jobs[u].k1) jobs[u].k0 = k;
+        jobs[u].k1 = k + 1;
+        job_of[k - 1] = (int64_t)u;
+    }
+    const uint64_t nj = jobs.size();
+    std::vector<IdxHit> starts(nj), hits(K);
+    {
+        const size_t a_j = a64(sizeof(IdxJob) * nj), a_s = a64(sizeof(IdxHit) * nj), a_h = a64(sizeof(IdxHit) * K);
+        if ((rc = reserve(S_INDEX, a_j + a_s + a_h + 64, &p)) != ZB_OK) return rc;
+        uint8_t *t = static_cast<uint8_t *>(p);
+        IdxJob *d_jobs = reinterpret_cast<IdxJob *>(t);
+        IdxHit *d_starts = reinterpret_cast<IdxHit *>(t + a_j), *d_hits = reinterpret_cast<IdxHit *>(t + a_j + a_s);
+        CKI(cudaMemcpyAsync(d_jobs, jobs.data(), sizeof(IdxJob) * nj, cudaMemcpyHostToDevice, st));
+        CKI(cudaMemsetAsync(d_starts, 0, a_s + a_h, st));
+        k_index_scan<<<(unsigned)nj, 32, 0, st>>>(d_src, d_jobs, S, d_starts, d_hits);
+        launches += 1;
+        CKI(cudaMemcpyAsync(starts.data(), d_starts, sizeof(IdxHit) * nj, cudaMemcpyDeviceToHost, st));
+        if (K) CKI(cudaMemcpyAsync(hits.data(), d_hits, sizeof(IdxHit) * K, cudaMemcpyDeviceToHost, st));
+        CKI(cudaStreamSynchronize(st));
+        CKI(cudaGetLastError());
+    }
+    // the member starts, then each target's point; stream order is bit order
+    std::vector<IdxPoint> pts;
+    auto add = [&](const IdxHit &h) { pts.push_back(IdxPoint{h.out_off, h.bit, h.hdr_bit, h.found - 1, h.btype, 0, 0}); };
+    for (uint64_t m = 0; m < nm; m++) add(starts[m]);
+    for (uint64_t k = 1; k <= K; k++) {
+        if (start_of[k - 1] >= 0) add(starts[start_of[k - 1]]);
+        else if (known[k - 1].found) add(known[k - 1]);
+        else if (job_of[k - 1] >= 0) {
+            const uint64_t m = jobs[job_of[k - 1]].member;
+            if (hits[k - 1].found) add(hits[k - 1]);
+            else if (m + 1 < nm) add(starts[m + 1]); // the next member's start
+        }
+    }
+    for (const IdxPoint &q : pts)
+        if (q.member >= nm || q.btype > 2) { snprintf(g_err, sizeof g_err, "index build: a scan job did not finish"); return ZB_E_INTERNAL; }
+    std::sort(pts.begin(), pts.end(), [](const IdxPoint &a, const IdxPoint &b) { return a.bit < b.bit; });
+    pts.erase(std::unique(pts.begin(), pts.end(), [](const IdxPoint &a, const IdxPoint &b) { return a.bit == b.bit; }), pts.end());
+    zb_index &x = *ib->out;
+    x.m = M;
+    x.p = pts;
+    x.woff.resize(pts.size());
+    uint64_t win = 0;
+    for (size_t i = 0; i < pts.size(); i++) {
+        x.p[i].window_len = zbi_window_len(pts[i].out_off, M[pts[i].member].out_start);
+        x.woff[i] = win;
+        win += x.p[i].window_len;
+    }
+    x.h = IdxHeader{kIdxMagic, kIdxVersion, S, total, res->in_bytes, res->check, window_bits, nm, (uint64_t)pts.size(), win};
+    x.win.resize(win);
+    if (win) {
+        const size_t a_p = a64(sizeof(IdxPoint) * pts.size()), a_w = a64(8 * pts.size());
+        if ((rc = reserve(S_INDEX, a_p + a_w + 64, &p)) != ZB_OK) return rc; // the scan's buffers are done with
+        IdxPoint *d_pts = static_cast<IdxPoint *>(p);
+        uint64_t *d_woff = reinterpret_cast<uint64_t *>(static_cast<uint8_t *>(p) + a_p);
+        if ((rc = reserve(S_INDEXW, win + 64, &p)) != ZB_OK) return rc;
+        uint8_t *d_win = static_cast<uint8_t *>(p);
+        CKI(cudaMemcpyAsync(d_pts, x.p.data(), sizeof(IdxPoint) * pts.size(), cudaMemcpyHostToDevice, st));
+        CKI(cudaMemcpyAsync(d_woff, x.woff.data(), 8 * pts.size(), cudaMemcpyHostToDevice, st));
+        k_index_windows<<<(unsigned)pts.size(), 256, 0, st>>>(d_dst, d_pts, d_woff, d_win);
+        launches += 1;
+        CKI(cudaMemcpyAsync(x.win.data(), d_win, win, cudaMemcpyDeviceToHost, st));
+    }
+    return ZB_OK;
+}
+
+// zb_index_extract: see zb_engine.h.  One launch (k_index_extract over all pieces of all ranges) and one host sync.
+int Engine::index_extract(const zb_index *x, const void *src, size_t src_len, bool src_dev, const uint64_t *offsets, size_t n_ranges,
+                          void *dst, const uint64_t *dst_off, bool dst_dev, zb_inflate_result *items)
+{
+    if (!x || (n_ranges && (!offsets || !dst_off || !items))) { snprintf(g_err, sizeof g_err, "index_extract: null argument"); return ZB_E_PARAM; }
+    if (n_ranges > kIdxMaxRanges) { snprintf(g_err, sizeof g_err, "index_extract: %zu ranges (at most %llu)", n_ranges, (unsigned long long)kIdxMaxRanges); return ZB_E_PARAM; }
+    if (src_len < x->h.in_bytes || (!src && x->h.in_bytes)) { snprintf(g_err, sizeof g_err, "index_extract: the input is shorter than the indexed stream"); return ZB_E_PARAM; }
+    for (size_t i = 0; i < n_ranges; i++) {
+        if (dst_off[i + 1] < dst_off[i]) { snprintf(g_err, sizeof g_err, "index_extract: offsets of range %zu decrease", i); return ZB_E_PARAM; }
+        if (dst_off[i + 1] - dst_off[i] > 0xffffffffull) { snprintf(g_err, sizeof g_err, "index_extract: slot of range %zu is 4 GiB or more", i); return ZB_E_PARAM; }
+    }
+    const uint64_t out_total = n_ranges ? dst_off[n_ranges] - dst_off[0] : 0;
+    if (out_total && !dst) { snprintf(g_err, sizeof g_err, "index_extract: null buffer"); return ZB_E_PARAM; }
+    for (size_t i = 0; i < n_ranges; i++) memset(&items[i], 0, sizeof items[i]);
+    if (n_ranges == 0) return ZB_OK;
+    CKI(cudaSetDevice(device));
+    launches = 0;
+    const IdxPoint *P = x->p.data();
+    const IdxMember *M = x->m.data();
+    const uint64_t np = x->p.size(), nm = x->m.size(), total = x->h.total_out;
+    struct HostPiece { uint64_t range, pi, a, b; IdxSpan sp; };
+    std::vector<HostPiece> hp;
+    for (size_t i = 0; i < n_ranges; i++) {
+        const uint64_t off = offsets[i], slot = dst_off[i + 1] - dst_off[i];
+        const uint64_t ob = off < total ? (slot < total - off ? slot : total - off) : 0;
+        items[i].out_bytes = ob;
+        for (uint64_t a = off, e = off + ob; a < e;) { // split at member boundaries
+            const uint64_t m = zbi_member_at(M, nm, a), b = e < M[m].out_end ? e : M[m].out_end, pi = zbi_lookup(P, np, a);
+            hp.push_back(HostPiece{i, pi, a, b, zbi_piece_span(P, np, M, pi, b)});
+            a = b;
+        }
+    }
+    const uint64_t npc = hp.size();
+    // the input the pieces need: for a host source the union of their spans, staged back to back
+    struct Iv { uint64_t lo, hi, at; };
+    std::vector<Iv> iv;
+    uint64_t staged = 0;
+    if (!src_dev) {
+        for (const HostPiece &h : hp) {
+            if (h.sp.hdr_hi > h.sp.hdr_lo) iv.push_back(Iv{h.sp.hdr_lo, h.sp.hdr_hi, 0});
+            iv.push_back(Iv{h.sp.body_lo, h.sp.body_hi, 0});
+        }
+        std::sort(iv.begin(), iv.end(), [](const Iv &a, const Iv &b) { return a.lo < b.lo; });
+        std::vector<Iv> mg;
+        for (const Iv &v : iv) {
+            if (!mg.empty() && v.lo <= mg.back().hi) { if (v.hi > mg.back().hi) mg.back().hi = v.hi; }
+            else mg.push_back(v);
+        }
+        for (Iv &v : mg) { v.at = staged; staged += v.hi - v.lo; }
+        iv.swap(mg);
+    }
+    // the windows of the points in use, once each
+    std::vector<uint64_t> used;
+    for (const HostPiece &h : hp) used.push_back(h.pi);
+    std::sort(used.begin(), used.end());
+    used.erase(std::unique(used.begin(), used.end()), used.end());
+    std::vector<uint64_t> wat(used.size());
+    uint64_t wbytes = 0;
+    for (size_t u = 0; u < used.size(); u++) { wat[u] = wbytes; wbytes += P[used[u]].window_len; }
+    // S_INDEX: pieces | decoder states | windows | staged input
+    const size_t a_pc = a64(sizeof(IdxPiece) * npc), a_st = a64(sizeof(InfState) * npc), a_w = a64(wbytes);
+    int rc;
+    void *p;
+    if ((rc = reserve(S_INDEX, a_pc + a_st + a_w + staged + 64, &p)) != ZB_OK) return rc;
+    uint8_t *d_t = static_cast<uint8_t *>(p);
+    IdxPiece *d_pc = reinterpret_cast<IdxPiece *>(d_t);
+    InfState *d_st = reinterpret_cast<InfState *>(d_t + a_pc);
+    uint8_t *d_win = d_t + a_pc + a_st, *d_in = d_win + a_w;
+    uint8_t *d_dst = static_cast<uint8_t *>(dst) + dst_off[0];
+    if (!dst_dev) {
+        if ((rc = reserve(S_INF1, out_total + 64, &p)) != ZB_OK) return rc;
+        d_dst = static_cast<uint8_t *>(p);
+    }
+    // host stage: pieces | decoder states (room only) | windows | staged input, uploaded in one copy
+    if ((rc = stage(a_pc + a_st + a_w + staged + 64)) != ZB_OK) return rc;
+    uint8_t *h_t = static_cast<uint8_t *>(h_stage);
+    IdxPiece *h_pc = reinterpret_cast<IdxPiece *>(h_t);
+    for (size_t u = 0; u < used.size(); u++) memcpy(h_t + a_pc + a_st + wat[u], x->win.data() + x->woff[used[u]], P[used[u]].window_len);
+    for (const Iv &v : iv) memcpy(h_t + a_pc + a_st + a_w + v.at, static_cast<const uint8_t *>(src) + v.lo, v.hi - v.lo);
+    auto in_ptr = [&](uint64_t lo) -> const uint8_t * {
+        if (src_dev) return static_cast<const uint8_t *>(src) + lo;
+        const Iv &v = *(std::upper_bound(iv.begin(), iv.end(), lo, [](uint64_t o, const Iv &w) { return o < w.lo; }) - 1);
+        return d_in + v.at + (lo - v.lo);
+    };
+    for (uint64_t k = 0; k < npc; k++) {
+        const HostPiece &h = hp[k];
+        const IdxPoint &pt = P[h.pi];
+        const size_t u = std::lower_bound(used.begin(), used.end(), h.pi) - used.begin();
+        const bool resume = pt.bit != pt.hdr_bit;
+        h_pc[k] = IdxPiece{in_ptr(h.sp.body_lo), resume ? in_ptr(h.sp.hdr_lo) : nullptr, d_win + wat[u],
+                           d_dst + (dst_off[h.range] - dst_off[0]) + (h.a - offsets[h.range]), h.sp.body_hi - h.sp.body_lo,
+                           h.sp.hdr_hi - h.sp.hdr_lo, pt.bit - 8 * h.sp.body_lo, pt.hdr_bit - 8 * h.sp.hdr_lo, h.a - pt.out_off, h.b - h.a,
+                           pt.btype, resume ? 1u : 0u, pt.window_len, 0};
+    }
+    CKI(cudaEventRecord(ev0, st));
+    if (!dst_dev) CKI(cudaMemsetAsync(d_dst, 0, out_total, st)); // the slots go back whole: behind a range's bytes there are zeros
+    CKI(cudaMemcpyAsync(d_pc, h_pc, a_pc, cudaMemcpyHostToDevice, st));
+    if (a_w + staged) CKI(cudaMemcpyAsync(d_win, h_t + a_pc + a_st, a_w + staged, cudaMemcpyHostToDevice, st));
+    if (npc) {
+        k_index_extract<<<(unsigned)npc, 32, sizeof(InfShared), st>>>(d_pc, d_st);
+        launches += 1;
+    }
+    std::vector<InfState> hs(npc);
+    if (npc) CKI(cudaMemcpyAsync(hs.data(), d_st, sizeof(InfState) * npc, cudaMemcpyDeviceToHost, st));
+    if (!dst_dev && out_total) CKI(cudaMemcpyAsync(static_cast<uint8_t *>(dst) + dst_off[0], d_dst, out_total, cudaMemcpyDeviceToHost, st));
+    CKI(cudaEventRecord(ev1, st));
+    CKI(cudaStreamSynchronize(st));
+    CKI(cudaGetLastError());
+    float ms = 0;
+    CKI(cudaEventElapsedTime(&ms, ev0, ev1));
+    for (uint64_t k = 0; k < npc; k++) {
+        zb_inflate_result &r = items[hp[k].range];
+        const InfState &s = hs[k];
+        if (r.status != ZB_OK) continue;
+        // the piece's output must reach its end: a decode that stopped short (the final block ended) met damaged input
+        const uint32_t e = s.err != IE_OK ? s.err : s.out_bytes < h_pc[k].skip + h_pc[k].want ? (uint32_t)IE_TRUNCATED : (uint32_t)IE_OK;
+        if (e != IE_OK) { r.status = ZB_E_DATA; snprintf(r.msg, sizeof r.msg, "%s", inf_msg(e)); }
+    }
+    int status = ZB_OK;
+    for (size_t i = 0; i < n_ranges; i++) {
+        items[i].gpu_launches = launches;
+        items[i].gpu_ms = ms;
+        if (status == ZB_OK) status = items[i].status;
+    }
     return status;
 }
 
