@@ -263,6 +263,22 @@ typedef struct zb_index_point {
 } zb_index_point;
 ZB_API int zb_index_build(zb_engine *e, const void *src, size_t src_len, int src_on_device, void *dst, size_t dst_cap, int dst_on_device,
                           int window_bits, uint32_t flags, uint64_t span, zb_inflate_result *res, zb_index **out);
+/* zb_deflate_index: zb_deflate_ex plus the index of the stream it writes, built from the writer's own blocks and symbols without a
+ *   decode (DESIGN.md §2l).  For the same arguments it returns the same code, the same bytes in dst and the same res as
+ *   zb_deflate_ex, every error included (gpu_launches and gpu_ms aside).  Only on ZB_OK *out is an index (else *out = NULL), and it
+ *   serializes to exactly the bytes zb_index_build gives for the stream just written with the same span and
+ *     window_bits 15 for zlib framing (window_bits 9..15), -15 for raw (-9..-15), 31 for gzip (25..31) and for ZB_FLAG_BGZF;
+ *     flags ZB_INF_MEMBERS for ZB_FLAG_BGZF (every member indexed, the 28-byte end-of-file member and its point included), else 0;
+ *   header, members, points and windows alike (in_bytes, check and window_bits are the build's: a raw stream's check is 1).
+ *   Accepted: every level, strategy and window size zb_deflate_ex accepts, and the flags ZB_FLAG_MEMLEVEL(m), ZB_FLAG_LOW_PARALLEL,
+ *   ZB_FLAG_CHECK_ADLER, ZB_FLAG_CHECK_CRC and ZB_FLAG_BGZF (with its own parameter rules).  ZB_FLAG_NOT_LAST, ZB_FLAG_END_PARTIAL,
+ *   ZB_FLAG_END_BLOCK and ZB_FLAG_PRIME give ZB_E_PARAM (a segment is not a stream to index), as does a span outside
+ *   [32768, 2^32]; *out stays NULL.  Preset dictionaries have no such call (zb_index_build refuses their streams).  Cost over
+ *   zb_deflate_ex: 2 kernel launches and 1 host sync, whatever the span and the input length.  The index is the object
+ *   zb_index_build returns: extract, serialize, get_point and free it the same way. */
+ZB_API int zb_deflate_index(zb_engine *e, const void *src, size_t src_len, int src_on_device, void *dst, size_t dst_cap,
+                            int dst_on_device, int level, int strategy, int window_bits, uint32_t flags, uint64_t span,
+                            zb_deflate_result *res, zb_index **out);
 ZB_API int zb_index_extract(zb_engine *e, const zb_index *idx, const void *src, size_t src_len, int src_on_device, const uint64_t *offsets,
                             size_t n_ranges, void *dst, const uint64_t *dst_off, int dst_on_device, zb_inflate_result *items);
 ZB_API int zb_index_serialize(const zb_index *idx, void *buf, size_t cap, size_t *len);

@@ -158,6 +158,9 @@ def lib():
             L.zb_index_get_info.argtypes = [vp, ctypes.POINTER(IndexInfo)]
             L.zb_index_get_point.argtypes = [vp, sz, ctypes.POINTER(IndexPoint)]
             L.zb_index_free.argtypes, L.zb_index_free.restype = [vp], None
+        if hasattr(L, "zb_deflate_index"):
+            L.zb_deflate_index.argtypes = [vp, vp, sz, ci, vp, sz, ci, ci, ci, ci, u32, u64, ctypes.POINTER(DeflateResult),
+                                           ctypes.POINTER(vp)]
         if hasattr(L, "zb_deflate_batch_dict"):
             L.zb_deflate_batch_dict.argtypes = [vp, vp, sz] + L.zb_deflate_batch.argtypes[1:]
             L.zb_inflate_batch_dict.argtypes = [vp, vp, sz] + L.zb_inflate_batch.argtypes[1:]
@@ -504,6 +507,34 @@ class Engine:
                                  window_bits, flags, ctypes.byref(res))
         self._check(rc)
         return (own.raw[: res.out_bytes] if own is not None else None), res
+
+    def deflate_indexed(self, src, span=1 << 20, level=6, strategy=0, window_bits=15, flags=0, mem_level=8, n=None,
+                        src_on_device=False, dst=None, dst_cap=0, dst_on_device=False):
+        """Engine.deflate plus the access-point index of the stream it writes (zb_deflate_index), built from the writer's own
+        blocks without decoding it: the Index that Engine.build_index gives for that stream with the same span.  Returns
+        (bytes or None, DeflateResult, Index).  Raises ZlibError as Engine.deflate does (.needed: the size a too small dst_cap
+        would have to be)."""
+        res = DeflateResult()
+        flags |= (mem_level & 15) << 8
+        keep = None
+        if not src_on_device:
+            data, keep = _buf(src)
+            n = len(data)
+            src = ctypes.addressof(keep)
+        own = None
+        if dst is None:
+            dst_cap = (lib().zb_bgzf_bound(n) if flags & ZB_FLAG_BGZF else lib().zb_deflate_bound(n)) + 64
+            own = ctypes.create_string_buffer(dst_cap)
+            dst = ctypes.addressof(own)
+            dst_on_device = False
+        h = ctypes.c_void_p()
+        rc = lib().zb_deflate_index(self.h, src, n, int(src_on_device), dst, dst_cap, int(dst_on_device), level, strategy,
+                                    window_bits, flags, span, ctypes.byref(res), ctypes.byref(h))
+        if rc != 0:
+            e = ZlibError(rc, lib().zb_last_error().decode())
+            e.needed = res.out_bytes
+            raise e
+        return (own.raw[: res.out_bytes] if own is not None else None), res, Index(h.value)
 
     def inflate(self, src, out_cap, n=None, window_bits=15, src_on_device=False, dst=None, dst_on_device=False, flags=0):
         """Returns (rc, bytes or None, InflateResult).  flags: ZB_INF_*."""

@@ -74,6 +74,7 @@ __global__ void k_bgzf_encode(JobBufs, BgzfJob);
 __global__ void k_bgzf_frame(JobBufs, BgzfJob);
 __global__ void k_batch_stage(const uint8_t *, const uint64_t *, const uint8_t *, BgzfJob, uint8_t *, uint64_t);
 __global__ void k_batch_dict_ghost(JobBufs, BgzfJob);
+__global__ void k_deflate_points(JobBufs, BgzfJob, IdxWriteJob); // zb_deflate_index (zb_kernels.cu)
 
 constexpr uint32_t kMatchSmemBytes = (kWSize + kMatchSub + 512) + (kWSize + kMatchSub) * 2 + ((kWSize + kMatchSub) / 32 + 1) * 4 * 4 + 8192;
 constexpr uint32_t kPathSmemBytes = kPathTile * 4 * 3;
@@ -193,7 +194,7 @@ int Engine::stage(size_t bytes)
 size_t deflate_bound(size_t n) { return (size_t)stream_bound(n); } // zb_bgzf.h
 
 int Engine::deflate(const void *src, size_t n_in, bool src_dev, void *dst, size_t dst_cap, bool dst_dev, int level, int strategy,
-                    int window_bits, uint32_t flags, zb_deflate_result *res, const void *dict, size_t dict_len)
+                    int window_bits, uint32_t flags, zb_deflate_result *res, const void *dict, size_t dict_len, IdxWrite *iw)
 {
     // A preset dictionary (deflate::set_dictionary, deflate.rs:498-564) is the input's prefix in the window: the kernels work on
     // dictionary ++ input in absolute coordinates and start parsing at `dstart`.  A dictionary that would fill the window
@@ -205,7 +206,7 @@ int Engine::deflate(const void *src, size_t n_in, bool src_dev, void *dst, size_
             snprintf(g_err, sizeof g_err, "ZB_FLAG_BGZF takes window_bits 31, Z_DEFAULT_STRATEGY, level -1..9 and no other flag");
             return ZB_E_PARAM;
         }
-        return deflate_bgzf(src, n_in, src_dev, dst, dst_cap, dst_dev, level, res);
+        return deflate_bgzf(src, n_in, src_dev, dst, dst_cap, dst_dev, level, res, iw);
     }
     size_t dstart = 0;
     if (dict_len) {
@@ -650,6 +651,14 @@ int Engine::deflate(const void *src, size_t n_in, bool src_dev, void *dst, size_
         res->out_bytes = out_bytes;
         return ZB_E_BUF;
     }
+    if (iw) { // zb_deflate_index: the index that zb_index_build gives for this stream (window_bits 15 / -15 / 31, no flags)
+        IdxWriteJob w{iw->span, zbi_targets(n, iw->span), n, 1, 0, level == 0 ? 1u : 0u, 0, nullptr, nullptr};
+        const IdxHeader h{kIdxMagic, kIdxVersion, iw->span, n, out_bytes, wrap ? h_info->adler : 1u, wrap == 0 ? -15 : wrap == 1 ? 15 : 31,
+                          0, 0, 0};
+        BgzfJob bj;
+        memset(&bj, 0, sizeof bj);
+        if ((rc = index_written(jb, bj, w, h, iw)) != ZB_OK) return rc;
+    }
     if (d_out != dst) {
         pbegin();
         CK(cudaMemcpyAsync(dst, d_out, out_bytes, dst_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
@@ -787,7 +796,8 @@ int Engine::members_launch(JobBufs &jb, BgzfJob &bj, int level, uint32_t *d_freq
 // ZB_FLAG_BGZF (zb_bgzf.h, DESIGN.md §2h): every 65280-byte block of the input is deflated alone and framed as one BGZF member.  The
 // members are staged side by side and every kernel covers all of them, so a call costs a fixed number of launches and two host
 // syncs (the file length, then the end of the copy) whatever its length.
-int Engine::deflate_bgzf(const void *src, size_t n, bool src_dev, void *dst, size_t dst_cap, bool dst_dev, int level, zb_deflate_result *res)
+int Engine::deflate_bgzf(const void *src, size_t n, bool src_dev, void *dst, size_t dst_cap, bool dst_dev, int level, zb_deflate_result *res,
+                         IdxWrite *iw)
 {
     if (!res || (!src && n) || !dst) return ZB_E_PARAM;
     memset(res, 0, sizeof *res);
@@ -836,6 +846,11 @@ int Engine::deflate_bgzf(const void *src, size_t n, bool src_dev, void *dst, siz
     if (out_bytes > dst_cap) {
         res->out_bytes = out_bytes;
         return ZB_E_BUF;
+    }
+    if (iw) { // zb_deflate_index: the index of zb_index_build with window_bits 31 and ZB_INF_MEMBERS, the end-of-file member included
+        IdxWriteJob w{iw->span, zbi_targets(n, iw->span), n, nm + 1, 1, 0, 0, nullptr, nullptr};
+        const IdxHeader h{kIdxMagic, kIdxVersion, iw->span, n, out_bytes, *h_crc, 31, 0, 0, 0};
+        if ((rc = index_written(jb, bj, w, h, iw)) != ZB_OK) return rc;
     }
     CK(cudaMemcpyAsync(dst, jb.out, out_bytes, dst_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
     CK(cudaEventRecord(ev1, st));
@@ -1011,6 +1026,34 @@ int Engine::deflate_batch(const void *dict, size_t dict_len, const void *src, co
     res->gpu_launches = launches;
     res->gpu_ms = ms;
     return ZB_OK;
+}
+
+// zb_deflate_index (DESIGN.md §2l): the access points of the stream just written, from the writer's block tables on the device.  One
+// launch of k_deflate_points over the targets and the members' first headers, one host sync for its candidates and the member
+// table, then index_fill: one launch of k_index_windows, whose windows come out of the staged input with the caller's final sync.
+// Needs no pinned staging (h_stage may hold the caller's results).
+int Engine::index_written(const JobBufs &jb, const BgzfJob &bj, const IdxWriteJob &job, const IdxHeader &h, IdxWrite *iw)
+{
+    int rc;
+    void *p;
+    IdxWriteJob w = job;
+    const uint64_t ns = w.K + w.nm;
+    const size_t a_c = (sizeof(IdxCand) * ns + 63) & ~(size_t)63;
+    if ((rc = reserve(S_INDEX, a_c + sizeof(IdxMember) * w.nm + 64, &p)) != ZB_OK) return rc;
+    w.cand = static_cast<IdxCand *>(p);
+    w.members = reinterpret_cast<IdxMember *>(static_cast<uint8_t *>(p) + a_c);
+    k_deflate_points<<<(unsigned)((ns + 7) / 8), 256, 0, st>>>(jb, bj, w);
+    launches++;
+    std::vector<IdxCand> c(ns);
+    std::vector<IdxMember> M(w.nm);
+    CK(cudaMemcpyAsync(c.data(), w.cand, sizeof(IdxCand) * ns, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(M.data(), w.members, sizeof(IdxMember) * w.nm, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    CK(cudaGetLastError());
+    std::vector<IdxPoint> pts;
+    for (const IdxCand &q : c)
+        if (q.found) pts.push_back(IdxPoint{q.out_off, q.bit, q.hdr_bit, q.member, q.btype, 0, 0});
+    return index_fill(*iw->out, std::move(M), std::move(pts), h, jb.in, w.bgzf ? kBgzfStride - kBgzfBlock : 0);
 }
 
 int Engine::checksum(bool crc, uint32_t start, const void *buf, size_t len, bool on_dev, uint32_t *out, float *ms_out)
@@ -1201,6 +1244,33 @@ int zb_index_build(zb_engine *z, const void *src, size_t src_len, int src_dev, v
     }
     if (rc == ZB_OK) *out = ib.out;
     else delete ib.out;
+    return rc;
+}
+
+int zb_deflate_index(zb_engine *z, const void *src, size_t src_len, int src_dev, void *dst, size_t cap, int dst_dev, int level, int strategy,
+                     int window_bits, uint32_t flags, uint64_t span, zb_deflate_result *res, zb_index **out)
+{
+    if (!z) return ZB_E_NODEVICE;
+    if (!out) return ZB_E_PARAM;
+    *out = nullptr;
+    if (flags & (ZB_FLAG_NOT_LAST | ZB_FLAG_END_PARTIAL | ZB_FLAG_END_BLOCK | ZB_FLAG_PRIME(7, 0xff))) {
+        snprintf(zb::g_err, sizeof zb::g_err, "deflate_index: a segment (NOT_LAST, END_*, PRIME) is not a stream to index");
+        return ZB_E_PARAM;
+    }
+    if (span < zb::kIdxMinSpan || span > zb::kIdxMaxSpan) { snprintf(zb::g_err, sizeof zb::g_err, "deflate_index: span %llu outside [32768, 2^32]", (unsigned long long)span); return ZB_E_PARAM; }
+    z->e.shard.phase = 0; // a range job in progress is gone (its buffers are reused)
+    zb::IdxWrite iw;
+    iw.span = span;
+    iw.out = new (std::nothrow) zb_index;
+    if (!iw.out) return ZB_E_MEM;
+    int rc;
+    try {
+        rc = z->e.deflate(src, src_len, src_dev != 0, dst, cap, dst_dev != 0, level, strategy, window_bits, flags, res, nullptr, 0, &iw);
+    } catch (const std::bad_alloc &) {
+        rc = ZB_E_MEM;
+    }
+    if (rc == ZB_OK) *out = iw.out;
+    else delete iw.out;
     return rc;
 }
 

@@ -56,6 +56,11 @@ struct IdxBuild {
     InfTrace tr;
     zb_index *out = nullptr;
 };
+// What zb_deflate_index asks of a deflate call: the index of the stream it writes, with points every `span` output bytes.
+struct IdxWrite {
+    uint64_t span = 0;
+    zb_index *out = nullptr;
+};
 
 struct Engine {
     static constexpr int kSlots = 44;
@@ -91,8 +96,11 @@ struct Engine {
     int reserve(int slot, size_t bytes, void **out);
     int stage(size_t bytes);
     int deflate(const void *src, size_t n, bool src_dev, void *dst, size_t dst_cap, bool dst_dev, int level, int strategy,
-                int window_bits, uint32_t flags, zb_deflate_result *res, const void *dict = nullptr, size_t dict_len = 0);
-    int deflate_bgzf(const void *src, size_t n, bool src_dev, void *dst, size_t dst_cap, bool dst_dev, int level, zb_deflate_result *res);
+                int window_bits, uint32_t flags, zb_deflate_result *res, const void *dict = nullptr, size_t dict_len = 0,
+                IdxWrite *iw = nullptr);
+    int deflate_bgzf(const void *src, size_t n, bool src_dev, void *dst, size_t dst_cap, bool dst_dev, int level, zb_deflate_result *res,
+                     IdxWrite *iw = nullptr);
+    int index_written(const JobBufs &jb, const BgzfJob &bj, const IdxWriteJob &w, const IdxHeader &h, IdxWrite *iw);
     int deflate_batch(const void *dict, size_t dict_len, const void *src, const uint64_t *src_off, size_t n_items, bool src_dev, void *dst,
                       size_t dst_cap, bool dst_dev, int level, int strategy, int window_bits, uint32_t flags, uint64_t *dst_off,
                       uint32_t *checks, zb_deflate_result *res);
@@ -106,6 +114,8 @@ struct Engine {
     int inflate_members(const uint8_t *d_src, size_t n, uint8_t *d_dst, size_t dst_cap, int window_bits, zb_inflate_result *res,
                         InfTrace *tr = nullptr);
     int index_points(const uint8_t *d_src, const uint8_t *d_dst, const zb_inflate_result *res, int window_bits, IdxBuild *ib);
+    int index_fill(zb_index &x, std::vector<IdxMember> &&M, std::vector<IdxPoint> &&pts, const IdxHeader &h, const uint8_t *d_src,
+                   uint64_t shift);
     int index_extract(const zb_index *x, const void *src, size_t src_len, bool src_dev, const uint64_t *offsets, size_t n_ranges,
                       void *dst, const uint64_t *dst_off, bool dst_dev, zb_inflate_result *items);
     int inflate_batch(const void *dict, size_t dict_len, const void *src, const uint64_t *src_off, size_t n_items, bool src_dev, void *dst,

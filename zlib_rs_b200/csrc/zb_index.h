@@ -1,8 +1,10 @@
 // zb_index.h -- random access into deflate, zlib and gzip streams: the access-point rule, the serialized index, its validation,
 // the lookup from an output offset to its point and the input a range needs (zb_index_* in zb_engine.h, DESIGN.md §2k).
 //
-// Like zb_members.h this is `__host__ __device__`: the index kernels of zb_inflate.cu use it, the host code of the engine uses it,
-// and tests/indexmodel compiles the same source for the CPU (with AddressSanitizer and UBSan) so the CPU tests check it.
+// Like zb_members.h this is `__host__ __device__`: the index kernels of zb_inflate.cu and the writer's k_deflate_points (zb_kernels.cu,
+// zb_deflate_index) use it, the host code of the engine uses it,
+// and tests/indexmodel and tests/writerindexmodel compile the same source for the CPU (with AddressSanitizer and UBSan) so the CPU
+// tests check it.
 //
 // An access point is a position in the compressed input where raw-block decoding can resume, given the 32 KiB of output in front
 // of it: the bit where a block's 3 header bits start (any block type), or the bit where a literal or length symbol starts inside a
@@ -80,6 +82,53 @@ template <typename Units>
 ZB_HD uint64_t zbi_unit_of(const Units &units, uint64_t n, uint64_t T)
 {
     return zbi_first(n, [&](uint64_t u) { return units.end(u) > T || units.start(u) >= T; });
+}
+
+// The rule as a writer applies it (zb_deflate_index, DESIGN.md §2l): the encoder knows its units, so it picks the point without
+// decoding.  A unit is a deflate block or a piece of deflate_quick's one static block (encoded one sym_buf at a time: only the
+// first piece carries the block header, only the last one the end-of-block code).  `units` lists one member's units in stream
+// order with
+//   start(u), end(u)  output range, member-relative
+//   header(u)         u starts with a block header (false for a deflate_quick piece after the first)
+//   type(u)           0 stored, 1 fixed, 2 dynamic
+//   nsyms(u)          literal and length symbols of u (their starts are the access points inside it)
+//   sym_pos(u, i)     output offset of symbol i of u, member-relative, increasing along i
+// The pick is a unit and either its header (sym == kIdxHeader) or its symbol `sym`; unit == n when the member holds no access point
+// at or after T.
+constexpr uint64_t kIdxHeader = ~0ull;
+struct IdxPick { uint64_t unit, sym; };
+template <typename Units>
+ZB_HD IdxPick zbi_pick(const Units &units, uint64_t n, uint64_t T)
+{
+    uint64_t u = zbi_unit_of(units, n, T);
+    if (u < n && units.start(u) < T) { // T inside u: its first symbol at or after T; a stored payload holds no point
+        const uint64_t ns = units.type(u) ? units.nsyms(u) : 0;
+        const uint64_t i = zbi_first(ns, [&](uint64_t k) { return units.sym_pos(u, k) >= T; });
+        if (i < ns) return IdxPick{u, i};
+        u++;                           // e.g. a match that ends the block covers T
+    }
+    for (; u < n; u++) {               // the first unit from u on that holds a point; a piece with only the end-of-block code holds none
+        if (units.header(u)) return IdxPick{u, kIdxHeader};
+        if (units.nsyms(u)) return IdxPick{u, 0};
+    }
+    return IdxPick{n, 0};
+}
+
+// ... over the members of a stream (one, or those of a BGZF file).  `members` has start(m), end(m) (output offsets in the whole
+// output), n_units(m) and pick(m, T) = zbi_pick over member m's units for a member-relative T.  A target goes to the first member
+// that ends after it or starts at or after it (zbi_unit_of); a member that holds no point at or after it hands it to the next
+// member's first header.  *m = nm: the target has no point (past the last point of the stream).
+template <typename Members>
+ZB_HD IdxPick zbi_pick_members(const Members &members, uint64_t nm, uint64_t T, uint64_t *m)
+{
+    uint64_t k = zbi_unit_of(members, nm, T);
+    if (k < nm && members.start(k) < T) {
+        const IdxPick p = members.pick(k, T - members.start(k));
+        if (p.unit < members.n_units(k)) { *m = k; return p; }
+        k++;
+    }
+    *m = k;
+    return k < nm ? members.pick(k, 0) : IdxPick{0, 0};
 }
 
 // Index of the last point with out_off <= off (points sorted); n_points when there is none.

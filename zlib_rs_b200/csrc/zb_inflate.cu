@@ -2223,30 +2223,49 @@ int Engine::index_points(const uint8_t *d_src, const uint8_t *d_dst, const zb_in
     }
     for (const IdxPoint &q : pts)
         if (q.member >= nm || q.btype > 2) { snprintf(g_err, sizeof g_err, "index build: a scan job did not finish"); return ZB_E_INTERNAL; }
+    return index_fill(*ib->out, std::move(M), std::move(pts), IdxHeader{kIdxMagic, kIdxVersion, S, total, res->in_bytes, res->check,
+                                                                         window_bits, 0, 0, 0}, d_dst, 0);
+}
+
+// The index of a stream from its members and its points (in any order, a point may come twice), for both producers: the build
+// (index_points) and the writer (zb_deflate_index).  Sorts the points by bit and drops duplicates, sets their window lengths and
+// offsets and the header's counts (h gives the rest), and gathers the windows with k_index_windows into x.win, which the caller's
+// final sync brings back.  Point p's window is the window_len bytes in front of d_src + p.out_off + p.member * shift: the decoded
+// output (shift 0), or a writer's staged input (BGZF members are staged kBgzfStride apart and hold kBgzfBlock output bytes each).
+int Engine::index_fill(zb_index &x, std::vector<IdxMember> &&M, std::vector<IdxPoint> &&pts, const IdxHeader &h, const uint8_t *d_src,
+                       uint64_t shift)
+{
+    int rc;
+    void *p;
     std::sort(pts.begin(), pts.end(), [](const IdxPoint &a, const IdxPoint &b) { return a.bit < b.bit; });
     pts.erase(std::unique(pts.begin(), pts.end(), [](const IdxPoint &a, const IdxPoint &b) { return a.bit == b.bit; }), pts.end());
-    zb_index &x = *ib->out;
-    x.m = M;
-    x.p = pts;
-    x.woff.resize(pts.size());
+    x.m = std::move(M);
+    x.p = std::move(pts);
+    const size_t np = x.p.size();
+    x.woff.resize(np);
     uint64_t win = 0;
-    for (size_t i = 0; i < pts.size(); i++) {
-        x.p[i].window_len = zbi_window_len(pts[i].out_off, M[pts[i].member].out_start);
+    for (size_t i = 0; i < np; i++) {
+        x.p[i].window_len = zbi_window_len(x.p[i].out_off, x.m[x.p[i].member].out_start);
         x.woff[i] = win;
         win += x.p[i].window_len;
     }
-    x.h = IdxHeader{kIdxMagic, kIdxVersion, S, total, res->in_bytes, res->check, window_bits, nm, (uint64_t)pts.size(), win};
+    x.h = h;
+    x.h.n_members = x.m.size();
+    x.h.n_points = np;
+    x.h.win_bytes = win;
     x.win.resize(win);
     if (win) {
-        const size_t a_p = a64(sizeof(IdxPoint) * pts.size()), a_w = a64(8 * pts.size());
+        std::vector<IdxPoint> at(x.p); // where each window ends in d_src
+        for (IdxPoint &q : at) q.out_off += q.member * shift;
+        const size_t a_p = a64(sizeof(IdxPoint) * np), a_w = a64(8 * np);
         if ((rc = reserve(S_INDEX, a_p + a_w + 64, &p)) != ZB_OK) return rc; // the scan's buffers are done with
         IdxPoint *d_pts = static_cast<IdxPoint *>(p);
         uint64_t *d_woff = reinterpret_cast<uint64_t *>(static_cast<uint8_t *>(p) + a_p);
         if ((rc = reserve(S_INDEXW, win + 64, &p)) != ZB_OK) return rc;
         uint8_t *d_win = static_cast<uint8_t *>(p);
-        CKI(cudaMemcpyAsync(d_pts, x.p.data(), sizeof(IdxPoint) * pts.size(), cudaMemcpyHostToDevice, st));
-        CKI(cudaMemcpyAsync(d_woff, x.woff.data(), 8 * pts.size(), cudaMemcpyHostToDevice, st));
-        k_index_windows<<<(unsigned)pts.size(), 256, 0, st>>>(d_dst, d_pts, d_woff, d_win);
+        CKI(cudaMemcpyAsync(d_pts, at.data(), sizeof(IdxPoint) * np, cudaMemcpyHostToDevice, st));
+        CKI(cudaMemcpyAsync(d_woff, x.woff.data(), 8 * np, cudaMemcpyHostToDevice, st));
+        k_index_windows<<<(unsigned)np, 256, 0, st>>>(d_src, d_pts, d_woff, d_win);
         launches += 1;
         CKI(cudaMemcpyAsync(x.win.data(), d_win, win, cudaMemcpyDeviceToHost, st));
     }

@@ -1982,4 +1982,102 @@ __global__ void k_links_dict_ghost_apply(JobBufs jb, const uint32_t *first)
     if (x != 0xffffffffu) jb.L[x] = (uint16_t)(x - (jb.start - 3)); // before Lr is copied from L
 }
 
+// ------------------------------------------------------------------------------------------------
+// zb_deflate_index (zb_index.h, DESIGN.md §2l): the access points of the stream just written, from the writer's own block tables.
+// ------------------------------------------------------------------------------------------------
+// The units of one member for zbi_pick: its deflate blocks (bit_base absolute), or headers that follow the stored-block rule of
+// zb_core.h (level 0, a BGZF member written stored) -- and, with rule_type 1, the empty static block of BGZF's end-of-file member.
+struct WriterUnits {
+    const BlockDesc *b;  // nullptr: the stored rule from byte0
+    const Sym *syms;
+    uint64_t out0;       // staged offset of the member's first input byte (BlockDesc::in_start is staged)
+    uint64_t len;        // the member's output bytes
+    uint64_t byte0;      // stored rule: the byte of the first block header
+    uint32_t rule_type, nb;
+    __device__ uint64_t start(uint64_t u) const { return b ? b[u].in_start - out0 : u * kStoredMax; }
+    __device__ uint64_t end(uint64_t u) const { return b ? b[u].in_start + b[u].in_len - out0 : min(len, (u + 1) * kStoredMax); }
+    __device__ bool header(uint64_t u) const { return b ? b[u].hdr_bits != 0 : true; }
+    __device__ uint32_t type(uint64_t u) const { return b ? b[u].type : rule_type; }
+    __device__ uint64_t nsyms(uint64_t u) const { return b && b[u].type ? b[u].sym_count : 0; }
+    __device__ uint64_t sym_pos(uint64_t u, uint64_t i) const { return syms[b[u].sym_begin + i].pos; } // member-relative
+    __device__ uint64_t bit(uint64_t u) const { return b ? b[u].bit_base : 8 * (byte0 + u * (kStoredMax + 5ull)); }
+};
+struct WriterMembers {
+    const JobBufs &jb;
+    const BgzfJob &bj;
+    const IdxWriteJob &w;
+    __device__ bool eof(uint64_t m) const { return w.bgzf && m + 1 == w.nm; }
+    __device__ uint64_t start(uint64_t m) const { return !w.bgzf ? 0 : eof(m) ? w.n : m * kBgzfBlock; }
+    __device__ uint64_t end(uint64_t m) const { return !w.bgzf ? w.n : eof(m) ? w.n : m * kBgzfBlock + bj.mlen[m]; }
+    __device__ WriterUnits units(uint64_t m) const
+    {
+        if (!w.bgzf) {
+            if (w.stored) return WriterUnits{nullptr, nullptr, 0, w.n, jb.hdr_len, 0, (uint32_t)stored_blocks(w.n)};
+            return WriterUnits{jb.blocks, jb.syms, 0, w.n, 0, 0, jb.info->n_blocks};
+        }
+        if (eof(m)) return WriterUnits{nullptr, nullptr, 0, 0, bj.ctl->out_bytes - kBgzfEofLen + kBgzfHeader, 1, 1};
+        const uint32_t len = bj.mlen[m];
+        if (bj.mstored[m]) return WriterUnits{nullptr, nullptr, 0, len, bj.mout[m] + kBgzfHeader, 0, (uint32_t)stored_blocks(len)};
+        return WriterUnits{jb.blocks + m * kBgzfMaxBlocks, jb.syms, bj.moff[m], len, 0, 0, bj.minfo[m].n_blocks};
+    }
+    __device__ uint64_t n_units(uint64_t m) const { return units(m).nb; }
+    __device__ IdxPick pick(uint64_t m, uint64_t T) const
+    {
+        const WriterUnits U = units(m);
+        return zbi_pick(U, U.nb, T);
+    }
+};
+
+// One warp per slot: the targets k * span, then every member's first header (which also writes the member's entry).  The pick is
+// two binary searches (units, then the unit's symbols by position); a symbol's bit is its unit's first symbol bit plus the code
+// lengths of the symbols in front of it, summed by the lanes with the block's codes, as encode_body writes them.
+__global__ void __launch_bounds__(256) k_deflate_points(JobBufs jb, BgzfJob bj, IdxWriteJob w)
+{
+    const uint64_t slot = (blockIdx.x * 256ull + threadIdx.x) >> 5;
+    const uint32_t lane = threadIdx.x & 31;
+    if (slot >= w.K + w.nm) return; // whole warps
+    const WriterMembers M{jb, bj, w};
+    uint64_t m;
+    IdxPick pk;
+    if (slot < w.K) pk = zbi_pick_members(M, w.nm, (slot + 1) * w.span, &m);
+    else {
+        m = slot - w.K;
+        pk = M.pick(m, 0);
+        if (lane == 0) {
+            IdxMember &e = w.members[m];
+            if (!w.bgzf) e = IdxMember{0, jb.info->out_bytes, 0, w.n};
+            else if (M.eof(m)) e = IdxMember{bj.ctl->out_bytes - kBgzfEofLen, bj.ctl->out_bytes, w.n, w.n};
+            else e = IdxMember{bj.mout[m], bj.mout[m] + bj.mbytes[m], M.start(m), M.end(m)};
+        }
+    }
+    IdxCand c{0, 0, 0, 0, 0, 0, 0};
+    if (m < w.nm) {
+        const WriterUnits U = M.units(m);
+        const uint64_t u = pk.unit;
+        c.member = (uint32_t)m;
+        c.btype = U.type(u);
+        c.found = 1;
+        if (pk.sym == kIdxHeader) {
+            c.out_off = M.start(m) + U.start(u);
+            c.bit = c.hdr_bit = U.bit(u);
+        } else {
+            const BlockDesc &bd = U.b[u];
+            uint32_t bits = 0;
+            for (uint64_t i = lane; i < pk.sym; i += 32) {
+                const Sym s = jb.syms[bd.sym_begin + i];
+                if (s.dist == 0) bits += bd.llen[s.lc];
+                else {
+                    const uint32_t lcode = c_tab.length_code[s.lc], dcode = d_code(c_tab, s.dist - 1u);
+                    bits += bd.llen[lcode + 257] + extra_lbits(lcode) + bd.dlen[dcode] + extra_dbits(dcode);
+                }
+            }
+            bits = __reduce_add_sync(0xffffffffu, bits);
+            c.out_off = M.start(m) + U.sym_pos(u, pk.sym);
+            c.bit = bd.bit_base + bd.hdr_bits + bits;
+            c.hdr_bit = U.header(u) ? bd.bit_base : U.bit(0); // deflate_quick writes one block: its header is in the first piece
+        }
+    }
+    if (lane == 0) w.cand[slot] = c;
+}
+
 } // namespace zb

@@ -7,6 +7,7 @@
 #include "zb_huff.h"
 #include "zb_slow.h"
 #include "zb_bgzf.h"
+#include "zb_index.h"
 
 namespace zb {
 
@@ -141,6 +142,23 @@ struct BgzfJob {
     uint32_t pstart;    // parse start of every member: the dictionary's bytes D' staged in front of each item (0: none)
     uint32_t fdict;     // zlib items get FDICT and DICTID = *dictid (a batch with a preset dictionary)
     const uint32_t *dictid;
+};
+
+// zb_deflate_index (DESIGN.md §2l): k_deflate_points runs one warp per slot, the targets k * span (k = 1..K) and then the first
+// header of every member, over the writer's own block tables.  A slot's candidate has found = 0 when its target has no point.
+struct IdxCand {
+    uint64_t out_off, bit, hdr_bit;
+    uint32_t member, btype, found, pad;
+};
+struct IdxWriteJob {
+    uint64_t span, K;     // targets k * span, k in [1, K]
+    uint64_t n;           // input bytes: the stream's output
+    uint32_t nm;          // members: 1 for one stream; for BGZF the data members and the end-of-file member
+    uint32_t bgzf;        // 1: the members of BgzfJob (after k_bgzf_scan); 0: one stream (after k_scan_blocks, or k_stored)
+    uint32_t stored;      // one stream written by k_stored (level 0): no block table, the headers follow stored_blocks()
+    uint32_t pad;
+    IdxCand *cand;        // K + nm slots
+    IdxMember *members;   // nm entries, written by the members' slots
 };
 
 cudaError_t upload_tables();
