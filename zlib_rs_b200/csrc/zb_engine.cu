@@ -1059,6 +1059,14 @@ int Engine::index_written(const JobBufs &jb, const BgzfJob &bj, const IdxWriteJo
 int Engine::checksum(bool crc, uint32_t start, const void *buf, size_t len, bool on_dev, uint32_t *out, float *ms_out)
 {
     if (!out) return ZB_E_PARAM;
+    if (len == 0) {
+        // the value of zero bytes is the start value, unreduced, as the reference returns it (an adler32 start whose halves are
+        // >= 65521 would come back reduced from k_adler_final)
+        *out = start;
+        launches = 0;
+        if (ms_out) *ms_out = 0.f;
+        return ZB_OK;
+    }
     CK(cudaSetDevice(device));
     int rc;
     void *p;
