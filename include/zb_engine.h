@@ -139,6 +139,31 @@ ZB_API int zb_deflate_batch_dict(zb_engine *e, const void *dict, size_t dict_len
                                  size_t n_items, int src_on_device, void *dst, size_t dst_cap, int dst_on_device, int level, int strategy,
                                  int window_bits, uint32_t flags, uint64_t *dst_off, uint32_t *checks, zb_deflate_result *res);
 
+/* zb_deflate_flushed: one stream with a full flush at every segment boundary (DESIGN.md §2m).  The input src[seg_off[0],
+ * seg_off[n_segs]) is cut into segments [seg_off[k], seg_off[k+1]) (seg_off: a host array of n_segs + 1 offsets; src a host or, with
+ * src_on_device, a device pointer).  dst receives byte for byte what the reference writes for
+ *     deflateInit2(level, Z_DEFLATED, window_bits, 8, Z_DEFAULT_STRATEGY)
+ *     deflate(segment k, Z_FULL_FLUSH)   for k < n_segs - 1
+ *     deflate(last segment, Z_FINISH)
+ * each call given its whole segment and enough output space: the seekable zlib / gzip / raw stream of dictzip-style writers.  After a
+ * full flush the reference forgets the history, so each segment decodes alone from its first byte.  restart (host, n_segs + 1
+ * entries) is filled: restart[k] is the offset in dst where segment k's deflate data begins (restart[0] = the header's length, 0, 2
+ * or 10), restart[n_segs] where the trailer begins; every segment but the last ends with 00 00 ff ff just before restart[k + 1].
+ * res: out_bytes, check (adler32 / crc32 of the whole input, 0 raw), data_type (as z_stream holds it after the last call),
+ * n_blocks (the empty stored blocks of the flushes included) and n_symbols, gpu_launches, gpu_ms, exact_parity = 1, bits_used = 8.
+ * Accepted: window_bits 15, -15 or 31 (one header, zb_deflate's, and one trailer); Z_DEFAULT_STRATEGY; level -1..9; flags 0 or
+ * ZB_FLAG_MEMLEVEL(8); every segment 1..65536 bytes, at most 65535 segments, at most 2^31 bytes in all.  Anything else gives
+ * ZB_E_PARAM with a zb_last_error() text.  n_segs = 0 gives exactly zb_deflate_ex's empty stream (restart[0] = the header's
+ * length).  dst_cap below the length gives ZB_E_BUF with res->out_bytes set to the length needed; zb_deflate_flushed_bound is
+ * always enough.  The segments are compressed side by side through the member kernels of zb_deflate_batch, each parsed as the
+ * batch item of its bytes (what the reference's window holds behind a segment never reaches its output, DESIGN.md §2m); a call
+ * costs a fixed number of launches and two host syncs whatever n_segs. */
+ZB_API int zb_deflate_flushed(zb_engine *e, const void *src, const uint64_t *seg_off, size_t n_segs, int src_on_device, void *dst,
+                              size_t dst_cap, int dst_on_device, int level, int strategy, int window_bits, uint32_t flags, uint64_t *restart,
+                              zb_deflate_result *res);
+/* the sum of zb_deflate_bound over the segments plus 18 bytes of framing; zb_deflate_bound(0) for an empty input */
+ZB_API size_t zb_deflate_flushed_bound(const uint64_t *seg_off, size_t n_segs);
+
 typedef struct zb_inflate_result {
     uint64_t out_bytes;
     uint64_t in_bytes;   /* compressed bytes consumed */
@@ -192,6 +217,23 @@ ZB_API int zb_inflate_batch(zb_engine *e, const void *src, const uint64_t *src_o
 ZB_API int zb_inflate_batch_dict(zb_engine *e, const void *dict, size_t dict_len, const void *src, const uint64_t *src_off,
                                  size_t n_items, int src_on_device, void *dst, const uint64_t *dst_off, int dst_on_device, int window_bits,
                                  zb_inflate_result *items);
+
+/* zb_inflate_flushed: decode any set of segments of a stream written with full flushes, each from its restart point with an empty
+ * window (DESIGN.md §2m).  Segment k is src[restart[k], restart[k+1]) (restart: host, n_segs + 1 entries, as zb_deflate_flushed
+ * fills it, or the cumulative output lengths after each Z_FULL_FLUSH of any zlib writer).  Item i decodes segment which[i] as raw
+ * deflate into its slot dst[dst_off[i], dst_off[i+1]) (which: n_which entries; dst_off: n_which + 1; host arrays).  items[i]:
+ *   ZB_OK     its blocks end exactly at restart[k+1]: with the empty non-final stored block (00 00 ff ff) for k < n_segs - 1, with
+ *             the BFINAL block for the last segment (the trailer is not read);
+ *   ZB_E_DATA the decoder's message for damage, or "segment does not end at its restart point";
+ *   ZB_E_BUF  the slot is too small.
+ * check is the adler32 (window_bits 15) or crc32 (31) of the segment's output, 0 for -15; in_bytes the segment's length.  One bad
+ * item never changes another's result; a host dst is written whole (zeros behind each output).  Returns ZB_OK when every item is
+ * OK, else the status of the first item that failed.  window_bits other than 15, -15 and 31, which[i] >= n_segs, restart points that
+ * decrease, restart[n_segs] > src_len, slots of 4 GiB or more or more than 2^20 items give ZB_E_PARAM.  One warp per item, four
+ * launches and one host sync; a host source is uploaded from restart[0] to restart[n_segs] in one copy. */
+ZB_API int zb_inflate_flushed(zb_engine *e, const void *src, size_t src_len, int src_on_device, const uint64_t *restart, size_t n_segs,
+                              const uint32_t *which, size_t n_which, void *dst, const uint64_t *dst_off, int dst_on_device, int window_bits,
+                              zb_inflate_result *items);
 
 /* Streaming building block (what inflate() of the zlib ABI runs on, zlib-rs/src/inflate.rs:2376-2457): decode the COMPLETE deflate
  * blocks of a raw deflate segment.  src/dict/dst are host buffers; decoding starts at bit `start_bit` of src with the last

@@ -161,6 +161,12 @@ def lib():
         if hasattr(L, "zb_deflate_index"):
             L.zb_deflate_index.argtypes = [vp, vp, sz, ci, vp, sz, ci, ci, ci, ci, u32, u64, ctypes.POINTER(DeflateResult),
                                            ctypes.POINTER(vp)]
+        if hasattr(L, "zb_deflate_flushed"):
+            u64p = ctypes.POINTER(u64)
+            L.zb_deflate_flushed.argtypes = [vp, vp, u64p, sz, ci, vp, sz, ci, ci, ci, ci, u32, u64p, ctypes.POINTER(DeflateResult)]
+            L.zb_deflate_flushed_bound.argtypes, L.zb_deflate_flushed_bound.restype = [u64p, sz], sz
+            L.zb_inflate_flushed.argtypes = [vp, vp, sz, ci, u64p, sz, ctypes.POINTER(u32), sz, vp, u64p, ci, ci,
+                                             ctypes.POINTER(InflateResult)]
         if hasattr(L, "zb_deflate_batch_dict"):
             L.zb_deflate_batch_dict.argtypes = [vp, vp, sz] + L.zb_deflate_batch.argtypes[1:]
             L.zb_inflate_batch_dict.argtypes = [vp, vp, sz] + L.zb_inflate_batch.argtypes[1:]
@@ -236,6 +242,17 @@ def deflate_batch_bound(lengths):
     """Largest output Engine.deflate_batch writes for items of these lengths: the sum of their zb_deflate_bound."""
     off = _offsets(list(lengths))
     return lib().zb_deflate_batch_bound(off, len(off) - 1)
+
+
+def flushed_offsets(n, seg_len):
+    """Segment offsets (n_segs + 1) of an input of n bytes cut every seg_len bytes; the last segment may be shorter."""
+    return list(range(0, n, seg_len)) + [n] if n else [0]
+
+
+def deflate_flushed_bound(seg_off):
+    """Largest stream Engine.deflate_flushed writes for these segment offsets (zb_deflate_flushed_bound)."""
+    off = (ctypes.c_uint64 * len(seg_off))(*seg_off)
+    return lib().zb_deflate_flushed_bound(off, len(seg_off) - 1)
 
 
 def compressBound(n):
@@ -632,6 +649,110 @@ class Engine:
             raw = own.raw
             outs = [raw[doff[i]:doff[i] + results[i].out_bytes] for i in range(n)]
         return rc, outs, results
+
+    def deflate_flushed(self, src, seg_len=None, seg_off=None, level=-1, window_bits=15, mem_level=8, src_on_device=False, n=None,
+                        strategy=0, flags=0, dst=None, dst_cap=0, dst_on_device=False):
+        """Deflate `src` as one stream with a full flush behind every segment but the last (zb_deflate_flushed): byte for byte
+        deflate(segment, Z_FULL_FLUSH) per segment and Z_FINISH on the last.  Cut the input every `seg_len` bytes, or at `seg_off`
+        (n_segs + 1 offsets into src).  Host `src` is bytes-like; a device `src` is a pointer with `n` (or seg_off).  Returns
+        (bytes or None, DeflateResult, restarts): restarts[k] is where segment k's deflate data begins in the stream and
+        restarts[-1] where the trailer begins.  With a caller's `dst` the first element is None.  Raises ZlibError (.needed: the
+        size a too small dst_cap would have to be)."""
+        keep = None
+        if not src_on_device:
+            data, keep = _buf(src)
+            n = len(data)
+            src = ctypes.addressof(keep)
+        if seg_off is None:
+            if seg_len is None or seg_len <= 0:
+                raise ValueError("deflate_flushed needs seg_len > 0 or seg_off")
+            if n is None:
+                raise ValueError("deflate_flushed with a device source and seg_len needs n")
+            seg_off = flushed_offsets(n, seg_len)
+        elif not src_on_device and seg_off[-1] > n:
+            raise ValueError("segment offsets reach %d bytes, the source has %d" % (seg_off[-1], n))
+        off = (ctypes.c_uint64 * len(seg_off))(*seg_off)
+        n_segs = len(seg_off) - 1
+        own = None
+        if dst is None:
+            dst_cap = lib().zb_deflate_flushed_bound(off, n_segs) + 64
+            own = ctypes.create_string_buffer(dst_cap)
+            dst = ctypes.addressof(own)
+            dst_on_device = False
+        restart = (ctypes.c_uint64 * (n_segs + 1))()
+        res = DeflateResult()
+        rc = lib().zb_deflate_flushed(self.h, src, off, n_segs, int(src_on_device), dst, dst_cap, int(dst_on_device), level, strategy,
+                                      window_bits, flags | ((mem_level & 15) << 8), restart, ctypes.byref(res))
+        if rc != 0:
+            e = ZlibError(rc, lib().zb_last_error().decode())
+            e.needed = res.out_bytes
+            raise e
+        return (own.raw[: res.out_bytes] if own is not None else None), res, list(restart)
+
+    def inflate_flushed(self, src, restarts, which, out_caps=None, window_bits=15, src_on_device=False, n=None, dst=None, dst_off=None,
+                        dst_on_device=False):
+        """Decode segments `which` of a stream written with full flushes, each from its restart point (zb_inflate_flushed).
+        `restarts`: n_segs + 1 offsets, as Engine.deflate_flushed returns them.  Item i decodes segment which[i] into a slot of
+        out_caps[i] bytes; a caller's `dst` takes `dst_off` (len(which) + 1 offsets) instead.  Host `src` is bytes or a writable
+        buffer (not copied by Python); a device `src` is a pointer with `n`.  Returns (outputs or None, list of InflateResult): every item carries its own status;
+        a call that fails as a whole (refused arguments, a device error) raises ZlibError."""
+        if src_on_device:
+            addr, keep = src, None
+        else:
+            addr, n, keep = _host_view(src)
+        rs = (ctypes.c_uint64 * len(restarts))(*restarts)
+        w = (ctypes.c_uint32 * max(len(which), 1))(*which)
+        k = len(which)
+        own = None
+        if dst is None:
+            doff = _offsets(list(out_caps))
+            own = ctypes.create_string_buffer(max(doff[k], 1))
+            dst = ctypes.addressof(own)
+            dst_on_device = False
+        else:
+            doff = (ctypes.c_uint64 * len(dst_off))(*dst_off)
+        res = (InflateResult * max(k, 1))()
+        rc = lib().zb_inflate_flushed(self.h, addr, n, int(src_on_device), rs, len(restarts) - 1, w, k, dst, doff, int(dst_on_device),
+                                      window_bits, res)
+        results = list(res)[:k]
+        if rc != 0 and not any(r.status == rc for r in results):  # a refusal or a failed call, not an item's status
+            raise ZlibError(rc, lib().zb_last_error().decode())
+        outs = None
+        if own is not None:
+            raw = own.raw
+            outs = [raw[doff[i]:doff[i] + results[i].out_bytes] for i in range(k)]
+        return outs, results
+
+    def read_flushed(self, src, restarts, seg_off, ranges, window_bits=15):
+        """Read byte ranges [(offset, length), ...] of the input of a flushed stream: every segment a range touches is decoded
+        once, all in one inflate_flushed call, and the ranges are sliced out of them.  `seg_off`: the segment offsets the stream
+        was written with.  Returns a list of bytes; raises ZlibError when a needed segment does not decode."""
+        import bisect
+        total = seg_off[-1]
+        need = set()
+        for o, ln in ranges:
+            if o < 0 or ln < 0 or o + ln > total:
+                raise ValueError("range (%d, %d) outside the %d input bytes" % (o, ln, total))
+            if ln:
+                a = bisect.bisect_right(seg_off, o) - 1
+                b = bisect.bisect_right(seg_off, o + ln - 1) - 1
+                need.update(range(a, b + 1))
+        which = sorted(need)
+        outs, items = self.inflate_flushed(src, restarts, which, [seg_off[k + 1] - seg_off[k] for k in which], window_bits=window_bits)
+        for k, r in zip(which, items):
+            if r.status != 0:
+                raise ZlibError(r.status, "segment %d: %s" % (k, r.msg.decode()))
+        seg = dict(zip(which, outs))
+        res = []
+        for o, ln in ranges:
+            parts, p = [], o
+            while p < o + ln:
+                k = bisect.bisect_right(seg_off, p) - 1
+                e = min(o + ln, seg_off[k + 1])
+                parts.append(seg[k][p - seg_off[k]:e - seg_off[k]])
+                p = e
+            res.append(b"".join(parts))
+        return res
 
     def build_index(self, src, out_cap, span=1 << 20, window_bits=15, flags=0, n=None, src_on_device=False, dst=None,
                     dst_on_device=False):

@@ -1,8 +1,8 @@
-// zb_bgzf.cu -- member writing (zb_bgzf.h): BGZF files (ZB_FLAG_BGZF, DESIGN.md §2h) and batches of streams (zb_deflate_batch,
-// DESIGN.md §2i).  The batch staging, the member parsers of levels 3..9, the member sizes and offsets, and the framing.  Every kernel
-// covers all members of the call, so a call costs the same launches whatever its length.  Levels 1/2 parse in k_serial_low_members
-// (zb_serial.cu); the block kernels k_bgzf_hist / k_bgzf_build / k_bgzf_encode share their bodies with the single-stream ones
-// (zb_kernels.cu).
+// zb_bgzf.cu -- member writing (zb_bgzf.h): BGZF files (ZB_FLAG_BGZF, DESIGN.md §2h), batches of streams (zb_deflate_batch,
+// DESIGN.md §2i) and flushed streams (zb_deflate_flushed, DESIGN.md §2m).  The batch staging, the member parsers of levels 3..9,
+// the member sizes and offsets, and the framing.  Every kernel covers all members of the call, so a call costs the same launches
+// whatever its length.  Levels 1/2 parse in k_serial_low_members (zb_serial.cu); the block kernels k_bgzf_hist / k_bgzf_build /
+// k_bgzf_encode share their bodies with the single-stream ones (zb_kernels.cu).
 #include "zb_kernels.cuh"
 
 namespace zb {
@@ -133,6 +133,7 @@ __global__ void __launch_bounds__(256) k_bgzf_size(JobBufs jb, BgzfJob bj)
     const uint32_t m = blockIdx.x * 256 + threadIdx.x;
     if (m >= bj.nm) return;
     const uint32_t len = bj.mlen[m];
+    const bool fin = !bj.flushed || m + 1 == bj.nm; // the member ends its stream: BFINAL, no empty stored block behind it
     bool stored = jb.level == 0;
     uint64_t payload = 0;
     uint32_t nb = 0;
@@ -145,14 +146,15 @@ __global__ void __launch_bounds__(256) k_bgzf_size(JobBufs jb, BgzfJob bj)
             bd.bit_base = bit;
             bit = bd.type == 0 ? ((bit + 3 + 7) & ~7ull) + 32 + 8ull * (uint16_t)bd.in_len : bit + bd.hdr_bits + bd.body_bits;
         }
-        payload = (bit + 7) >> 3;
+        payload = flush_payload(bit, fin);
         atomicAdd(&bj.ctl->n_syms, bj.minfo[m].n_syms);
         if (bj.wrap == kWrapBgzf && bgzf_stored(payload)) stored = true;
     }
-    if (stored) { payload = stored_payload(len); nb = (uint32_t)stored_blocks(len); } // one block for a BGZF member
+    if (stored) { payload = stored_payload(len) + (fin ? 0 : 5); nb = (uint32_t)stored_blocks(len); } // one block for a BGZF member
     atomicAdd(&bj.ctl->n_blocks, nb);
     bj.mstored[m] = stored;
-    bj.mbytes[m] = member_header_len(bj.wrap, bj.fdict) + (uint32_t)payload + member_trailer_len(bj.wrap);
+    bj.mbytes[m] = bj.flushed ? flush_header_len(bj.wrap, m) + (uint32_t)payload + flush_trailer_len(bj.wrap, m, bj.nm)
+                              : member_header_len(bj.wrap, bj.fdict) + (uint32_t)payload + member_trailer_len(bj.wrap);
 }
 
 // One CTA: the members' offsets in the output (exclusive scan of their lengths), the blocks' absolute bit positions, the output
@@ -174,9 +176,9 @@ __global__ void __launch_bounds__(1024) k_bgzf_scan(JobBufs jb, BgzfJob bj)
         __syncthreads();
     }
     uint64_t off = part[tid] - s;
-    const uint32_t hl = member_header_len(bj.wrap, bj.fdict);
     for (uint32_t i = beg; i < end; i++) {
         bj.mout[i] = off;
+        const uint32_t hl = bj.flushed ? flush_header_len(bj.wrap, i) : member_header_len(bj.wrap, bj.fdict);
         if (!bj.mstored[i]) {
             const uint32_t nb = bj.minfo[i].n_blocks;
             for (uint32_t k = 0; k < nb; k++) jb.blocks[i * kBgzfMaxBlocks + k].bit_base += 8ull * (off + hl);
@@ -199,8 +201,25 @@ __global__ void __launch_bounds__(256) k_bgzf_frame(JobBufs jb, BgzfJob bj)
         return;
     }
     uint8_t *o = jb.out + bj.mout[m];
-    const uint32_t len = bj.mlen[m], bytes = bj.mbytes[m], hl = member_header_len(bj.wrap, bj.fdict);
+    const uint32_t len = bj.mlen[m], bytes = bj.mbytes[m];
     const bool stored = bj.mstored[m] != 0;
+    if (bj.flushed) { // one stream: its header, its trailer (the whole input's check), the empty stored block behind every other member
+        const bool fin = m + 1 == bj.nm;
+        const uint32_t hl = flush_header_len(bj.wrap, m);
+        if (tid == 0) {
+            if (m == 0) stream_header(o, bj.wrap, zlib_level_flags(jb.level, false), 7, gzip_xfl((int)jb.level, 0));
+            if (fin) stream_trailer(o + bytes - stream_trailer_len(bj.wrap), bj.wrap, *bj.fcheck, bj.isize);
+            else { o[bytes - 2] = 0xff; o[bytes - 1] = 0xff; } // 00 00 ff ff: the zeroed output holds the rest
+        }
+        if (stored) {
+            const uint32_t nb = (uint32_t)stored_blocks(len);
+            if (tid < nb) stored_header(o + hl + tid * (kStoredMax + 5), min(kStoredMax, len - tid * kStoredMax), fin && tid + 1 == nb);
+            const uint8_t *src = jb.in + bj.moff[m];
+            for (uint32_t i = tid; i < len; i += 256) o[hl + 5 * (i / kStoredMax + 1) + i] = src[i];
+        }
+        return;
+    }
+    const uint32_t hl = member_header_len(bj.wrap, bj.fdict);
     if (tid == 0) {
         if (bj.wrap == kWrapBgzf) bgzf_header(o, bytes);
         else stream_header(o, bj.wrap, zlib_level_flags(jb.level, false), 7, gzip_xfl((int)jb.level, 0), bj.fdict != 0,
@@ -214,6 +233,22 @@ __global__ void __launch_bounds__(256) k_bgzf_frame(JobBufs jb, BgzfJob bj)
         const uint8_t *src = jb.in + bj.moff[m] + bj.pstart; // the item's bytes only
         for (uint32_t i = tid; i < len; i += 256) o[hl + 5 * (i / kStoredMax + 1) + i] = src[i];
     }
+}
+
+// Flushed streams (zb_bgzf.h), after the parse: a segment that does not end the stream flushes no empty block when its symbols filled its last block
+// (levels 2..9; deflate_quick's block always ends at the flush).  That block was flushed by the parser's loop, so it keeps the
+// window base of a block the loop flushed.  One thread per member.
+__global__ void __launch_bounds__(256) k_flush_blocks(JobBufs jb, BgzfJob bj)
+{
+    const uint32_t m = blockIdx.x * 256 + threadIdx.x;
+    if (m + 1 >= bj.nm) return;
+    JobInfo &mi = bj.minfo[m];
+    const uint32_t n = mi.n_syms, bs = jb.block_syms;
+    if (n == 0 || n % bs || mi.n_blocks != n / bs + 1) return;
+    mi.n_blocks = n / bs;
+    const uint32_t base = (uint32_t)bj.moff[m];
+    mi.final_base = jb.slow_mode ? base_at(jb.syms[base + n - 1].pos + 1, bj.mlen[m], jb.wsize) // as k_bgzf_hist
+                                 : jb.block_base[m * kBgzfMaxBlocks + n / bs - 1];
 }
 
 } // namespace zb

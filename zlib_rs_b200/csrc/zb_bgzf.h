@@ -1,5 +1,7 @@
-// zb_bgzf.h -- the rules of member writing: BGZF files (ZB_FLAG_BGZF in zb_engine.h, DESIGN.md §2h) and batches of independent
-// streams (zb_deflate_batch, DESIGN.md §2i).  Both compress many members side by side through the same kernels (zb_bgzf.cu).
+// zb_bgzf.h -- the rules of member writing: BGZF files (ZB_FLAG_BGZF in zb_engine.h, DESIGN.md §2h), batches of independent
+// streams (zb_deflate_batch, DESIGN.md §2i) and streams with a full flush at every segment boundary (zb_deflate_flushed, DESIGN.md
+// §2m, at the end of this file).  All compress many members side by side through the same kernels (zb_bgzf.cu); tests/flushmodel
+// compiles the flushed rules.
 //
 // Like zb_members.h this is `__host__ __device__`: the kernels of zb_bgzf.cu follow these rules, and tests/bgzfmodel and
 // tests/batchmodel compile the same source, so the CPU tests check the member-relative parse against the oracle and the framing
@@ -135,5 +137,54 @@ struct BgzfAcc {
     }
     ZB_HD bool inserted(uint32_t) const { return true; }
 };
+
+// ---------------------------------------------------------------------------------------------------------------------------------
+// Flushed streams (zb_deflate_flushed, DESIGN.md §2m): the input cut into segments, written as deflateInit2(level, 8, -15 / 15 /
+// 31) + deflate(segment k, Z_FULL_FLUSH) for every segment but the last + deflate(last, Z_FINISH), each call with its whole segment.
+//
+// A full flush that consumed all its input clears head[] and sets strstart = block_start = insert = 0 (deflate.rs:2739-2751), so
+// segment k is parsed as a fresh stream of its own length N_k: its own window schedule, chains and block cuts.  Member k of the
+// member core is segment k, staged and parsed as a batch item; only its framing differs (below the bytes behind it are shown not
+// to matter).
+//
+// Framing.  One header in front of member 0; every member but the last closes its last block with BFINAL = 0, and the flush writes
+// the empty stored block behind it (3 zero bits, alignment, 00 00 ff ff); the last member ends with BFINAL = 1 and the trailer.  A
+// segment flushes no empty block when its symbols fill its last block exactly (the parsers' loops flushed it; `if sym_next != 0`,
+// deflate_{fast,medium,slow}), except deflate_quick, whose one static block always ends at the flush.  Level 0: deflate_stored
+// cuts the segment into stored blocks of at most 65535 bytes by the direct-copy path (stored_blocks), BFINAL = 0 on all of them,
+// and returns BlockDone, so the marker follows; under Z_FINISH its last block has BFINAL = 1.  Byte for byte: the segments are
+// byte aligned and concatenated, so restart[k] (the first byte of segment k) is a raw restart point.
+//
+// The bytes behind a segment.  The window buffer (2 w_size bytes) is never cleared, so behind segment k's N_k bytes it holds what
+// earlier segments left there (their bytes, moved down by a slide of a segment of 65274 bytes or more), where a one-shot input of
+// N_k bytes has zeros.  No parser of levels 1..9 lets those bytes reach a symbol, a block or the state a flush carries over, so
+// segment k is staged and parsed exactly as a batch item of its bytes, zeros behind it (tests/flushmodel checks both halves:
+// the oracle's window after each flush is not zeros, and its symbols are this parse's).  Every read behind the input is one of:
+//   - a hash of a string reaching past the end: lookups need lookahead >= 4 (every parser), and the positions whose inserted
+//     hashes reach past the end (inside a match that ends there) come after every later lookup of the segment; the next segment
+//     starts with head[] cleared, and prev[] is reached only through head[];
+//   - a match comparison (compare256, the 8-byte prefilter, scan_end): both sides compare input bytes until the candidate has
+//     matched all `lookahead` bytes left, and from then on its length is at least the lookahead.  If that beats best_len,
+//     longest_match returns (lookahead, this candidate) at once, whatever follows; deflate_quick clamps its one candidate to the
+//     lookahead.  best_len >= lookahead happens only in deflate_slow with prev_length >= lookahead, and there every outcome of
+//     the walk (a candidate returning lookahead, best_len, or LM_BREAK_MATCHING's min(best_len, lookahead)) is at most prev_length,
+//     so the previous match is emitted and the result dropped;
+//   - level 9's head[] probes of the strings at scan + 1 .. scan + best_len - 2: past the end only when best_len = prev_length >=
+//     lookahead, the same dropped result.
+// The match_start such a dropped walk leaves is read again only with prev_length >= 3, after a walk that set it; a segment ends
+// with prev_length <= 2, and level 9's rolling hash is recomputed from the segment's first two bytes in its first fill_window.
+// Level 0 reads no window byte at all (deflate_stored reads back only its own pending input, and a full flush leaves none).
+
+// Member m of nm in a flushed stream: header only on the first, trailer only on the last, the marker behind every other.
+ZB_HD uint32_t flush_header_len(uint32_t wrap, uint32_t m) { return m == 0 ? stream_header_len(wrap) : 0u; }
+ZB_HD uint32_t flush_trailer_len(uint32_t wrap, uint32_t m, uint32_t nm) { return m + 1 == nm ? stream_trailer_len(wrap) : 0u; }
+// Bytes of a member's payload ending at bit `bits` (from its first byte): the empty stored block behind it unless it is the last.
+ZB_HD uint64_t flush_payload(uint64_t bits, bool last) { return last ? (bits + 7) >> 3 : (((bits + 3 + 7) >> 3) + 4); }
+
+// zb_deflate_flushed_bound.  Segment k of N_k bytes costs at most what zb_deflate_bound (stream_bound) allows a one-shot stream of
+// N_k bytes, header and trailer included: its blocks are those of that stream (at most stored + the quick overhead), with at most
+// 3 + 7 bits of the empty block's header and alignment and its 4 bytes instead of a trailer.  stream_bound has 18 + 64 bytes of
+// slack beyond framing, so the marker fits in it.  The sum over the segments, plus one header and trailer (18 bytes), bounds the
+// stream; an empty input gets stream_bound(0), the one-shot empty stream.
 
 } // namespace zb

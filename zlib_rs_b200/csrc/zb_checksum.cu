@@ -461,6 +461,47 @@ __global__ void __launch_bounds__(256) k_adler_segments(const uint8_t *__restric
     }
 }
 
+// k_adler_join: adler32_combine of the first *count segment checks, in order (the counterpart of k_crc_join).  Each thread folds a
+// run of segments into (adler, length); a tree joins the runs.  The empty run (1, 0) is the identity.
+__device__ __forceinline__ uint32_t adler_combine(uint32_t a1, uint32_t a2, uint64_t len2) // adler32.rs combine
+{
+    const uint32_t rem = (uint32_t)(len2 % kAdlerBase);
+    uint32_t s1 = a1 & 0xffffu;
+    uint32_t s2 = (uint32_t)(((uint64_t)rem * s1) % kAdlerBase);
+    s1 += (a2 & 0xffffu) + kAdlerBase - 1;
+    s2 += (a1 >> 16) + (a2 >> 16) + kAdlerBase - rem;
+    if (s1 >= kAdlerBase) s1 -= kAdlerBase;
+    if (s1 >= kAdlerBase) s1 -= kAdlerBase;
+    if (s2 >= 2 * kAdlerBase) s2 -= 2 * kAdlerBase;
+    if (s2 >= kAdlerBase) s2 -= kAdlerBase;
+    return s1 | (s2 << 16);
+}
+__global__ void __launch_bounds__(1024) k_adler_join(const uint32_t *__restrict__ adler, const uint32_t *__restrict__ len,
+                                                     const uint32_t *__restrict__ count, uint32_t *__restrict__ out)
+{
+    __shared__ uint32_t sa[1024];
+    __shared__ uint64_t sl[1024];
+    const uint32_t tid = threadIdx.x, n = *count, per = (n + 1023) / 1024;
+    const uint32_t beg = min(n, tid * per), end = min(n, beg + per);
+    uint32_t a = 1;
+    uint64_t l = 0;
+    for (uint32_t i = beg; i < end; i++) { a = adler_combine(a, adler[i], len[i]); l += len[i]; }
+    sa[tid] = a;
+    sl[tid] = l;
+    __syncthreads();
+    for (uint32_t h = 1; h < 1024; h <<= 1) {
+        if ((tid & (2 * h - 1)) == 0) { sa[tid] = adler_combine(sa[tid], sa[tid + h], sl[tid + h]); sl[tid] += sl[tid + h]; }
+        __syncthreads();
+    }
+    if (tid == 0) *out = sa[0];
+}
+
+cudaError_t launch_adler32_join(const uint32_t *d_adler, const uint32_t *d_len, const uint32_t *d_count, uint32_t *d_out, cudaStream_t st)
+{
+    k_adler_join<<<1, 1024, 0, st>>>(d_adler, d_len, d_count, d_out);
+    return cudaGetLastError();
+}
+
 cudaError_t launch_adler32_segments(const uint8_t *d_buf, const uint64_t *d_off, const uint32_t *d_len, uint32_t nseg, uint32_t *d_adler,
                                     cudaStream_t st)
 {

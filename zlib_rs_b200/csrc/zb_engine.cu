@@ -74,6 +74,7 @@ __global__ void k_bgzf_encode(JobBufs, BgzfJob);
 __global__ void k_bgzf_frame(JobBufs, BgzfJob);
 __global__ void k_batch_stage(const uint8_t *, const uint64_t *, const uint8_t *, BgzfJob, uint8_t *, uint64_t);
 __global__ void k_batch_dict_ghost(JobBufs, BgzfJob);
+__global__ void k_flush_blocks(JobBufs, BgzfJob);
 __global__ void k_deflate_points(JobBufs, BgzfJob, IdxWriteJob); // zb_deflate_index (zb_kernels.cu)
 
 constexpr uint32_t kMatchSmemBytes = (kWSize + kMatchSub + 512) + (kWSize + kMatchSub) * 2 + ((kWSize + kMatchSub) / 32 + 1) * 4 * 4 + 8192;
@@ -737,6 +738,9 @@ int Engine::members_reserve(JobBufs &jb, BgzfJob &bj, uint32_t nm, uint32_t S, s
     bj.pstart = 0;
     bj.fdict = 0;
     bj.dictid = nullptr;
+    bj.flushed = 0;
+    bj.fcheck = nullptr;
+    bj.isize = 0;
     bj.moff = reinterpret_cast<uint64_t *>(t);
     bj.mout = reinterpret_cast<uint64_t *>(t + m8);
     bj.mlen = reinterpret_cast<uint32_t *>(t + 2 * m8);
@@ -776,6 +780,7 @@ int Engine::members_launch(JobBufs &jb, BgzfJob &bj, int level, uint32_t *d_freq
             k_bgzf_slow_walk<<<(nm + 31) / 32, 32, 0, st>>>(jb, bj);
             launches += 2;
         }
+        if (bj.flushed && jb.serial_mode != 1) { k_flush_blocks<<<nm / 256 + 1, 256, 0, st>>>(jb, bj); launches++; } // zb_bgzf.cu
         k_bgzf_hist<<<nslots, 256, 0, st>>>(jb, bj, d_freq);
         k_bgzf_build<<<nslots, 32, 0, st>>>(jb, bj, d_freq);
         launches += 2;
@@ -1028,6 +1033,140 @@ int Engine::deflate_batch(const void *dict, size_t dict_len, const void *src, co
     return ZB_OK;
 }
 
+// zb_deflate_flushed (zb_bgzf.h, DESIGN.md §2m): segment k of the input is member k of the member core, staged and parsed like a
+// batch item and framed as one stream with a full flush behind every segment but the last.
+// The whole input's check joins the segments' checks on the device.  A call costs a fixed number of launches and two host syncs
+// whatever the number and lengths of its segments.
+int Engine::deflate_flushed(const void *src, const uint64_t *seg_off, size_t n_segs, bool src_dev, void *dst, size_t dst_cap, bool dst_dev,
+                            int level, int strategy, int window_bits, uint32_t flags, uint64_t *restart, zb_deflate_result *res)
+{
+    if (!res || !restart || (n_segs && (!seg_off || !dst))) { snprintf(g_err, sizeof g_err, "deflate_flushed: null argument"); return ZB_E_PARAM; }
+    memset(res, 0, sizeof *res);
+    const uint32_t ml = (flags >> 8) & 15u;
+    uint32_t wrap;
+    if (window_bits == 15) wrap = 1;
+    else if (window_bits == 31) wrap = 2;
+    else if (window_bits == -15) wrap = 0;
+    else { snprintf(g_err, sizeof g_err, "deflate_flushed takes window_bits 15, -15 or 31"); return ZB_E_PARAM; }
+    if ((flags & ~ZB_FLAG_MEMLEVEL(15)) || (ml && ml != 8) || strategy != 0 || level < -1 || level > 9) {
+        snprintf(g_err, sizeof g_err, "deflate_flushed takes Z_DEFAULT_STRATEGY, level -1..9, memLevel 8 and no flag");
+        return ZB_E_PARAM;
+    }
+    if (n_segs > kBatchMaxItems) {
+        snprintf(g_err, sizeof g_err, "deflate_flushed: %zu segments (at most %llu)", n_segs, (unsigned long long)kBatchMaxItems);
+        return ZB_E_PARAM;
+    }
+    if (n_segs == 0) { // an empty input: the one-shot empty stream (restart[0] is still the header's length)
+        restart[0] = stream_header_len(wrap);
+        return deflate(src, 0, src_dev, dst, dst_cap, dst_dev, level, strategy, window_bits, flags, res);
+    }
+    const uint32_t nm = (uint32_t)n_segs;
+    uint64_t span = 0, bound = 18;
+    for (uint32_t i = 0; i < nm; i++) {
+        if (seg_off[i + 1] <= seg_off[i] || seg_off[i + 1] - seg_off[i] > kMemberMax) {
+            snprintf(g_err, sizeof g_err, "deflate_flushed: segment %u is not 1..%u bytes", i, kMemberMax);
+            return ZB_E_PARAM;
+        }
+        span = batch_stage_next(span, seg_off[i + 1] - seg_off[i]);
+        bound += stream_bound(seg_off[i + 1] - seg_off[i]);
+    }
+    const uint64_t total = seg_off[nm] - seg_off[0];
+    if (total > kBatchMaxBytes) { snprintf(g_err, sizeof g_err, "deflate_flushed: %llu bytes in all (at most 2^31)", (unsigned long long)total); return ZB_E_PARAM; }
+    if (!src) { snprintf(g_err, sizeof g_err, "deflate_flushed: null source"); return ZB_E_PARAM; }
+    if (level == -1) level = 6;
+    CK(cudaSetDevice(device));
+    launches = 0;
+    const uint32_t S = (uint32_t)span; // 2^31 input bytes + at most 127 bytes of gap and alignment per segment: below 2^32
+    const size_t out_cap = (bound + 15) & ~(size_t)15;
+    JobBufs jb;
+    BgzfJob bj;
+    uint32_t *d_freq;
+    int rc;
+    if ((rc = members_reserve(jb, bj, nm, S, span, level, out_cap, wrap, &d_freq)) != ZB_OK) return rc;
+    bj.flushed = 1;
+    bj.isize = (uint32_t)total;
+    // pinned staging: the member table up (moff | mlen | seg_off | count), the control block and offsets down
+    const size_t t_up = (size_t)nm * 8 + (size_t)nm * 8 + ((size_t)nm + 1) * 8 + 16, t_down = sizeof(BgzfCtl) + (size_t)nm * 8 + 16;
+    if ((rc = stage(t_up + t_down + 64)) != ZB_OK) return rc;
+    uint8_t *h = static_cast<uint8_t *>(h_stage);
+    uint64_t *h_moff = reinterpret_cast<uint64_t *>(h);
+    uint32_t *h_mlen = reinterpret_cast<uint32_t *>(h + (size_t)nm * 8);
+    uint64_t *h_soff = reinterpret_cast<uint64_t *>(h + (size_t)nm * 16);
+    uint32_t *h_count = reinterpret_cast<uint32_t *>(h_soff + nm + 1);
+    BgzfCtl *h_ctl = reinterpret_cast<BgzfCtl *>(h + ((t_up + 15) & ~(size_t)15));
+    uint64_t *h_mout = reinterpret_cast<uint64_t *>(h_ctl + 1);
+    uint32_t *h_check = reinterpret_cast<uint32_t *>(h_mout + nm);
+    uint64_t off = 0;
+    for (uint32_t i = 0; i < nm; i++) {
+        h_moff[i] = off;
+        h_mlen[i] = (uint32_t)(seg_off[i + 1] - seg_off[i]);
+        off = batch_stage_next(off, h_mlen[i]);
+    }
+    memcpy(h_soff, seg_off, ((size_t)nm + 1) * 8);
+    *h_count = nm;
+    // S_BATCH: the caller's offsets | the joined check | a host source
+    const size_t a_soff = (((size_t)nm + 1) * 8 + 63) & ~(size_t)63;
+    void *p;
+    if ((rc = reserve(S_BATCH, a_soff + 64 + (src_dev ? 0 : total), &p)) != ZB_OK) return rc;
+    uint8_t *t = static_cast<uint8_t *>(p);
+    uint64_t *d_soff = reinterpret_cast<uint64_t *>(t);
+    bj.fcheck = reinterpret_cast<uint32_t *>(t + a_soff);
+    const uint8_t *d_src = src_dev ? static_cast<const uint8_t *>(src) + seg_off[0] : t + a_soff + 64;
+    const size_t mi_bytes = ((size_t)nm * sizeof(JobInfo) + 15) & ~(size_t)15;
+
+    CK(cudaEventRecord(ev0, st));
+    CK(cudaMemcpyAsync(bj.moff, h_moff, (size_t)nm * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(bj.mlen, h_mlen, (size_t)nm * 4, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_soff, h_soff, ((size_t)nm + 1) * 8, cudaMemcpyHostToDevice, st));
+    if (!src_dev) CK(cudaMemcpyAsync(const_cast<uint8_t *>(d_src), static_cast<const uint8_t *>(src) + seg_off[0], total, cudaMemcpyHostToDevice, st));
+    // staging: every segment at its offset with zeros behind it, as a batch item (zb_bgzf.h: the bytes behind a segment do not matter)
+    k_batch_stage<<<nm, 256, 0, st>>>(d_src, d_soff, nullptr, bj, const_cast<uint8_t *>(jb.in), span);
+    CK(cudaMemsetAsync(const_cast<uint8_t *>(jb.in) + span, 0, kPad + 16, st));
+    launches++;
+    CK(cudaMemsetAsync(bj.minfo, 0, mi_bytes + sizeof(BgzfCtl), st));
+    CK(cudaMemcpyAsync(&bj.ctl->count, h_count, 4, cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(jb.out, 0, out_cap, st));
+    // the segments' checks, joined in order into the whole input's
+    if (wrap == 1) {
+        CK(launch_adler32_segments(jb.in, bj.moff, bj.mlen, nm, bj.mcheck, st));
+        CK(launch_adler32_join(bj.mcheck, bj.mlen, &bj.ctl->count, bj.fcheck, st));
+    } else if (wrap == 2) {
+        CK(launch_crc32_segments(jb.in, bj.moff, bj.mlen, nm, bj.mcheck, st));
+        CK(launch_crc32_join(bj.mcheck, bj.mlen, &bj.ctl->count, bj.fcheck, st));
+    } else CK(cudaMemsetAsync(bj.fcheck, 0, 4, st));
+    if (wrap) launches += 2;
+    if ((rc = members_launch(jb, bj, level, d_freq)) != ZB_OK) return rc;
+    CK(cudaMemcpyAsync(h_ctl, bj.ctl, sizeof(BgzfCtl), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(h_mout, bj.mout, (size_t)nm * 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(h_check, bj.fcheck, 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (h_ctl->error) { snprintf(g_err, sizeof g_err, "engine error flags 0x%x (flushed)", h_ctl->error); return ZB_E_INTERNAL; }
+    const uint64_t out_bytes = h_ctl->out_bytes;
+    if (out_bytes > dst_cap) {
+        res->out_bytes = out_bytes;
+        return ZB_E_BUF;
+    }
+    CK(cudaMemcpyAsync(dst, jb.out, out_bytes, dst_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
+    CK(cudaEventRecord(ev1, st));
+    CK(cudaStreamSynchronize(st));
+    float ms = 0;
+    CK(cudaEventElapsedTime(&ms, ev0, ev1));
+    restart[0] = stream_header_len(wrap);
+    for (uint32_t i = 1; i < nm; i++) restart[i] = h_mout[i];
+    restart[nm] = out_bytes - stream_trailer_len(wrap);
+    res->out_bytes = out_bytes;
+    res->check = *h_check;
+    res->data_type = (int32_t)h_ctl->data_type;
+    res->iterations = level > 0 ? 1 : 0;
+    res->n_symbols = h_ctl->n_syms;
+    res->n_blocks = h_ctl->n_blocks + nm - 1; // with the empty stored block of every full flush
+    res->gpu_launches = launches;
+    res->exact_parity = 1;
+    res->gpu_ms = ms;
+    res->bits_used = 8;
+    return ZB_OK;
+}
+
 // zb_deflate_index (DESIGN.md §2l): the access points of the stream just written, from the writer's block tables on the device.  One
 // launch of k_deflate_points over the targets and the members' first headers, one host sync for its candidates and the member
 // table, then index_fill: one launch of k_index_windows, whose windows come out of the staged input with the caller's final sync.
@@ -1181,6 +1320,22 @@ int zb_deflate_batch(zb_engine *z, const void *src, const uint64_t *src_off, siz
                               dst_off, checks, res);
 }
 
+int zb_deflate_flushed(zb_engine *z, const void *src, const uint64_t *seg_off, size_t n_segs, int src_dev, void *dst, size_t cap,
+                       int dst_dev, int level, int strategy, int window_bits, uint32_t flags, uint64_t *restart, zb_deflate_result *res)
+{
+    if (!z) return ZB_E_NODEVICE;
+    z->e.shard.phase = 0; // a range job in progress is gone (its buffers are reused)
+    return z->e.deflate_flushed(src, seg_off, n_segs, src_dev != 0, dst, cap, dst_dev != 0, level, strategy, window_bits, flags, restart, res);
+}
+
+size_t zb_deflate_flushed_bound(const uint64_t *seg_off, size_t n_segs)
+{
+    if (n_segs == 0) return (size_t)zb::stream_bound(0);
+    uint64_t b = 18; // one header and trailer (zb_bgzf.h)
+    for (size_t i = 0; i < n_segs; i++) b += zb::stream_bound(seg_off[i + 1] - seg_off[i]);
+    return (size_t)b;
+}
+
 size_t zb_deflate_batch_bound(const uint64_t *src_off, size_t n_items)
 {
     size_t b = 0;
@@ -1205,6 +1360,14 @@ int zb_inflate_batch(zb_engine *z, const void *src, const uint64_t *src_off, siz
     if (!z) return ZB_E_NODEVICE;
     z->e.shard.phase = 0; // a range job in progress is gone (its buffers are reused)
     return z->e.inflate_batch(nullptr, 0, src, src_off, n_items, src_dev != 0, dst, dst_off, dst_dev != 0, window_bits, items);
+}
+
+int zb_inflate_flushed(zb_engine *z, const void *src, size_t src_len, int src_dev, const uint64_t *restart, size_t n_segs, const uint32_t *which,
+                       size_t n_which, void *dst, const uint64_t *dst_off, int dst_dev, int window_bits, zb_inflate_result *items)
+{
+    if (!z) return ZB_E_NODEVICE;
+    z->e.shard.phase = 0; // a range job in progress is gone (its buffers are reused)
+    return z->e.inflate_flushed(src, src_len, src_dev != 0, restart, n_segs, which, n_which, dst, dst_off, dst_dev != 0, window_bits, items);
 }
 
 int zb_inflate(zb_engine *z, const void *src, size_t n, int src_dev, void *dst, size_t cap, int dst_dev, int window_bits,

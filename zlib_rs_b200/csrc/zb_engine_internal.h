@@ -104,6 +104,10 @@ struct Engine {
     int deflate_batch(const void *dict, size_t dict_len, const void *src, const uint64_t *src_off, size_t n_items, bool src_dev, void *dst,
                       size_t dst_cap, bool dst_dev, int level, int strategy, int window_bits, uint32_t flags, uint64_t *dst_off,
                       uint32_t *checks, zb_deflate_result *res);
+    int deflate_flushed(const void *src, const uint64_t *seg_off, size_t n_segs, bool src_dev, void *dst, size_t dst_cap, bool dst_dev,
+                        int level, int strategy, int window_bits, uint32_t flags, uint64_t *restart, zb_deflate_result *res);
+    int inflate_flushed(const void *src, size_t src_len, bool src_dev, const uint64_t *restart, size_t n_segs, const uint32_t *which,
+                        size_t n_which, void *dst, const uint64_t *dst_off, bool dst_dev, int window_bits, zb_inflate_result *items);
     int members_reserve(JobBufs &jb, BgzfJob &bj, uint32_t nm, uint32_t S, size_t span, int level, size_t out_cap, uint32_t wrap,
                         uint32_t **d_freq);
     int members_launch(JobBufs &jb, BgzfJob &bj, int level, uint32_t *d_freq);

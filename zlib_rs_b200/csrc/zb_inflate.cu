@@ -1512,6 +1512,63 @@ __global__ void __launch_bounds__(256) k_batch_verdict(const InfState *ist, cons
     out[i] = BatchResult{r.out_bytes, r.in_bytes, check, err};
 }
 
+// ================================================================================================
+// Flushed streams (zb_inflate_flushed, DESIGN.md §2m): item i decodes one segment of a stream written with Z_FULL_FLUSH, as raw
+// deflate from its restart point with an empty window (inflate_warp's segment mode, D0 = 0).
+//   k_flushed_members   one warp per item.  A segment that is not the last is decoded up to the LEN field of its closing empty
+//                       stored block, so the decoder stops in front of LEN/NLEN with every bit used (stored_wait);
+//   k_crc_segments, k_adler_segments  the check of each item's output;
+//   k_flushed_verdict   one status per item: the decoder's, or whether the segment ends at its restart point as a flush ends.
+// ================================================================================================
+struct FlushItem {
+    uint64_t in_off, in_len, out_off, out_cap;
+    uint32_t fin, pad; // fin: the last segment, which ends with the BFINAL block
+};
+
+__global__ void __launch_bounds__(32) k_flushed_members(const uint8_t *__restrict__ src, const FlushItem *items, uint8_t *__restrict__ dst,
+                                                        int window_bits, InfState *ist, uint64_t *out_off, uint32_t *crc_len,
+                                                        uint32_t *adler_len)
+{
+    extern __shared__ __align__(16) uint8_t smem_raw[];
+    const uint32_t i = blockIdx.x;
+    const FlushItem it = items[i];
+    const uint64_t n = it.fin ? it.in_len : (it.in_len >= 4 ? it.in_len - 4 : 0);
+    inflate_warp(*reinterpret_cast<InfShared *>(smem_raw), src + it.in_off, n, dst + it.out_off, it.out_cap, -15, ist + i,
+                 InfSeg{0, nullptr, 0, 1});
+    __syncwarp();
+    if (threadIdx.x == 0) {
+        const InfState &r = ist[i];
+        const uint32_t o = r.err == IE_OUTPUT_FULL ? 0u : (uint32_t)r.out_bytes; // slots hold below 4 GiB (host check)
+        out_off[i] = it.out_off;
+        crc_len[i] = window_bits == 31 ? o : 0u;
+        adler_len[i] = window_bits == 15 ? o : 0u;
+    }
+}
+
+constexpr uint32_t kFlushBadEnd = 0xffffu; // BatchResult::err of a segment that does not end at its restart point
+__global__ void __launch_bounds__(256) k_flushed_verdict(const uint8_t *__restrict__ src, const FlushItem *items, const InfState *ist,
+                                                         const uint32_t *crc, const uint32_t *adler, uint32_t n, int window_bits,
+                                                         BatchResult *out)
+{
+    const uint32_t i = blockIdx.x * 256 + threadIdx.x;
+    if (i >= n) return;
+    const InfState &r = ist[i];
+    const FlushItem it = items[i];
+    uint32_t err = r.err;
+    if (it.fin) {
+        // the BFINAL block is complete and ends in the segment's last byte
+        if (err == IE_TRUNCATED || (err == IE_OK && (!r.final_done || (r.blk_bit + 7) >> 3 != it.in_len))) err = kFlushBadEnd;
+    } else if (err == IE_TRUNCATED || err == IE_OK) {
+        // stopped in front of LEN/NLEN of a stored block whose header starts at blk_bit: BFINAL 0, then 00 00 ff ff to the end
+        const uint8_t *e = src + it.in_off + it.in_len - 4;
+        const bool marker = err == IE_TRUNCATED && r.stored_wait && it.in_len >= 5 && e[0] == 0 && e[1] == 0 && e[2] == 0xff &&
+                            e[3] == 0xff && ((src[it.in_off + (r.blk_bit >> 3)] >> (r.blk_bit & 7)) & 1u) == 0;
+        err = marker ? (uint32_t)IE_OK : kFlushBadEnd;
+    }
+    const uint32_t check = window_bits == 31 ? crc[i] : window_bits == 15 ? adler[i] : 0u;
+    out[i] = BatchResult{r.out_bytes, it.in_len, check, err};
+}
+
 struct IdxPiece;
 __global__ void __launch_bounds__(32) k_index_extract(const IdxPiece *pieces, InfState *st);
 
@@ -1550,6 +1607,8 @@ int Engine::inflate_init()
     if (e != cudaSuccess) { snprintf(g_err, sizeof g_err, "k_members attr: %s", cudaGetErrorString(e)); return ZB_E_CUDA; }
     e = cudaFuncSetAttribute(k_batch_members, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(InfShared));
     if (e != cudaSuccess) { snprintf(g_err, sizeof g_err, "k_batch_members attr: %s", cudaGetErrorString(e)); return ZB_E_CUDA; }
+    e = cudaFuncSetAttribute(k_flushed_members, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(InfShared));
+    if (e != cudaSuccess) { snprintf(g_err, sizeof g_err, "k_flushed_members attr: %s", cudaGetErrorString(e)); return ZB_E_CUDA; }
     e = cudaFuncSetAttribute(k_index_extract, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(InfShared));
     if (e != cudaSuccess) { snprintf(g_err, sizeof g_err, "k_index_extract attr: %s", cudaGetErrorString(e)); return ZB_E_CUDA; }
     if (cudaMalloc(&d_inf_state, sizeof(InfState)) != cudaSuccess) return ZB_E_MEM;
@@ -1966,6 +2025,104 @@ int Engine::inflate_batch(const void *dict, size_t dict_len, const void *src, co
         r.check = b.check;
         r.status = b.err == IE_OK ? ZB_OK : b.err == IE_OUTPUT_FULL ? ZB_E_BUF : ZB_E_DATA;
         if (r.status == ZB_E_DATA) snprintf(r.msg, sizeof r.msg, "%s", inf_msg(b.err));
+        r.gpu_launches = launches;
+        r.gpu_ms = ms;
+        if (status == ZB_OK) status = r.status;
+    }
+    return status;
+}
+
+// zb_inflate_flushed: see zb_engine.h.  Fixed launches (k_flushed_members, the two checksum kernels, k_flushed_verdict) and one
+// host sync.  A host source is uploaded as one range, [restart[0], restart[n_segs]).
+int Engine::inflate_flushed(const void *src, size_t src_len, bool src_dev, const uint64_t *restart, size_t n_segs, const uint32_t *which,
+                            size_t n_which, void *dst, const uint64_t *dst_off, bool dst_dev, int window_bits, zb_inflate_result *items)
+{
+    if (!restart || (n_which && (!which || !dst_off || !items))) { snprintf(g_err, sizeof g_err, "inflate_flushed: null argument"); return ZB_E_PARAM; }
+    if (window_bits != 15 && window_bits != -15 && window_bits != 31) {
+        snprintf(g_err, sizeof g_err, "inflate_flushed takes window_bits 15, -15 or 31");
+        return ZB_E_PARAM;
+    }
+    if (n_which > kBatchMaxInflateItems) {
+        snprintf(g_err, sizeof g_err, "inflate_flushed: %zu items (at most %llu)", n_which, (unsigned long long)kBatchMaxInflateItems);
+        return ZB_E_PARAM;
+    }
+    for (size_t k = 0; k < n_segs; k++)
+        if (restart[k + 1] < restart[k]) { snprintf(g_err, sizeof g_err, "inflate_flushed: restart points decrease at %zu", k); return ZB_E_PARAM; }
+    if (restart[n_segs] > src_len) {
+        snprintf(g_err, sizeof g_err, "inflate_flushed: restart[%zu] = %llu lies beyond the %zu source bytes", n_segs,
+                 (unsigned long long)restart[n_segs], src_len);
+        return ZB_E_PARAM;
+    }
+    const uint32_t nm = (uint32_t)n_which;
+    for (uint32_t i = 0; i < nm; i++) {
+        if (which[i] >= n_segs) { snprintf(g_err, sizeof g_err, "inflate_flushed: item %u names segment %u of %zu", i, which[i], n_segs); return ZB_E_PARAM; }
+        if (dst_off[i + 1] < dst_off[i]) { snprintf(g_err, sizeof g_err, "inflate_flushed: offsets of item %u decrease", i); return ZB_E_PARAM; }
+        if (dst_off[i + 1] - dst_off[i] > 0xffffffffull) { snprintf(g_err, sizeof g_err, "inflate_flushed: slot of item %u is 4 GiB or more", i); return ZB_E_PARAM; }
+    }
+    const uint64_t in_lo = restart[0], in_total = restart[n_segs] - restart[0], out_total = nm ? dst_off[nm] - dst_off[0] : 0;
+    if ((nm && in_total && !src) || (out_total && !dst)) { snprintf(g_err, sizeof g_err, "inflate_flushed: null buffer"); return ZB_E_PARAM; }
+    for (uint32_t i = 0; i < nm; i++) memset(&items[i], 0, sizeof items[i]);
+    if (nm == 0) return ZB_OK;
+    CKI(cudaSetDevice(device));
+    launches = 0;
+    int rc;
+    void *p;
+    // S_BATCH: item table | results | output offsets | the two checksum length tables and their checks | decoder states
+    const size_t a_items = ((size_t)nm * sizeof(FlushItem) + 63) & ~(size_t)63, a_res = ((size_t)nm * sizeof(BatchResult) + 63) & ~(size_t)63;
+    const size_t a4 = ((size_t)nm * 4 + 63) & ~(size_t)63, a8 = ((size_t)nm * 8 + 63) & ~(size_t)63;
+    const size_t a_ist = ((size_t)nm * sizeof(InfState) + 63) & ~(size_t)63;
+    if ((rc = reserve(S_BATCH, a_items + a_res + a8 + 4 * a4 + a_ist, &p)) != ZB_OK) return rc;
+    uint8_t *t = static_cast<uint8_t *>(p);
+    FlushItem *d_items = reinterpret_cast<FlushItem *>(t);
+    BatchResult *d_res = reinterpret_cast<BatchResult *>(t + a_items);
+    uint64_t *d_ooff = reinterpret_cast<uint64_t *>(t + a_items + a_res);
+    uint32_t *d_clen = reinterpret_cast<uint32_t *>(t + a_items + a_res + a8), *d_alen = d_clen + a4 / 4;
+    uint32_t *d_crc = d_alen + a4 / 4, *d_adler = d_crc + a4 / 4;
+    InfState *d_ist = reinterpret_cast<InfState *>(d_adler + a4 / 4);
+    if ((rc = stage(a_items + a_res + 16)) != ZB_OK) return rc;
+    FlushItem *h_items = static_cast<FlushItem *>(h_stage);
+    BatchResult *h_res = reinterpret_cast<BatchResult *>(static_cast<uint8_t *>(h_stage) + a_items);
+    for (uint32_t i = 0; i < nm; i++) {
+        const uint32_t k = which[i];
+        h_items[i] = FlushItem{restart[k] - in_lo, restart[k + 1] - restart[k], dst_off[i] - dst_off[0], dst_off[i + 1] - dst_off[i],
+                               k + 1 == n_segs ? 1u : 0u, 0};
+    }
+    const uint8_t *d_src = static_cast<const uint8_t *>(src) + in_lo;
+    uint8_t *d_dst = static_cast<uint8_t *>(dst) + dst_off[0];
+    CKI(cudaEventRecord(ev0, st));
+    if (!src_dev) {
+        if ((rc = reserve(S_INF0, in_total + 64, &p)) != ZB_OK) return rc;
+        if (in_total) CKI(cudaMemcpyAsync(p, d_src, in_total, cudaMemcpyHostToDevice, st));
+        d_src = static_cast<const uint8_t *>(p);
+    }
+    if (!dst_dev) {
+        if ((rc = reserve(S_INF1, out_total + 64, &p)) != ZB_OK) return rc;
+        d_dst = static_cast<uint8_t *>(p);
+        CKI(cudaMemsetAsync(d_dst, 0, out_total, st)); // the slots go back whole: what lies behind an item's output is zeros
+    }
+    CKI(cudaMemcpyAsync(d_items, h_items, (size_t)nm * sizeof(FlushItem), cudaMemcpyHostToDevice, st));
+    k_flushed_members<<<nm, 32, sizeof(InfShared), st>>>(d_src, d_items, d_dst, window_bits, d_ist, d_ooff, d_clen, d_alen);
+    CKI(launch_crc32_segments(d_dst, d_ooff, d_clen, nm, d_crc, st));
+    CKI(launch_adler32_segments(d_dst, d_ooff, d_alen, nm, d_adler, st));
+    k_flushed_verdict<<<(nm + 255) / 256, 256, 0, st>>>(d_src, d_items, d_ist, d_crc, d_adler, nm, window_bits, d_res);
+    launches += 4;
+    CKI(cudaMemcpyAsync(h_res, d_res, (size_t)nm * sizeof(BatchResult), cudaMemcpyDeviceToHost, st));
+    if (!dst_dev && out_total) CKI(cudaMemcpyAsync(static_cast<uint8_t *>(dst) + dst_off[0], d_dst, out_total, cudaMemcpyDeviceToHost, st));
+    CKI(cudaEventRecord(ev1, st));
+    CKI(cudaStreamSynchronize(st));
+    CKI(cudaGetLastError());
+    float ms = 0;
+    CKI(cudaEventElapsedTime(&ms, ev0, ev1));
+    int status = ZB_OK;
+    for (uint32_t i = 0; i < nm; i++) {
+        zb_inflate_result &r = items[i];
+        const BatchResult &b = h_res[i];
+        r.out_bytes = b.out_bytes;
+        r.in_bytes = b.in_bytes;
+        r.check = b.check;
+        r.status = b.err == IE_OK ? ZB_OK : b.err == IE_OUTPUT_FULL ? ZB_E_BUF : ZB_E_DATA;
+        if (r.status == ZB_E_DATA)
+            snprintf(r.msg, sizeof r.msg, "%s", b.err == kFlushBadEnd ? "segment does not end at its restart point" : inf_msg(b.err));
         r.gpu_launches = launches;
         r.gpu_ms = ms;
         if (status == ZB_OK) status = r.status;

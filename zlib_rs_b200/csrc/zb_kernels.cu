@@ -1868,7 +1868,7 @@ __global__ void __launch_bounds__(256) k_bgzf_hist(JobBufs jb, BgzfJob bj, uint3
         const bool last = k + 1 == nblocks;
         bd.sym_begin = base + begin;
         bd.sym_count = count;
-        bd.last = last;
+        bd.last = last && (!bj.flushed || m + 1 == bj.nm); // a segment of a flushed stream ends its stream only if it is the last
         const uint32_t start = begin == 0 ? bj.pstart : sym_end(syms[begin - 1]);
         const uint32_t end = last ? len : sym_end(syms[begin + count - 1]);
         bd.in_start = base + start;
@@ -1886,7 +1886,8 @@ __global__ void __launch_bounds__(32) k_bgzf_build(JobBufs jb, BgzfJob bj, const
     const uint32_t b = blockIdx.x, m = b / kBgzfMaxBlocks, k = b % kBgzfMaxBlocks;
     const uint32_t nblocks = bj.minfo[m].n_blocks;
     if (k >= nblocks) return;
-    build_blocks_body(&jb.blocks[b], freq + (size_t)b * 320, jb.serial_mode == 1, k == 0, k + 1 == nblocks, true, false);
+    build_blocks_body(&jb.blocks[b], freq + (size_t)b * 320, jb.serial_mode == 1, k == 0, k + 1 == nblocks, !bj.flushed || m + 1 == bj.nm,
+                      false);
 }
 
 // bit_base is absolute here (k_bgzf_scan); a member written stored has no blocks to encode

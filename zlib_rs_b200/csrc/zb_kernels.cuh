@@ -142,6 +142,10 @@ struct BgzfJob {
     uint32_t pstart;    // parse start of every member: the dictionary's bytes D' staged in front of each item (0: none)
     uint32_t fdict;     // zlib items get FDICT and DICTID = *dictid (a batch with a preset dictionary)
     const uint32_t *dictid;
+    uint32_t flushed;   // 1: the members are the segments of one stream written with Z_FULL_FLUSH (zb_deflate_flushed): `wrap`
+                        // frames the stream, member 0 has the header, the last the trailer, every other one the empty stored block
+    uint32_t *fcheck;   // flushed: the check of the whole input, joined from mcheck
+    uint32_t isize;     // flushed: the input length mod 2^32 (gzip's ISIZE)
 };
 
 // zb_deflate_index (DESIGN.md §2l): k_deflate_points runs one warp per slot, the targets k * span (k = 1..K) and then the first
@@ -171,6 +175,7 @@ cudaError_t launch_crc32(const uint8_t *d_buf, uint64_t len, uint32_t start, voi
 cudaError_t launch_crc32_segments(const uint8_t *d_buf, const uint64_t *d_off, const uint32_t *d_len, uint32_t nseg, uint32_t *d_crc,
                                   cudaStream_t st);
 cudaError_t launch_crc32_join(const uint32_t *d_crc, const uint32_t *d_len, const uint32_t *d_count, uint32_t *d_out, cudaStream_t st);
+cudaError_t launch_adler32_join(const uint32_t *d_adler, const uint32_t *d_len, const uint32_t *d_count, uint32_t *d_out, cudaStream_t st);
 // adler32 of every segment [off[s], off[s] + len[s]) of d_buf (batch items, zb_bgzf.cu / zb_inflate.cu)
 cudaError_t launch_adler32_segments(const uint8_t *d_buf, const uint64_t *d_off, const uint32_t *d_len, uint32_t nseg, uint32_t *d_adler,
                                     cudaStream_t st);
