@@ -286,7 +286,31 @@ ZB_API int zb_inflate_blocks(zb_engine *e, const void *src, size_t src_len, uint
  *     points   n_points x {u64 out_off, bit, hdr_bit; u32 member, btype, window_len, 0}, sorted by (out_off, bit)  (40 bytes)
  *     windows  the window_len bytes of every point, in point order
  * zb_index_deserialize: validates every field (magic, version, lengths, order, bits below 8 * in_bytes, members, btype, window
- *   lengths) and gives ZB_E_DATA for a malformed blob, never reading outside buf[0, len).
+ *   lengths) and gives ZB_E_DATA for a malformed blob, never reading outside buf[0, len).  Span 0 (a member index) is accepted
+ *   exactly when there is one point per member.
+ *
+ * Member indexes of BGZF files (DESIGN.md §2n).  A BGZF member starts with an empty window, its BSIZE says where the next member
+ * starts and its ISIZE how long its output is; so its start is an access point, found from about 30 header bytes per member.
+ * zb_index_bgzf: the index of the BGZF file src[0, src_len), built from the member headers alone: nothing is decoded and no window
+ *   is stored.  Members are taken from offset 0 on while the next two bytes are 1f 8b (as ZB_INF_MEMBERS goes on); any other bytes
+ *   end the walk, and the 28-byte end-of-file member is an ordinary member with empty output.  The index has span 0, window_bits 31,
+ *   one point per member (its first block header, window_len 0), out_start / out_end the prefix sums of ISIZE, total_out their
+ *   sum, in_bytes the end of the last member, and check the crc32_combine of the trailer CRCs over the ISIZEs: what zb_index_build
+ *   reports for an intact file.  res: status, in_bytes, out_bytes (= total_out), check, gpu_launches, gpu_ms, msg.
+ *   ZB_E_DATA, *out = NULL: no BGZF member at offset 0, a 1f 8b member that is not BGZF or runs past src_len, or a member whose first
+ *   block has BTYPE 3; the message names the member's offset (zb_index_build indexes any gzip file).
+ *   A host source is walked on the host and never uploaded (0 launches; files larger than device memory can be indexed).  A device
+ *   source is walked on the device: 7 launches and 2 host syncs, and more than 2^20 BGZF header candidates give ZB_E_PARAM.  Both
+ *   give the same index, byte for byte.
+ *   The index trusts BSIZE and ISIZE, as .gzi readers do.  zb_index_extract checks ISIZE where a range needs it: a range that
+ *   reaches a member's end is decoded to the end of that member's final block, and gets ZB_E_DATA "incorrect length check" when
+ *   that block does not end exactly there.  Extract, serialize, get_point and free work on a member index as on any index;
+ *   zb_index_build and zb_deflate_index never make one.
+ * zb_index_voffset: *out_off = the output offset of the BGZF virtual offset voffset = coffset << 16 | uoffset (as in BAI, TBI and
+ *   CSI chunks): coffset must be some member's in_start and uoffset at most that member's output length (equal to it is the next
+ *   member's start); then *out_off = out_start + uoffset.  Anything else gives ZB_E_PARAM.  Works on every index with members,
+ *   zb_index_build(ZB_INF_MEMBERS) indexes of BGZF files included.  A BAI chunk [vbeg, vend) is the range
+ *   [voffset(vbeg), voffset(vend)) of zb_index_extract.
  * An index is host memory, independent of the engine that built it, and read-only: several threads may extract through one index
  * with an engine each. */
 typedef struct zb_index zb_index;
@@ -321,6 +345,8 @@ ZB_API int zb_index_build(zb_engine *e, const void *src, size_t src_len, int src
 ZB_API int zb_deflate_index(zb_engine *e, const void *src, size_t src_len, int src_on_device, void *dst, size_t dst_cap,
                             int dst_on_device, int level, int strategy, int window_bits, uint32_t flags, uint64_t span,
                             zb_deflate_result *res, zb_index **out);
+ZB_API int zb_index_bgzf(zb_engine *e, const void *src, size_t src_len, int src_on_device, zb_inflate_result *res, zb_index **out);
+ZB_API int zb_index_voffset(const zb_index *idx, uint64_t voffset, uint64_t *out_off);
 ZB_API int zb_index_extract(zb_engine *e, const zb_index *idx, const void *src, size_t src_len, int src_on_device, const uint64_t *offsets,
                             size_t n_ranges, void *dst, const uint64_t *dst_off, int dst_on_device, zb_inflate_result *items);
 ZB_API int zb_index_serialize(const zb_index *idx, void *buf, size_t cap, size_t *len);

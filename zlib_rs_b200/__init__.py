@@ -158,6 +158,9 @@ def lib():
             L.zb_index_get_info.argtypes = [vp, ctypes.POINTER(IndexInfo)]
             L.zb_index_get_point.argtypes = [vp, sz, ctypes.POINTER(IndexPoint)]
             L.zb_index_free.argtypes, L.zb_index_free.restype = [vp], None
+        if hasattr(L, "zb_index_bgzf"):
+            L.zb_index_bgzf.argtypes = [vp, vp, sz, ci, ctypes.POINTER(InflateResult), ctypes.POINTER(vp)]
+            L.zb_index_voffset.argtypes = [vp, u64, ctypes.POINTER(u64)]
         if hasattr(L, "zb_deflate_index"):
             L.zb_deflate_index.argtypes = [vp, vp, sz, ci, vp, sz, ci, ci, ci, ci, u32, u64, ctypes.POINTER(DeflateResult),
                                            ctypes.POINTER(vp)]
@@ -449,6 +452,15 @@ class Index:
             out.append(dict(out_off=p.out_off, bit=p.bit, hdr_bit=p.hdr_bit, member=p.member, btype=p.btype, window_len=p.window_len,
                             window=ctypes.string_at(p.window, p.window_len) if p.window_len else b""))
         return out
+
+    def voffset(self, v):
+        """The output offset of the BGZF virtual offset v = coffset << 16 | uoffset (zb_index_voffset): coffset a member's first
+        byte, uoffset at most its output length.  Raises ZlibError(ZB_E_PARAM) for any other v."""
+        out = ctypes.c_uint64(0)
+        rc = lib().zb_index_voffset(self.h, v, ctypes.byref(out))
+        if rc != 0:
+            raise ZlibError(rc, lib().zb_last_error().decode())
+        return out.value
 
     def close(self):
         if self.h:
@@ -773,6 +785,19 @@ class Engine:
         rc = lib().zb_index_build(self.h, src, n, int(src_on_device), dst, out_cap, int(dst_on_device), window_bits, flags, span,
                                   ctypes.byref(res), ctypes.byref(h))
         return rc, (own.raw[: res.out_bytes] if own is not None else None), res, (Index(h.value) if rc == 0 and h.value else None)
+
+    def index_bgzf(self, src, n=None, src_on_device=False):
+        """The member index of a BGZF file from its headers alone, without a decode (zb_index_bgzf): one point per member, span 0.
+        A host `src` (bytes or any buffer) is walked on the host and not uploaded; a device `src` is a pointer + n.  Returns
+        (rc, InflateResult, Index or None); the Index only with rc == 0.  A BAI chunk [vbeg, vend) is then
+        extract(src, idx, [(idx.voffset(vbeg), idx.voffset(vend) - idx.voffset(vbeg))])."""
+        res = InflateResult()
+        keep = None
+        if not src_on_device:
+            src, n, keep = _host_view(src)
+        h = ctypes.c_void_p()
+        rc = lib().zb_index_bgzf(self.h, src, n, int(src_on_device), ctypes.byref(res), ctypes.byref(h))
+        return rc, res, (Index(h.value) if rc == 0 and h.value else None)
 
     def extract(self, src, index, ranges, n=None, src_on_device=False, dst=None, dst_off=None, dst_on_device=False):
         """Extract byte ranges of an indexed stream in one call (zb_index_extract).  `ranges`: a list of (offset, length); a

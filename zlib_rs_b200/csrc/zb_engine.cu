@@ -4,6 +4,7 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
+#include <algorithm>
 #include <new>
 #include "../../include/zb_engine.h"
 #include "zb_kernels.cuh"
@@ -1443,6 +1444,39 @@ int zb_deflate_index(zb_engine *z, const void *src, size_t src_len, int src_dev,
     if (rc == ZB_OK) *out = iw.out;
     else delete iw.out;
     return rc;
+}
+
+int zb_index_bgzf(zb_engine *z, const void *src, size_t src_len, int src_dev, zb_inflate_result *res, zb_index **out)
+{
+    if (!z) return ZB_E_NODEVICE;
+    if (!out || !res || (!src && src_len)) { snprintf(zb::g_err, sizeof zb::g_err, "index_bgzf: null argument"); return ZB_E_PARAM; }
+    *out = nullptr;
+    z->e.shard.phase = 0; // a range job in progress is gone (its buffers are reused)
+    zb_index *x = new (std::nothrow) zb_index;
+    if (!x) return ZB_E_MEM;
+    int rc;
+    try {
+        rc = z->e.index_bgzf(src, src_len, src_dev != 0, res, x);
+    } catch (const std::bad_alloc &) {
+        rc = ZB_E_MEM;
+    }
+    if (rc == ZB_OK) *out = x;
+    else delete x;
+    return rc;
+}
+
+int zb_index_voffset(const zb_index *x, uint64_t voffset, uint64_t *out_off)
+{
+    if (!x || !out_off) return ZB_E_PARAM;
+    const uint64_t coff = voffset >> 16, uoff = voffset & 0xffff;
+    const auto m = std::lower_bound(x->m.begin(), x->m.end(), coff, [](const zb::IdxMember &a, uint64_t c) { return a.in_start < c; });
+    if (m == x->m.end() || m->in_start != coff || uoff > m->out_end - m->out_start) {
+        snprintf(zb::g_err, sizeof zb::g_err, "index_voffset: %llu:%llu is not a position in a member", (unsigned long long)coff,
+                 (unsigned long long)uoff);
+        return ZB_E_PARAM;
+    }
+    *out_off = m->out_start + uoff;
+    return ZB_OK;
 }
 
 int zb_index_extract(zb_engine *z, const zb_index *idx, const void *src, size_t src_len, int src_dev, const uint64_t *offsets,

@@ -120,6 +120,7 @@ struct Engine {
     int index_points(const uint8_t *d_src, const uint8_t *d_dst, const zb_inflate_result *res, int window_bits, IdxBuild *ib);
     int index_fill(zb_index &x, std::vector<IdxMember> &&M, std::vector<IdxPoint> &&pts, const IdxHeader &h, const uint8_t *d_src,
                    uint64_t shift);
+    int index_bgzf(const void *src, size_t n, bool src_dev, zb_inflate_result *res, zb_index *x);
     int index_extract(const zb_index *x, const void *src, size_t src_len, bool src_dev, const uint64_t *offsets, size_t n_ranges,
                       void *dst, const uint64_t *dst_off, bool dst_dev, zb_inflate_result *items);
     int inflate_batch(const void *dict, size_t dict_len, const void *src, const uint64_t *src_off, size_t n_items, bool src_dev, void *dst,

@@ -23,9 +23,13 @@
 //   IdxMember  x n_members         32 bytes each
 //   IdxPoint   x n_points          40 bytes each
 //   windows                        the window_len bytes of every point, in point order (win_bytes in all)
+//
+// A member index (span 0, zb_index_bgzf, DESIGN.md §2n) is built from BGZF member headers alone: one point per member, its first
+// block header, with an empty window.  zbi_bgzf_member and zbi_bgzf_walk below give its rows.
 #pragma once
 #include <string.h>
 #include "zb_core.h"
+#include "zb_members.h"
 
 namespace zb {
 
@@ -167,7 +171,8 @@ ZB_HD IdxSpan zbi_piece_span(const IdxPoint *p, uint64_t n_points, const IdxMemb
 }
 
 // Validation of a serialized index (it may come from outside the program): 0 when every field is consistent, else -1.  Nothing
-// outside buf[0, len) is read.  Checked: magic, version, lengths and counts (no overflow); members contiguous in the output and
+// outside buf[0, len) is read.  Checked: magic, version, span in [32 KiB, 4 GiB] or 0 (a member index) with exactly one point per
+// member, which the rules below then put at its member's start with an empty window; lengths and counts (no overflow); members contiguous in the output and
 // ordered in the input within in_bytes; points sorted by (out_off, bit) with strictly increasing bits below 8 * in_bytes, each inside
 // its member's input and output, members in order with a point at every member's start; btype 0..2 (a stored point is a header);
 // window_len = min(32768, the output in front of the point in its member); win_bytes the sum of the window lengths.
@@ -177,7 +182,7 @@ ZB_HD int zbi_validate(const uint8_t *buf, uint64_t len, IdxHeader *out)
     if (!buf || len < sizeof h) return -1;
     memcpy(&h, buf, sizeof h);
     if (h.magic != kIdxMagic || h.version != kIdxVersion) return -1;
-    if (h.span < kIdxMinSpan || h.span > kIdxMaxSpan) return -1;
+    if (h.span == 0 ? h.n_points != h.n_members : (h.span < kIdxMinSpan || h.span > kIdxMaxSpan)) return -1; // span 0: a member index
     const uint64_t rest = len - sizeof h;
     if (h.n_members == 0 || h.n_members > rest / sizeof(IdxMember)) return -1;
     const uint64_t after_m = rest - h.n_members * sizeof(IdxMember);
@@ -216,6 +221,45 @@ ZB_HD int zbi_validate(const uint8_t *buf, uint64_t len, IdxHeader *out)
     }
     if (cur != h.n_members - 1 || win != h.win_bytes) return -1;
     if (out) *out = h;
+    return 0;
+}
+
+// ---- Member index of a BGZF file (zb_index_bgzf, DESIGN.md §2n).  Every BGZF member starts with an empty window, so its first block
+// header is an access point, and its header says where it ends (BSIZE) and how much output it holds (ISIZE): the index needs no
+// decode.  It trusts BSIZE and ISIZE as .gzi readers do; zb_index_extract checks ISIZE for every range that reaches a member's end.
+
+// Member m's rows: p is its first byte, at input offset in_start; len = BSIZE + 1 as zbm_bgzf_bsize accepted it; out_start the
+// output in front of it.  *crc: its trailer CRC.
+ZB_HD void zbi_bgzf_member(const uint8_t *p, uint64_t in_start, uint32_t len, uint64_t out_start, uint32_t m, IdxMember *mb,
+                           IdxPoint *pt, uint32_t *crc)
+{
+    const uint64_t hl = (uint64_t)zbm_header_len(p, len); // zbm_bgzf_bsize checked that the header and the trailer fit in len
+    const uint64_t bit = 8 * (in_start + hl);
+    *mb = IdxMember{in_start, in_start + len, out_start, out_start + zbm_isize(p, len)};
+    *pt = IdxPoint{out_start, bit, bit, m, (uint32_t)(p[hl] >> 1) & 3u, 0, 0};
+    *crc = zbm_isize(p, len - 4); // the 4 bytes in front of ISIZE
+}
+
+// The walk: members from offset 0 on while the next two bytes are 1f 8b (gz_look, as ZB_INF_MEMBERS goes on).  emit(m, in_start,
+// len) takes each member.  Returns 0 with *in_bytes the end of the last member; else ZBI_BGZF_NOT (no BGZF member at offset *bad:
+// another gzip member, a member that runs past n, or no member at 0) or ZBI_BGZF_BTYPE (the first block of the member at *bad has
+// BTYPE 3), and emit has taken the members in front of *bad.
+constexpr int ZBI_BGZF_NOT = 1, ZBI_BGZF_BTYPE = 2;
+// Host only (a file larger than device memory can be walked; the device path finds the same members with the member-table kernels).
+template <typename Emit>
+inline int zbi_bgzf_walk(const uint8_t *src, uint64_t n, uint64_t *in_bytes, uint64_t *bad, Emit emit)
+{
+    uint64_t in = 0;
+    for (uint32_t m = 0;; m++) {
+        if (m && (n - in < 2 || src[in] != 0x1f || src[in + 1] != 0x8b)) break;
+        const int32_t bs = zbm_bgzf_bsize(src + in, n - in);
+        if (bs < 0) { *bad = in; return ZBI_BGZF_NOT; }
+        const uint32_t len = (uint32_t)bs + 1;
+        if (((src[in + zbm_header_len(src + in, len)] >> 1) & 3u) == 3) { *bad = in; return ZBI_BGZF_BTYPE; }
+        emit(m, in, len);
+        in += len;
+    }
+    *in_bytes = in;
     return 0;
 }
 

@@ -151,11 +151,14 @@ enum Cmd { C_NONE = 0, C_REFILL, C_FLUSH, C_COPY, C_DONE };
 // A range of an indexed stream (zb_index_extract, kRange = true, always in segment mode): the segment starts at an access point.
 // When that point is inside a block (resume), the block's tables come from its header at bit hdr_bit of hdr[0, hdr_n) -- a dynamic
 // header, or for a fixed block just its BFINAL bit -- and decoding goes on at the segment's start bit.  The first `skip` bytes of
-// output are discarded, the next `want` go to dst[0, want), and decoding stops as soon as they are complete.
+// output are discarded, the next `want` go to dst[0, want), and decoding stops as soon as they are complete.  With to_end (a range
+// of a member index that reaches its member's end, whose ISIZE is only a hint) decoding goes on to the end of the final block
+// instead, and more output than skip + want fails with IE_LENGTH_CHECK; so does a final block that ends short of it (the caller
+// tells that from out_bytes).
 struct InfRange {
     const uint8_t *hdr;
     uint64_t hdr_n, hdr_bit, skip, want;
-    uint32_t btype, resume;
+    uint32_t btype, resume, to_end;
 };
 
 // The one-warp decoder: a whole stream (header, blocks, trailer) or, in segment mode, raw blocks from a bit position.  Output goes to
@@ -234,6 +237,7 @@ __device__ __forceinline__ void inflate_warp(InfShared &S, const uint8_t *__rest
     }
     __syncwarp();
     const uint64_t rstop = D0 + rg.skip + rg.want; // kRange: the output position where decoding stops
+    const uint64_t rlim = rstop + (rg.to_end ? 1 : 0); // ... and with to_end the first one it must not reach
 
 #define NEED(nb) do { while (bits < (nb)) { hold |= (uint64_t)((ipos < n) ? S.in[ipos & (kInRing - 1)] : 0) << bits; ipos++; bits += 8; } } while (0)
 #define BITS(nb) ((uint32_t)(hold & ((1ull << (nb)) - 1)))
@@ -250,7 +254,7 @@ __device__ __forceinline__ void inflate_warp(InfShared &S, const uint8_t *__rest
             // run until a cooperative action is needed
             while (cmd == C_NONE) {
                 if (mode == 5) { cmd = C_DONE; break; }
-                if constexpr (kRange) { if (opos >= rstop) { mode = 5; continue; } }
+                if constexpr (kRange) { if (opos >= rlim) { if (rg.to_end) FAIL(IE_LENGTH_CHECK); else mode = 5; continue; } }
                 if (ifill < n && ifill - ipos < 1024) { cmd = C_REFILL; break; }
                 if (opos - oflush >= kOutRing / 2 + 2048) { cmd = C_FLUSH; break; }
                 if (consumed_bits > 8 * n) { FAIL(IE_TRUNCATED); continue; }
@@ -382,7 +386,7 @@ __device__ __forceinline__ void inflate_warp(InfShared &S, const uint8_t *__rest
                 if (mode == 2) { // stored bytes (bit buffer is byte aligned here)
                     uint32_t k = 0;
                     while (stored_left && k < 4096) {
-                        if constexpr (kRange) { if (opos >= rstop) break; }
+                        if constexpr (kRange) { if (opos >= rlim) break; }
                         if (ifill < n && ifill - ipos < 16) break;
                         if (opos - D0 >= cap) { FAIL(IE_OUTPUT_FULL); break; }
                         NEED(8);
@@ -397,7 +401,7 @@ __device__ __forceinline__ void inflate_warp(InfShared &S, const uint8_t *__rest
                 if (mode == 3) { // literal/length/distance loop (inflate.rs:1918-2158)
                     uint32_t budget = 512;
                     while (budget--) {
-                        if constexpr (kRange) { if (opos >= rstop) break; }
+                        if constexpr (kRange) { if (opos >= rlim) break; }
                         if (ifill < n && ifill - ipos < 64) break;
                         if (opos - oflush >= kOutRing - 4096) break;
                         NEED(48);
@@ -2283,7 +2287,7 @@ struct IdxPiece {
     const uint8_t *body, *hdr, *win;
     uint8_t *dst;
     uint64_t body_n, hdr_n, start_bit, hdr_bit, skip, want; // start_bit / hdr_bit: relative to body / hdr
-    uint32_t btype, resume, win_len, pad;
+    uint32_t btype, resume, win_len, to_end; // to_end: InfRange::to_end
 };
 
 __global__ void __launch_bounds__(32) k_index_extract(const IdxPiece *pieces, InfState *st)
@@ -2292,7 +2296,7 @@ __global__ void __launch_bounds__(32) k_index_extract(const IdxPiece *pieces, In
     const IdxPiece pc = pieces[blockIdx.x];
     inflate_warp<true>(*reinterpret_cast<InfShared *>(smem_raw), pc.body, pc.body_n, pc.dst, 1ull << 62, -15, st + blockIdx.x,
                        InfSeg{pc.start_bit, pc.win, pc.win_len, 1}, InfDict{nullptr, nullptr, 0, 0},
-                       InfRange{pc.hdr, pc.hdr_n, pc.hdr_bit, pc.skip, pc.want, pc.btype, pc.resume});
+                       InfRange{pc.hdr, pc.hdr_n, pc.hdr_bit, pc.skip, pc.want, pc.btype, pc.resume, pc.to_end});
 }
 
 static size_t a64(size_t b) { return (b + 63) & ~(size_t)63; }
@@ -2429,6 +2433,149 @@ int Engine::index_fill(zb_index &x, std::vector<IdxMember> &&M, std::vector<IdxP
     return ZB_OK;
 }
 
+// ---- zb_index_bgzf (zb_index.h, DESIGN.md §2n): the member index of a BGZF file from its headers alone.  From a device source the
+// member table of ZB_INF_MEMBERS finds the run of BGZF members from offset 0 (k_mem_count, k_mem_scan, k_mem_emit, k_mem_jump,
+// k_mem_chain with no output cap); k_bgzf_points, one thread per member, writes its rows and trailer CRC, and k_crc_join the check.
+struct BgzfSum {
+    uint64_t first, end; // where the run starts (it must start at 0) and ends
+    uint32_t count, more; // members of the run; more: the two bytes behind it are 1f 8b (a member that is not BGZF)
+    uint32_t check, pad;
+};
+
+__global__ void __launch_bounds__(256) k_bgzf_points(const uint8_t *__restrict__ src, uint64_t n, const uint64_t *moff, const uint32_t *mlen,
+                                                     const uint64_t *mout, const MemCtl *ctl, BgzfSum *sum, IdxMember *rm, IdxPoint *rp,
+                                                     uint32_t *crc)
+{
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x, count = ctl->count;
+    if (t >= count) return;
+    zbi_bgzf_member(src + moff[t], moff[t], mlen[t], mout[t], t, rm + t, rp + t, crc + t);
+    if (t == 0) { sum->first = moff[0]; sum->count = count; }
+    if (t == count - 1) {
+        const uint64_t e = moff[t] + mlen[t];
+        sum->end = e;
+        sum->more = n - e >= 2 && src[e] == 0x1f && src[e + 1] == 0x8b;
+    }
+}
+
+// Launches (device source): 7; host syncs: 2 (the candidate count, then everything in one copy).  A host source is walked on the host
+// with the same rules (zbi_bgzf_walk) and nothing is uploaded.
+int Engine::index_bgzf(const void *src, size_t n, bool src_dev, zb_inflate_result *res, zb_index *x)
+{
+    int rc;
+    void *p;
+    memset(res, 0, sizeof *res);
+    launches = 0;
+    std::vector<IdxMember> M;
+    std::vector<IdxPoint> P;
+    std::vector<uint32_t> crc;
+    uint64_t in = 0, bad = 0;
+    uint32_t check = 0;
+    int walk = 0;
+    if (!src_dev) {
+        walk = zbi_bgzf_walk(static_cast<const uint8_t *>(src), n, &in, &bad, [&](uint32_t m, uint64_t at, uint32_t len) {
+            IdxMember mb;
+            IdxPoint pt;
+            uint32_t c;
+            zbi_bgzf_member(static_cast<const uint8_t *>(src) + at, at, len, M.empty() ? 0 : M.back().out_end, m, &mb, &pt, &c);
+            M.push_back(mb);
+            P.push_back(pt);
+            check = (uint32_t)crc32_combine64(check, c, (z_off64_t)(mb.out_end - mb.out_start));
+        });
+    } else {
+        CKI(cudaSetDevice(device));
+        CKI(cudaEventRecord(ev0, st));
+        const uint8_t *d_src = static_cast<const uint8_t *>(src);
+        const uint64_t ntiles = (n + kMemTile - 1) / kMemTile;
+        if (ntiles > 0xffffffffull) { snprintf(g_err, sizeof g_err, "index_bgzf: input of %zu bytes is too long", n); return ZB_E_PARAM; }
+        if ((rc = reserve(S_MEMT, sizeof(MemCtl) + 64 + 8 * ntiles, &p)) != ZB_OK) return rc;
+        MemCtl *d_ctl = static_cast<MemCtl *>(p), h_ctl;
+        uint32_t *d_tcnt = reinterpret_cast<uint32_t *>(static_cast<uint8_t *>(p) + ((sizeof(MemCtl) + 63) & ~(size_t)63));
+        uint32_t *d_tbase = d_tcnt + ntiles;
+        uint32_t nc = 0;
+        if (ntiles) {
+            k_mem_count<<<(unsigned)ntiles, 256, 0, st>>>(d_src, n, d_tcnt);
+            k_mem_scan<<<1, 1024, 0, st>>>(d_tcnt, (uint32_t)ntiles, d_tbase, d_ctl);
+            launches += 2;
+            CKI(cudaMemcpyAsync(&h_ctl, d_ctl, sizeof h_ctl, cudaMemcpyDeviceToHost, st));
+            CKI(cudaStreamSynchronize(st));
+            nc = h_ctl.ncand;
+        }
+        if (nc > kMemMaxCand) {
+            snprintf(g_err, sizeof g_err, "index_bgzf: %u BGZF header candidates in a device source (at most %u); index it from a host source",
+                     nc, kMemMaxCand);
+            return ZB_E_PARAM;
+        }
+        if (nc == 0) walk = ZBI_BGZF_NOT; // bad = 0
+        else {
+            const uint32_t levels = 32 - __builtin_clz(nc);
+            const size_t n1 = (size_t)nc + 1;
+            const size_t rows = a64(sizeof(BgzfSum)) + (sizeof(IdxMember) + sizeof(IdxPoint)) * (size_t)nc; // copied back whole
+            const size_t bytes = n1 * (8 + 4 + 4 * levels + 8 + 4 + 4 + 8 + 4) + rows + 16 * 64;
+            if ((rc = reserve(S_MEMC, bytes, &p)) != ZB_OK) return rc;
+            uint8_t *q = static_cast<uint8_t *>(p);
+            auto take = [&](size_t b) { uint8_t *r = q; q += a64(b); return r; };
+            uint64_t *d_off = reinterpret_cast<uint64_t *>(take(8 * n1));
+            uint32_t *d_len = reinterpret_cast<uint32_t *>(take(4 * n1));
+            uint32_t *d_jmp = reinterpret_cast<uint32_t *>(take(4 * n1 * levels));
+            uint64_t *d_moff = reinterpret_cast<uint64_t *>(take(8 * n1));
+            uint32_t *d_mlen = reinterpret_cast<uint32_t *>(take(4 * n1));
+            uint32_t *d_misz = reinterpret_cast<uint32_t *>(take(4 * n1));
+            uint64_t *d_mout = reinterpret_cast<uint64_t *>(take(8 * n1));
+            uint32_t *d_mcrc = reinterpret_cast<uint32_t *>(take(4 * n1));
+            uint8_t *d_rows = take(rows);
+            BgzfSum *d_sum = reinterpret_cast<BgzfSum *>(d_rows);
+            IdxMember *d_rm = reinterpret_cast<IdxMember *>(d_rows + a64(sizeof(BgzfSum)));
+            IdxPoint *d_rp = reinterpret_cast<IdxPoint *>(d_rm + nc);
+            k_mem_emit<<<(unsigned)ntiles, 256, 0, st>>>(d_src, n, d_tbase, d_off, d_len);
+            k_mem_jump<<<1, 1024, 0, st>>>(d_off, d_len, nc, levels, d_jmp);
+            k_mem_chain<<<1, 1024, 0, st>>>(d_src, d_off, d_len, d_jmp, nc, levels, 0, ~0ull, d_moff, d_mlen, d_misz, d_mout, d_ctl);
+            k_bgzf_points<<<(nc + 255) / 256, 256, 0, st>>>(d_src, n, d_moff, d_mlen, d_mout, d_ctl, d_sum, d_rm, d_rp, d_mcrc);
+            CKI(launch_crc32_join(d_mcrc, d_misz, &d_ctl->count, &d_sum->check, st));
+            launches += 5;
+            std::vector<uint8_t> h(rows);
+            CKI(cudaMemcpyAsync(h.data(), d_rows, rows, cudaMemcpyDeviceToHost, st));
+            CKI(cudaStreamSynchronize(st));
+            CKI(cudaGetLastError());
+            BgzfSum sum;
+            memcpy(&sum, h.data(), sizeof sum);
+            const IdxMember *hm = reinterpret_cast<const IdxMember *>(h.data() + a64(sizeof(BgzfSum)));
+            const IdxPoint *hp = reinterpret_cast<const IdxPoint *>(hm + nc);
+            if (sum.first != 0) walk = ZBI_BGZF_NOT; // bad = 0
+            for (uint32_t m = 0; !walk && m < sum.count; m++)
+                if (hp[m].btype == 3) { walk = ZBI_BGZF_BTYPE; bad = hm[m].in_start; }
+            if (!walk && sum.more) { walk = ZBI_BGZF_NOT; bad = sum.end; }
+            if (!walk) {
+                M.assign(hm, hm + sum.count);
+                P.assign(hp, hp + sum.count);
+                in = sum.end;
+                check = sum.check;
+            }
+        }
+        CKI(cudaEventRecord(ev1, st));
+        CKI(cudaStreamSynchronize(st));
+        CKI(cudaEventElapsedTime(&res->gpu_ms, ev0, ev1));
+    }
+    res->gpu_launches = launches;
+    if (walk) {
+        if (walk == ZBI_BGZF_BTYPE) {
+            snprintf(res->msg, sizeof res->msg, "invalid block type in the BGZF member at %llu", (unsigned long long)bad);
+            snprintf(g_err, sizeof g_err, "index_bgzf: %s", res->msg);
+        } else {
+            snprintf(res->msg, sizeof res->msg, "no BGZF member at %llu: use zb_index_build", (unsigned long long)bad);
+            snprintf(g_err, sizeof g_err, "index_bgzf: no BGZF member that ends within the input at offset %llu (another gzip member, "
+                     "or a truncated one); zb_index_build indexes any gzip file", (unsigned long long)bad);
+        }
+        res->status = ZB_E_DATA;
+        return ZB_E_DATA;
+    }
+    const uint64_t total = M.back().out_end;
+    res->in_bytes = in;
+    res->out_bytes = total;
+    res->check = check;
+    res->status = ZB_OK;
+    return index_fill(*x, std::move(M), std::move(P), IdxHeader{kIdxMagic, kIdxVersion, 0, total, in, check, 31, 0, 0, 0}, nullptr, 0);
+}
+
 // zb_index_extract: see zb_engine.h.  One launch (k_index_extract over all pieces of all ranges) and one host sync.
 int Engine::index_extract(const zb_index *x, const void *src, size_t src_len, bool src_dev, const uint64_t *offsets, size_t n_ranges,
                           void *dst, const uint64_t *dst_off, bool dst_dev, zb_inflate_result *items)
@@ -2518,10 +2665,11 @@ int Engine::index_extract(const zb_index *x, const void *src, size_t src_len, bo
         const IdxPoint &pt = P[h.pi];
         const size_t u = std::lower_bound(used.begin(), used.end(), h.pi) - used.begin();
         const bool resume = pt.bit != pt.hdr_bit;
+        const bool to_end = x->h.span == 0 && h.b == M[pt.member].out_end; // a member index: check the member's ISIZE
         h_pc[k] = IdxPiece{in_ptr(h.sp.body_lo), resume ? in_ptr(h.sp.hdr_lo) : nullptr, d_win + wat[u],
                            d_dst + (dst_off[h.range] - dst_off[0]) + (h.a - offsets[h.range]), h.sp.body_hi - h.sp.body_lo,
                            h.sp.hdr_hi - h.sp.hdr_lo, pt.bit - 8 * h.sp.body_lo, pt.hdr_bit - 8 * h.sp.hdr_lo, h.a - pt.out_off, h.b - h.a,
-                           pt.btype, resume ? 1u : 0u, pt.window_len, 0};
+                           pt.btype, resume ? 1u : 0u, pt.window_len, to_end ? 1u : 0u};
     }
     CKI(cudaEventRecord(ev0, st));
     if (!dst_dev) CKI(cudaMemsetAsync(d_dst, 0, out_total, st)); // the slots go back whole: behind a range's bytes there are zeros
@@ -2543,8 +2691,10 @@ int Engine::index_extract(const zb_index *x, const void *src, size_t src_len, bo
         zb_inflate_result &r = items[hp[k].range];
         const InfState &s = hs[k];
         if (r.status != ZB_OK) continue;
-        // the piece's output must reach its end: a decode that stopped short (the final block ended) met damaged input
-        const uint32_t e = s.err != IE_OK ? s.err : s.out_bytes < h_pc[k].skip + h_pc[k].want ? (uint32_t)IE_TRUNCATED : (uint32_t)IE_OK;
+        // the piece's output must reach its end: a decode that stopped short (the final block ended) met damaged input, or, for a
+        // piece that runs to its member's end in a member index, a member whose ISIZE is larger than its output
+        const uint32_t shortfall = h_pc[k].to_end ? (uint32_t)IE_LENGTH_CHECK : (uint32_t)IE_TRUNCATED;
+        const uint32_t e = s.err != IE_OK ? s.err : s.out_bytes < h_pc[k].skip + h_pc[k].want ? shortfall : (uint32_t)IE_OK;
         if (e != IE_OK) { r.status = ZB_E_DATA; snprintf(r.msg, sizeof r.msg, "%s", inf_msg(e)); }
     }
     int status = ZB_OK;
