@@ -139,6 +139,32 @@ ZB_API int zb_deflate_batch_dict(zb_engine *e, const void *dict, size_t dict_len
                                  size_t n_items, int src_on_device, void *dst, size_t dst_cap, int dst_on_device, int level, int strategy,
                                  int window_bits, uint32_t flags, uint64_t *dst_off, uint32_t *checks, zb_deflate_result *res);
 
+/* zb_deflate_batch_params: a batch whose items each carry their own deflateInit2 parameters (DESIGN.md §2o).  params holds 1 entry,
+ * used for every item, or n_items entries, one per item; any other n_params is ZB_E_PARAM.  An entry is accepted exactly when
+ * deflateInit2 accepts it: level -1..9, strategy 0..4 (Z_DEFAULT_STRATEGY, Z_FILTERED, Z_HUFFMAN_ONLY, Z_RLE, Z_FIXED), window_bits
+ * 8..15 (zlib; 8 is 9 with CINFO 1), -9..-15 (raw) or 25..31 (gzip), mem_level 1..9.  Item i's stream is byte for byte what
+ * zb_deflate_ex(item_i, level, strategy, window_bits, ZB_FLAG_MEMLEVEL(mem_level)) returns for it alone, with exact_parity = 1:
+ * the reference's deflateInit2(level, 8, window_bits, mem_level, strategy) + deflate(Z_FINISH).  The streams are packed back to
+ * back in input order; dst_off, checks (adler32 zlib, crc32 gzip, 0 raw) and res are filled as by zb_deflate_batch, whose limits
+ * apply (65536 bytes per item, 65535 items, 2^31 bytes in all; ZB_E_BUF with res->out_bytes the size needed; zb_deflate_batch_bound
+ * is always enough).  No flags and no dictionary.
+ * Launches: 1 staging, 1 for the adler32 of the zlib items and 1 for the crc32 of the gzip items when such items are present, 2 for
+ * the links of the levels 3..8 and 2 for those of level 9 when present, the parsers of the classes present (1 each for levels 1, 2,
+ * 3..6 and Z_HUFFMAN_ONLY, 2 each for levels 7..9 and Z_RLE), 3 for the blocks unless every item is stored (level 0), and 3 for
+ * the sizes, offsets and framing: they depend on which classes and framings occur, never on the number or lengths of the items.
+ * Device memory: besides the buffers of zb_deflate_batch, each item gets len / (2^(mem_level+6) - 1) + 1 block slots of about
+ * 1.3 KB (none at level 0), so 2^31 bytes at memLevel 1 need about 22 GB of them (1.3 GB at memLevel 8).  When the device cannot
+ * provide them the call returns ZB_E_MEM with a zb_last_error() text before it launches anything; dst is left untouched. */
+typedef struct zb_batch_params {
+    int32_t level;       /* -1..9 (-1 = 6) */
+    int32_t strategy;    /* Z_DEFAULT_STRATEGY 0, Z_FILTERED 1, Z_HUFFMAN_ONLY 2, Z_RLE 3, Z_FIXED 4 */
+    int32_t window_bits; /* 8..15 zlib, -9..-15 raw, 25..31 gzip, as deflateInit2 */
+    int32_t mem_level;   /* 1..9 */
+} zb_batch_params;
+ZB_API int zb_deflate_batch_params(zb_engine *e, const void *src, const uint64_t *src_off, size_t n_items, int src_on_device,
+                                   const zb_batch_params *params, size_t n_params, void *dst, size_t dst_cap, int dst_on_device,
+                                   uint64_t *dst_off, uint32_t *checks, zb_deflate_result *res);
+
 /* zb_deflate_flushed: one stream with a full flush at every segment boundary (DESIGN.md §2m).  The input src[seg_off[0],
  * seg_off[n_segs]) is cut into segments [seg_off[k], seg_off[k+1]) (seg_off: a host array of n_segs + 1 offsets; src a host or, with
  * src_on_device, a device pointer).  dst receives byte for byte what the reference writes for

@@ -84,6 +84,12 @@ class IndexPoint(ctypes.Structure):
                 ("btype", ctypes.c_uint32), ("window_len", ctypes.c_uint32), ("window", ctypes.c_void_p)]
 
 
+class BatchParams(ctypes.Structure):
+    """deflateInit2 parameters of one item of Engine.deflate_batch_params (zb_batch_params)."""
+    _fields_ = [("level", ctypes.c_int32), ("strategy", ctypes.c_int32), ("window_bits", ctypes.c_int32),
+                ("mem_level", ctypes.c_int32)]
+
+
 class ZlibError(Exception):
     def __init__(self, code, msg=""):
         super().__init__("zlib error %d %s" % (code, msg))
@@ -170,6 +176,10 @@ def lib():
             L.zb_deflate_flushed_bound.argtypes, L.zb_deflate_flushed_bound.restype = [u64p, sz], sz
             L.zb_inflate_flushed.argtypes = [vp, vp, sz, ci, u64p, sz, ctypes.POINTER(u32), sz, vp, u64p, ci, ci,
                                              ctypes.POINTER(InflateResult)]
+        if hasattr(L, "zb_deflate_batch_params"):
+            u64p = ctypes.POINTER(u64)
+            L.zb_deflate_batch_params.argtypes = [vp, vp, u64p, sz, ci, ctypes.POINTER(BatchParams), sz, vp, sz, ci, u64p,
+                                                  ctypes.POINTER(u32), ctypes.POINTER(DeflateResult)]
         if hasattr(L, "zb_deflate_batch_dict"):
             L.zb_deflate_batch_dict.argtypes = [vp, vp, sz] + L.zb_deflate_batch.argtypes[1:]
             L.zb_inflate_batch_dict.argtypes = [vp, vp, sz] + L.zb_inflate_batch.argtypes[1:]
@@ -615,6 +625,42 @@ class Engine:
         else:
             dptr, dlen, dkeep = _dictionary(dictionary, src_on_device)
             rc = lib().zb_deflate_batch_dict(self.h, dptr, dlen, *args)
+        if rc != 0:
+            e = ZlibError(rc, lib().zb_last_error().decode())
+            e.needed = res.out_bytes
+            raise e
+        offs = list(dst_off)
+        raw = own.raw if own is not None else None
+        outs = [raw[offs[i]:offs[i + 1]] for i in range(n)] if own is not None else None
+        return outs, offs, list(checks)[:n], res
+
+    def deflate_batch_params(self, items, params, src_on_device=False, src_off=None, dst=None, dst_cap=0, dst_on_device=False):
+        """Deflate every item as its own stream with its own deflateInit2 parameters in one call (zb_deflate_batch_params).
+        `params` is one (level, strategy, window_bits, mem_level) tuple for every item, or a list of them, one per item.  Item
+        i's stream is byte for byte what Engine.deflate gives for it alone with its parameters.  Items, `dst` and the result are
+        as in deflate_batch: (list of bytes or None, offsets (n + 1), checks, DeflateResult).  Raises ZlibError (.needed: the
+        size a too small dst_cap would have to be)."""
+        res = DeflateResult()
+        keep = None
+        if src_on_device:
+            off = (ctypes.c_uint64 * len(src_off))(*src_off)
+            src = items
+        else:
+            keep, off = _gather(items)
+            src = ctypes.addressof(keep)
+        n = len(off) - 1
+        plist = [tuple(params)] if params and not isinstance(params[0], (tuple, list)) else [tuple(p) for p in params]
+        par = (BatchParams * max(len(plist), 1))(*[BatchParams(*p) for p in plist])
+        own = None
+        if dst is None:
+            dst_cap = lib().zb_deflate_batch_bound(off, n) + 64
+            own = ctypes.create_string_buffer(dst_cap)
+            dst = ctypes.addressof(own)
+            dst_on_device = False
+        dst_off = (ctypes.c_uint64 * (n + 1))()
+        checks = (ctypes.c_uint32 * max(n, 1))()
+        rc = lib().zb_deflate_batch_params(self.h, src, off, n, int(src_on_device), par, len(plist), dst, dst_cap, int(dst_on_device),
+                                           dst_off, checks, ctypes.byref(res))
         if rc != 0:
             e = ZlibError(rc, lib().zb_last_error().decode())
             e.needed = res.out_bytes

@@ -65,16 +65,19 @@ __global__ void __launch_bounds__(32) k_bgzf_medium(JobBufs jb, BgzfJob bj)
 {
     __shared__ uint32_t ins[kMemberMax / 32];
     if (threadIdx.x != 0) return;
-    const uint32_t m = blockIdx.x, base = (uint32_t)bj.moff[m], p0 = bj.pstart, len = p0 + bj.mlen[m], bs = jb.block_syms;
-    const BgzfAcc a{jb.in + base, jb.L + base, len, 4u};
+    const uint32_t m = blockIdx.x, base = (uint32_t)bj.moff[m], p0 = bj.pstart, len = p0 + bj.mlen[m];
+    const uint32_t bs = bj.mp ? bj.mp[m].bs : jb.block_syms, w = bj.mp ? bj.mp[m].wsize : kWSize;
+    const LevelParams lp = bj.mp ? level_params(bj.mp[m].level) : jb.lp;
+    const BgzfAcc a{jb.in + base, jb.L + base, len, 4u, w, w - kMinLookahead};
     Sym *syms = jb.syms + base;
-    uint32_t *bb = jb.block_base + m * kBgzfMaxBlocks;
+    uint32_t *bb = jb.block_base + bj.slot0(m);
     uint32_t k = 0, left = bs, blk = 0;
     auto emit = [&](const Sym &s, uint32_t B) {
         syms[k++] = s;
         if (--left == 0) { bb[blk++] = B; left = bs; } // the window base when this symbol fills the block (k_block_hist's sym_base)
     };
-    const uint32_t fb = serial_medium(a, len, p0, ins, kMemberMax / 32, jb.lp, emit);
+    const uint32_t fb = w == kWSize ? serial_medium(a, len, p0, ins, kMemberMax / 32, lp, emit)
+                                    : serial_medium(a, len, p0, ins, kMemberMax / 32, lp, emit, DynWin{w});
     JobInfo &mi = bj.minfo[m];
     mi.n_syms = k;
     mi.final_base = fb;
@@ -91,10 +94,46 @@ __global__ void __launch_bounds__(256) k_bgzf_slow_steps(JobBufs jb, BgzfJob bj)
     if (i >= bj.mlen[m]) return;
     const uint32_t y = bj.pstart + i, len = bj.pstart + bj.mlen[m];
     const uint32_t base = (uint32_t)bj.moff[m], x = base + y;
-    const BgzfAcc a{jb.in + base, jb.L + base, len, jb.sp.slow ? 3u : 4u};
-    const SlowStep s = slow_step(a, y, len, jb.sp);
+    SlowParams sp = jb.sp;
+    if (bj.mp) { sp = slow_params(bj.mp[m].level); sp.filtered = bj.mp[m].filtered; sp.wsize = bj.mp[m].wsize; }
+    const BgzfAcc a{jb.in + base, jb.L + base, len, sp.slow ? 3u : 4u, sp.wsize, sp.slow ? sp.wsize - 1u : sp.maxdist()};
+    const SlowStep s = slow_step(a, y, len, sp);
     jb.M[x] = pack_step(s);
     jb.nxt[x] = s.next;
+}
+
+// Z_RLE members (zb_deflate_batch_params): the step of k_rle at every member position, with the member's window, in the format of
+// k_bgzf_slow_steps; k_bgzf_slow_walk walks them.  Reads stay within the member.
+__global__ void __launch_bounds__(256) k_bgzf_rle_steps(JobBufs jb, BgzfJob bj)
+{
+    const uint32_t m = blockIdx.x / (kMemberMax / 256), y = (blockIdx.x % (kMemberMax / 256)) * 256 + threadIdx.x;
+    if (m >= bj.nm) return;
+    const uint32_t len = bj.mlen[m];
+    if (y >= len) return;
+    const uint32_t x = (uint32_t)bj.moff[m] + y;
+    const SlowStep s = rle_step(jb.in + bj.moff[m], y, len, bj.mp[m].wsize, len);
+    jb.M[x] = pack_step(s);
+    jb.nxt[x] = s.next;
+}
+
+// Z_HUFFMAN_ONLY members (zb_deflate_batch_params): every byte a literal, as k_literal_syms writes them, one thread per member
+// position.  A block ends every `bs` symbols; the window base of a block's flush is k_block_hist's rule (k_bgzf_hist), the last
+// block's is deflate_huff's (k_literal_syms).
+__global__ void __launch_bounds__(256) k_bgzf_literals(JobBufs jb, BgzfJob bj)
+{
+    const uint32_t m = blockIdx.x / (kMemberMax / 256), y = (blockIdx.x % (kMemberMax / 256)) * 256 + threadIdx.x;
+    if (m >= bj.nm) return;
+    const uint32_t len = bj.mlen[m], base = (uint32_t)bj.moff[m];
+    if (y == 0) {
+        const uint32_t w = bj.mp[m].wsize, q = len ? len - 1 : 0;
+        uint32_t B = q < 2 * w ? 0 : w * (1 + (q - 2 * w) / w);
+        if (len - B >= 2 * w - kMinLookahead) B += w;
+        JobInfo &mi = bj.minfo[m];
+        mi.n_syms = len;
+        mi.n_blocks = len / bj.mp[m].bs + 1;
+        mi.final_base = B;
+    }
+    if (y < len) jb.syms[base + y] = Sym{0, jb.in[base + y], y};
 }
 
 // ... and one thread per member walks the steps from the parse start and writes the symbols (k_emit_slow + k_tail_slow of one
@@ -103,7 +142,9 @@ __global__ void __launch_bounds__(32) k_bgzf_slow_walk(JobBufs jb, BgzfJob bj)
 {
     const uint32_t m = blockIdx.x * 32 + threadIdx.x;
     if (m >= bj.nm) return;
-    const uint32_t base = (uint32_t)bj.moff[m], len = bj.pstart + bj.mlen[m], bs = jb.block_syms;
+    const uint32_t base = (uint32_t)bj.moff[m], len = bj.pstart + bj.mlen[m];
+    const uint32_t bs = bj.mp ? bj.mp[m].bs : jb.block_syms, w = bj.mp ? bj.mp[m].wsize : jb.wsize;
+    const bool lazy = bj.mp ? bj.mp[m].cls != kClassRle : jb.slow_mode == 1;
     const uint8_t *d = jb.in + base;
     const uint32_t *M = jb.M + base, *nxt = jb.nxt + base;
     Sym *syms = jb.syms + base;
@@ -118,10 +159,11 @@ __global__ void __launch_bounds__(32) k_bgzf_slow_walk(JobBufs jb, BgzfJob bj)
     }
     JobInfo &mi = bj.minfo[m];
     mi.n_syms = n;
-    mi.final_base = base_at(len, len, jb.wsize);
+    mi.final_base = base_at(len, len, w);
     uint32_t nb = n / bs + 1;
-    // k_tail_slow's rule: a pending last literal tallied into a just-filled symbol buffer makes that block the last one
-    if (n > 0 && n % bs == 0 && syms[n - 1].dist == 0 && syms[n - 1].pos + 1 == len) nb--;
+    // k_tail_slow's rule: a pending last literal tallied into a just-filled symbol buffer makes that block the last one (deflate_slow
+    // only: Z_RLE, whose steps this walk also follows, has no pending literal)
+    if (lazy && n > 0 && n % bs == 0 && syms[n - 1].dist == 0 && syms[n - 1].pos + 1 == len) nb--;
     mi.n_blocks = nb;
 }
 
@@ -134,15 +176,16 @@ __global__ void __launch_bounds__(256) k_bgzf_size(JobBufs jb, BgzfJob bj)
     if (m >= bj.nm) return;
     const uint32_t len = bj.mlen[m];
     const bool fin = !bj.flushed || m + 1 == bj.nm; // the member ends its stream: BFINAL, no empty stored block behind it
-    bool stored = jb.level == 0;
+    const uint32_t wrap = bj.wrap_of(m);
+    bool stored = bj.mp ? bj.mp[m].cls == kClassStored : jb.level == 0;
     uint64_t payload = 0;
     uint32_t nb = 0;
     if (!stored) {
         nb = bj.minfo[m].n_blocks;
-        if (nb == 0 || nb > kBgzfMaxBlocks) { atomicOr(&bj.ctl->error, 1u); return; }
+        if (nb == 0 || nb > bj.nslots(m)) { atomicOr(&bj.ctl->error, 1u); return; }
         uint64_t bit = 0;
         for (uint32_t k = 0; k < nb; k++) {
-            BlockDesc &bd = jb.blocks[m * kBgzfMaxBlocks + k];
+            BlockDesc &bd = jb.blocks[bj.slot0(m) + k];
             bd.bit_base = bit;
             bit = bd.type == 0 ? ((bit + 3 + 7) & ~7ull) + 32 + 8ull * (uint16_t)bd.in_len : bit + bd.hdr_bits + bd.body_bits;
         }
@@ -154,19 +197,19 @@ __global__ void __launch_bounds__(256) k_bgzf_size(JobBufs jb, BgzfJob bj)
     atomicAdd(&bj.ctl->n_blocks, nb);
     bj.mstored[m] = stored;
     bj.mbytes[m] = bj.flushed ? flush_header_len(bj.wrap, m) + (uint32_t)payload + flush_trailer_len(bj.wrap, m, bj.nm)
-                              : member_header_len(bj.wrap, bj.fdict) + (uint32_t)payload + member_trailer_len(bj.wrap);
+                              : member_header_len(wrap, bj.fdict) + (uint32_t)payload + member_trailer_len(wrap);
 }
 
-// One CTA: the members' offsets in the output (exclusive scan of their lengths), the blocks' absolute bit positions, the output
-// length.
-__global__ void __launch_bounds__(1024) k_bgzf_scan(JobBufs jb, BgzfJob bj)
+// One CTA: the members' offsets in the output (exclusive scan of their lengths, in input order), the blocks' absolute bit
+// positions, the output length.
+__global__ void __launch_bounds__(1024, 1) k_bgzf_scan(JobBufs jb, BgzfJob bj)
 {
     __shared__ uint64_t part[1024];
     const uint32_t tid = threadIdx.x, n = bj.nm, per = (n + 1023) / 1024;
     const uint32_t beg = min(n, tid * per), end = min(n, beg + per);
     if (bj.ctl->error) return;
     uint64_t s = 0;
-    for (uint32_t i = beg; i < end; i++) s += bj.mbytes[i];
+    for (uint32_t i = beg; i < end; i++) s += bj.mbytes[bj.morder ? bj.morder[i] : i];
     part[tid] = s;
     __syncthreads();
     for (uint32_t h = 1; h < 1024; h <<= 1) {
@@ -176,17 +219,21 @@ __global__ void __launch_bounds__(1024) k_bgzf_scan(JobBufs jb, BgzfJob bj)
         __syncthreads();
     }
     uint64_t off = part[tid] - s;
-    for (uint32_t i = beg; i < end; i++) {
+    for (uint32_t j = beg; j < end; j++) {
+        const uint32_t i = bj.morder ? bj.morder[j] : j;
         bj.mout[i] = off;
-        const uint32_t hl = bj.flushed ? flush_header_len(bj.wrap, i) : member_header_len(bj.wrap, bj.fdict);
+        const uint32_t hl = bj.flushed ? flush_header_len(bj.wrap, i) : member_header_len(bj.wrap_of(i), bj.fdict);
         if (!bj.mstored[i]) {
             const uint32_t nb = bj.minfo[i].n_blocks;
-            for (uint32_t k = 0; k < nb; k++) jb.blocks[i * kBgzfMaxBlocks + k].bit_base += 8ull * (off + hl);
+            for (uint32_t k = 0; k < nb; k++) jb.blocks[bj.slot0(i) + k].bit_base += 8ull * (off + hl);
         }
         off += bj.mbytes[i];
     }
     if (tid == 1023) bj.ctl->out_bytes = part[1023] + (bj.wrap == kWrapBgzf ? kBgzfEofLen : 0);
-    if (tid == 0) bj.ctl->data_type = (n && !bj.mstored[0] && jb.blocks[0].sym_count) ? jb.blocks[0].data_type : 2u;
+    if (tid == 0) {
+        const uint32_t f = n ? (bj.morder ? bj.morder[0] : 0u) : 0u; // the first item's first block
+        bj.ctl->data_type = (n && !bj.mstored[f] && jb.blocks[bj.slot0(f)].sym_count) ? jb.blocks[bj.slot0(f)].data_type : 2u;
+    }
 }
 
 // One CTA per member: header (BGZF's with BSIZE, or the item's zlib / gzip header, with FDICT and DICTID behind a dictionary), trailer, and the stored blocks of a member
@@ -219,13 +266,16 @@ __global__ void __launch_bounds__(256) k_bgzf_frame(JobBufs jb, BgzfJob bj)
         }
         return;
     }
-    const uint32_t hl = member_header_len(bj.wrap, bj.fdict);
+    const uint32_t wrap = bj.wrap_of(m), hl = member_header_len(wrap, bj.fdict);
     if (tid == 0) {
-        if (bj.wrap == kWrapBgzf) bgzf_header(o, bytes);
-        else stream_header(o, bj.wrap, zlib_level_flags(jb.level, false), 7, gzip_xfl((int)jb.level, 0), bj.fdict != 0,
-                           bj.fdict ? *bj.dictid : 0u);
-        const uint32_t tw = bj.wrap == kWrapBgzf ? 2u : bj.wrap; // BGZF's trailer is gzip's
-        stream_trailer(o + bytes - member_trailer_len(bj.wrap), tw, bj.mcheck[m], len);
+        if (wrap == kWrapBgzf) bgzf_header(o, bytes);
+        else if (bj.mp) { // the item's own framing (zb_bgzf.h)
+            const MemberParams &mp = bj.mp[m];
+            stream_header(o, wrap, mp.lflags, mp.cinfo, mp.xfl);
+        } else stream_header(o, wrap, zlib_level_flags(jb.level, false), 7, gzip_xfl((int)jb.level, 0), bj.fdict != 0,
+                             bj.fdict ? *bj.dictid : 0u);
+        const uint32_t tw = wrap == kWrapBgzf ? 2u : wrap; // BGZF's trailer is gzip's
+        stream_trailer(o + bytes - member_trailer_len(wrap), tw, wrap == 2 && bj.mcrc ? bj.mcrc[m] : bj.mcheck[m], len);
     }
     if (stored) {
         const uint32_t nb = (uint32_t)stored_blocks(len);
@@ -248,7 +298,7 @@ __global__ void __launch_bounds__(256) k_flush_blocks(JobBufs jb, BgzfJob bj)
     mi.n_blocks = n / bs;
     const uint32_t base = (uint32_t)bj.moff[m];
     mi.final_base = jb.slow_mode ? base_at(jb.syms[base + n - 1].pos + 1, bj.mlen[m], jb.wsize) // as k_bgzf_hist
-                                 : jb.block_base[m * kBgzfMaxBlocks + n / bs - 1];
+                                 : jb.block_base[bj.slot0(m) + n / bs - 1];
 }
 
 } // namespace zb

@@ -116,16 +116,23 @@ ZB_HD uint64_t stream_bound(uint64_t n) { return n + ((n + 7) >> 3) + ((n + 63) 
 // A link that reaches farther back than y crosses the member's start: "no link".  `need` is the span of the hash (4 bytes, 3 for
 // the rolling hash of level 9): a position whose hash reaches past the end has no link.  Every position counts as inserted:
 // serial_medium keeps its own bitmap, and deflate_slow inserts every position.
+// With a window w below 32 KiB (zb_deflate_batch_params) the same holds with w in place of 32 KiB: behind the member the window
+// buffer holds zeros up to 2w, then the bytes one window earlier (GAccW's rule), and a link longer than the window's link range
+// `cap` (w - MIN_LOOKAHEAD, or w - 1 for the rolling hash) is "no link".  The link kernels cut links at the 32 KiB range; a link is
+// the nearest earlier position with the same hash, so when that one lies beyond `cap` no position within `cap` has the hash either,
+// and cutting it here gives exactly the links of a w-byte window.
 struct BgzfAcc {
     const uint8_t *data; // in + moff[m]
     const uint16_t *L;   // links of the staged buffer, from the same offset
     uint32_t N;          // the member's length
     uint32_t need;
+    uint32_t w = kWSize;     // the member's window
+    uint32_t cap = 0xffffu;  // its link range (the 32 KiB links need no further cut)
     ZB_HD uint32_t byte(uint32_t y) const
     {
         while (y >= N) {
-            if (y < 2 * kWSize) return 0;
-            y -= kWSize;
+            if (y < 2 * w) return 0;
+            y -= w;
         }
         return data[y];
     }
@@ -133,10 +140,110 @@ struct BgzfAcc {
     {
         if (y + need > N) return 0;
         const uint32_t d = L[y];
-        return d <= y ? d : 0u;
+        return d <= y && d <= cap ? d : 0u;
     }
     ZB_HD bool inserted(uint32_t) const { return true; }
 };
+
+// ---------------------------------------------------------------------------------------------------------------------------------
+// Batches with parameters per item (zb_deflate_batch_params, DESIGN.md §2o).  Item i carries its own deflateInit2(level, 8,
+// window_bits, mem_level, strategy) and becomes the stream zb_deflate_ex writes for it alone with those parameters.  The rules of
+// Engine::deflate pick the item's parser class; the host stages the items class by class (a permutation maps staged members back to
+// input order), and every parser kernel runs once over its class's member range, reading the member's own record below.
+enum MemberClass : uint32_t {
+    kClassStored = 0, // level 0 (whatever the strategy: stored.rs ignores it)
+    kClassQuick,      // level 1: deflate_quick (Z_DEFAULT_STRATEGY, Z_FILTERED, Z_FIXED)
+    kClassFast,       // level 2: deflate_fast
+    kClassMedium,     // levels 3..6: deflate_medium (Z_FILTERED changes only the lazy levels)
+    kClassSlow,       // levels 7, 8: deflate_slow, standard hash
+    kClassSlow9,      // level 9: deflate_slow, rolling hash
+    kClassRle,        // Z_RLE at levels 1..9
+    kClassHuff,       // Z_HUFFMAN_ONLY at levels 1..9
+    kClasses
+};
+
+struct MemberParams {
+    uint8_t cls;      // MemberClass
+    uint8_t level;    // 1..9 (0 for stored members)
+    uint8_t wrap;     // 0 raw / 1 zlib / 2 gzip
+    uint8_t cinfo;    // effective windowBits - 8
+    uint8_t lflags;   // zlib FLEVEL
+    uint8_t xfl;      // gzip XFL
+    uint8_t filtered; // Z_FILTERED at levels 7..9
+    uint8_t fixed;    // Z_FIXED: static blocks only
+    uint32_t wsize;   // window of the parse
+    uint32_t bs;      // symbols per deflate block
+};
+
+// deflateInit2_'s acceptance (deflate.rs:285-312) and the member's record, or false.  windowBits 8 is 9 with CINFO 1.  The window of
+// the parse follows Engine::deflate: the levels 3..9 and Z_RLE keep the 32 KiB window while the item never leaves the smaller one
+// (len + MIN_LOOKAHEAD <= w: only CINFO differs), every other class parses with w itself.
+ZB_HD bool batch_member_params(int level, int strategy, int window_bits, int mem_level, uint32_t len, MemberParams *mp)
+{
+    if (level == -1) level = 6;
+    if (level < 0 || level > 9 || strategy < 0 || strategy > 4 || mem_level < 1 || mem_level > 9) return false;
+    uint32_t wrap;
+    int wb;
+    if (window_bits >= 8 && window_bits <= 15) { wrap = 1; wb = window_bits; }
+    else if (window_bits >= -15 && window_bits <= -9) { wrap = 0; wb = -window_bits; }
+    else if (window_bits >= 25 && window_bits <= 31) { wrap = 2; wb = window_bits - 16; }
+    else return false;
+    if (wb == 8) wb = 9;
+    const uint32_t w = 1u << wb;
+    const bool huff = strategy == 2 && level != 0, rle = strategy == 3 && level != 0;
+    uint32_t cls;
+    if (level == 0) cls = kClassStored;
+    else if (huff) cls = kClassHuff;
+    else if (rle) cls = kClassRle;
+    else if (level == 1) cls = kClassQuick;
+    else if (level == 2) cls = kClassFast;
+    else if (level <= 6) cls = kClassMedium;
+    else cls = level == 9 ? kClassSlow9 : kClassSlow;
+    const bool keep32 = (cls == kClassMedium || cls == kClassSlow || cls == kClassSlow9 || cls == kClassRle) &&
+                        (uint64_t)len + kMinLookahead <= w;
+    mp->cls = (uint8_t)cls;
+    mp->level = (uint8_t)level;
+    mp->wrap = (uint8_t)wrap;
+    mp->cinfo = (uint8_t)(wb - 8);
+    // FLEVEL follows the requested level; Z_RLE writes level 1's, Z_HUFFMAN_ONLY and Z_FIXED their own (Engine::deflate)
+    mp->lflags = (uint8_t)zlib_level_flags(rle ? 1u : (uint32_t)level, huff || strategy == 4);
+    mp->xfl = (uint8_t)gzip_xfl(level, strategy);
+    mp->filtered = strategy == 1 && level >= 7;
+    mp->fixed = strategy == 4;
+    mp->wsize = keep32 ? kWSize : w;
+    mp->bs = cls == kClassQuick ? kBlockSyms : (1u << (mem_level + 6)) - 1u; // deflate_quick's pieces; lit_bufsize - 1 otherwise
+    return true;
+}
+// Block slots of a member: as many deflate blocks as its parse can flush (at most one symbol per input byte), none when stored.
+ZB_HD uint32_t member_slots(const MemberParams &mp, uint32_t len) { return mp.cls == kClassStored ? 0u : len / mp.bs + 1; }
+
+// The staging of zb_deflate_batch_params, in two steps that tests/batchparammodel runs as the engine does.
+// 1. A stable counting sort of the items by class: class c becomes the staged members [cbeg[c], cbeg[c + 1]) (cbeg: kClasses + 1
+//    entries) and item i the staged member morder[i].
+ZB_HD void batch_class_order(const MemberParams *mp, uint32_t n, uint32_t *cbeg, uint32_t *morder)
+{
+    uint32_t next[kClasses];
+    for (uint32_t c = 0; c <= kClasses; c++) cbeg[c] = 0;
+    for (uint32_t i = 0; i < n; i++) cbeg[mp[i].cls + 1]++;
+    for (uint32_t c = 0; c < kClasses; c++) { cbeg[c + 1] += cbeg[c]; next[c] = cbeg[c]; }
+    for (uint32_t i = 0; i < n; i++) morder[i] = next[mp[i].cls]++;
+}
+// 2. Over the staged members (records smp, lengths slen): the staged offsets (batch_stage_next) and the block-slot table mslot
+//    (n + 1 prefix sums of member_slots).  Returns the staged span.  The slots cost 1280 bytes of histogram and a BlockDesc each:
+//    at most 2^31 / 127 + 65535 of them (2^31 bytes at memLevel 1), about 22 GB of device memory.
+ZB_HD uint64_t batch_params_layout(const MemberParams *smp, const uint32_t *slen, uint32_t n, uint64_t *moff, uint32_t *mslot)
+{
+    uint64_t span = 0;
+    uint32_t slots = 0;
+    for (uint32_t m = 0; m < n; m++) {
+        moff[m] = span;
+        span = batch_stage_next(span, slen[m]);
+        mslot[m] = slots;
+        slots += member_slots(smp[m], slen[m]);
+    }
+    mslot[n] = slots;
+    return span;
+}
 
 // ---------------------------------------------------------------------------------------------------------------------------------
 // Flushed streams (zb_deflate_flushed, DESIGN.md §2m): the input cut into segments, written as deflateInit2(level, 8, -15 / 15 /

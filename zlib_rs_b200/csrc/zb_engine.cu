@@ -67,6 +67,8 @@ __global__ void k_serial_low_members(JobBufs, BgzfJob);
 __global__ void k_bgzf_medium(JobBufs, BgzfJob);
 __global__ void k_bgzf_slow_steps(JobBufs, BgzfJob);
 __global__ void k_bgzf_slow_walk(JobBufs, BgzfJob);
+__global__ void k_bgzf_rle_steps(JobBufs, BgzfJob);
+__global__ void k_bgzf_literals(JobBufs, BgzfJob);
 __global__ void k_bgzf_hist(JobBufs, BgzfJob, uint32_t *);
 __global__ void k_bgzf_build(JobBufs, BgzfJob, const uint32_t *);
 __global__ void k_bgzf_size(JobBufs, BgzfJob);
@@ -693,8 +695,23 @@ int Engine::deflate(const void *src, size_t n_in, bool src_dev, void *dst, size_
 int Engine::members_reserve(JobBufs &jb, BgzfJob &bj, uint32_t nm, uint32_t S, size_t span, int level, size_t out_cap, uint32_t wrap,
                             uint32_t **d_freq)
 {
-    const uint32_t nmt = S / kLinkTile + 1, nslots = nm * kBgzfMaxBlocks;
-    const bool links = level >= 3, slow = level >= 7;
+    int rc;
+    if ((rc = members_alloc(jb, bj, nm, S, span, out_cap, wrap, nm * kBgzfMaxBlocks, level > 0, level >= 3, level >= 7, d_freq)) != ZB_OK)
+        return rc;
+    jb.level = (uint32_t)level;
+    jb.block_syms = kBlockSyms; // memLevel 8; deflate_quick's pieces have the same size
+    jb.serial_mode = level == 1 || level == 2 ? (uint32_t)level : 0u;
+    if (level >= 3 && level <= 6) jb.lp = level_params(level);
+    if (level >= 7) { jb.slow_mode = 1; jb.sp = slow_params(level); jb.sp.wsize = kWSize; }
+    return ZB_OK;
+}
+
+// ... the buffers alone: `nslots` block slots, symbols when the members are parsed, links and the steps of the lazy parsers when
+// they need them.  The tables of a batch with parameters per item (BgzfJob::mp ..) are left to the caller.
+int Engine::members_alloc(JobBufs &jb, BgzfJob &bj, uint32_t nm, uint32_t S, size_t span, size_t out_cap, uint32_t wrap, uint32_t nslots,
+                          bool parse, bool links, bool slow, uint32_t **d_freq)
+{
+    const uint32_t nmt = S / kLinkTile + 1;
     memset(&jb, 0, sizeof jb);
     int rc;
     void *p;
@@ -703,16 +720,11 @@ int Engine::members_reserve(JobBufs &jb, BgzfJob &bj, uint32_t nm, uint32_t S, s
     jb.field = static_cast<type>(p);
     RES(S_IN, span + kPad + 16, in, const uint8_t *)
     jb.N = S;
-    jb.level = (uint32_t)level;
     jb.wsize = kWSize;
-    jb.block_syms = kBlockSyms; // memLevel 8; deflate_quick's pieces have the same size
-    jb.serial_mode = level == 1 || level == 2 ? (uint32_t)level : 0u;
-    if (level >= 3 && level <= 6) jb.lp = level_params(level);
-    if (slow) { jb.slow_mode = 1; jb.sp = slow_params(level); jb.sp.wsize = kWSize; }
     RES(S_OUT, out_cap + 16, out, uint8_t *)
     jb.out_cap = out_cap;
     *d_freq = nullptr;
-    if (level > 0 && nm) {
+    if (parse && nm) {
         RES(S_SYMS, (span + 64) * sizeof(Sym), syms, Sym *)
         RES(S_BLOCKS, (size_t)nslots * sizeof(BlockDesc), blocks, BlockDesc *)
         RES(S_BBASE, (size_t)nslots * 4, block_base, uint32_t *)
@@ -742,6 +754,10 @@ int Engine::members_reserve(JobBufs &jb, BgzfJob &bj, uint32_t nm, uint32_t S, s
     bj.flushed = 0;
     bj.fcheck = nullptr;
     bj.isize = 0;
+    bj.mp = nullptr;
+    bj.mslot = nullptr;
+    bj.morder = nullptr;
+    bj.mcrc = nullptr;
     bj.moff = reinterpret_cast<uint64_t *>(t);
     bj.mout = reinterpret_cast<uint64_t *>(t + m8);
     bj.mlen = reinterpret_cast<uint32_t *>(t + 2 * m8);
@@ -756,7 +772,7 @@ int Engine::members_reserve(JobBufs &jb, BgzfJob &bj, uint32_t nm, uint32_t S, s
 // ... and its launches behind the staging: links, parse, blocks, sizes and offsets, encoding, framing.
 int Engine::members_launch(JobBufs &jb, BgzfJob &bj, int level, uint32_t *d_freq)
 {
-    const uint32_t nm = bj.nm, S = jb.N, nmt = S / kLinkTile + 1, nslots = nm * kBgzfMaxBlocks;
+    const uint32_t nm = bj.nm, S = jb.N, nmt = S / kLinkTile + 1;
     const bool links = level >= 3, slow = level >= 7;
     if (level > 0 && nm) {
         if (links) {
@@ -782,6 +798,15 @@ int Engine::members_launch(JobBufs &jb, BgzfJob &bj, int level, uint32_t *d_freq
             launches += 2;
         }
         if (bj.flushed && jb.serial_mode != 1) { k_flush_blocks<<<nm / 256 + 1, 256, 0, st>>>(jb, bj); launches++; } // zb_bgzf.cu
+    }
+    return members_blocks(jb, bj, level > 0 && nm, nm * kBgzfMaxBlocks, d_freq);
+}
+
+// ... from the parse on: the blocks of `nslots` block slots (when some member has any), sizes and offsets, encoding, framing.
+int Engine::members_blocks(JobBufs &jb, BgzfJob &bj, bool blocks, uint32_t nslots, uint32_t *d_freq)
+{
+    const uint32_t nm = bj.nm;
+    if (blocks) {
         k_bgzf_hist<<<nslots, 256, 0, st>>>(jb, bj, d_freq);
         k_bgzf_build<<<nslots, 32, 0, st>>>(jb, bj, d_freq);
         launches += 2;
@@ -789,7 +814,7 @@ int Engine::members_launch(JobBufs &jb, BgzfJob &bj, int level, uint32_t *d_freq
     k_bgzf_size<<<nm / 256 + 1, 256, 0, st>>>(jb, bj);
     k_bgzf_scan<<<1, 1024, 0, st>>>(jb, bj);
     launches += 2;
-    if (level > 0 && nm) {
+    if (blocks) {
         k_bgzf_encode<<<nslots, 1024, 0, st>>>(jb, bj);
         launches++;
     }
@@ -1027,6 +1052,231 @@ int Engine::deflate_batch(const void *dict, size_t dict_len, const void *src, co
     res->out_bytes = out_bytes;
     res->data_type = (int32_t)h_ctl->data_type;
     res->iterations = level > 0 ? 1 : 0;
+    res->n_symbols = h_ctl->n_syms;
+    res->n_blocks = h_ctl->n_blocks;
+    res->gpu_launches = launches;
+    res->gpu_ms = ms;
+    return ZB_OK;
+}
+
+// zb_deflate_batch_params (zb_bgzf.h, DESIGN.md §2o): item i is deflated alone with its own deflateInit2 parameters, byte for byte
+// what zb_deflate_ex gives for it.  The host stages the items class by class (MemberClass) and keeps the permutation; the link
+// passes run over the staged range of the classes that need them, every parser kernel once over its class's members, and the
+// block, size, scan, encode and frame kernels once over all members, reading each member's record.  The launches of a call depend
+// on the set of classes and framings present, never on the number or the lengths of the items.
+int Engine::deflate_batch_params(const void *src, const uint64_t *src_off, size_t n_items, bool src_dev, const zb_batch_params *params,
+                                 size_t n_params, void *dst, size_t dst_cap, bool dst_dev, uint64_t *dst_off, uint32_t *checks,
+                                 zb_deflate_result *res)
+{
+    if (!res || !dst_off || (n_items && (!src_off || !dst || !params))) {
+        snprintf(g_err, sizeof g_err, "deflate_batch_params: null argument");
+        return ZB_E_PARAM;
+    }
+    memset(res, 0, sizeof *res);
+    if (n_params != 1 && n_params != n_items) {
+        snprintf(g_err, sizeof g_err, "deflate_batch_params: %zu parameter sets for %zu items (1 or one per item)", n_params, n_items);
+        return ZB_E_PARAM;
+    }
+    if (n_items > kBatchMaxItems) { snprintf(g_err, sizeof g_err, "deflate_batch_params: %zu items (at most %llu)", n_items, (unsigned long long)kBatchMaxItems); return ZB_E_PARAM; }
+    const uint32_t nm = (uint32_t)n_items;
+    // pinned staging: up moff | mlen | soff | mp | mslot | morder | lz | lg, down the control block | mout | adler32 | crc32
+    const size_t t_up = (size_t)nm * (8 + 4 + 8 + sizeof(MemberParams) + 4 + 4 + 4 + 4) + 4 + 64;
+    const size_t t_down = sizeof(BgzfCtl) + (size_t)nm * 16 + 16;
+    int rc;
+    if ((rc = stage(t_up + t_down + 64)) != ZB_OK) return rc;
+    uint8_t *h = static_cast<uint8_t *>(h_stage);
+    uint64_t *h_moff = reinterpret_cast<uint64_t *>(h);
+    uint64_t *h_soff = h_moff + nm;
+    MemberParams *h_mp = reinterpret_cast<MemberParams *>(h_soff + nm);
+    uint32_t *h_mlen = reinterpret_cast<uint32_t *>(h_mp + nm);
+    uint32_t *h_morder = h_mlen + nm, *h_lz = h_morder + nm, *h_lg = h_lz + nm, *h_mslot = h_lg + nm; // mslot: nm + 1
+    BgzfCtl *h_ctl = reinterpret_cast<BgzfCtl *>(h + ((t_up + 15) & ~(size_t)15));
+    uint64_t *h_mout = reinterpret_cast<uint64_t *>(h_ctl + 1);
+    uint32_t *h_adler = reinterpret_cast<uint32_t *>(h_mout + nm), *h_crc = h_adler + nm;
+    // every item's record (deflateInit2_'s rules), then a stable counting sort by class
+    uint64_t total = 0, bound = 0;
+    for (uint32_t i = 0; i < nm; i++) {
+        if (src_off[i + 1] < src_off[i] || src_off[i + 1] - src_off[i] > kMemberMax) {
+            snprintf(g_err, sizeof g_err, "deflate_batch_params: item %u is not 0..%u bytes", i, kMemberMax);
+            return ZB_E_PARAM;
+        }
+        const uint32_t len = (uint32_t)(src_off[i + 1] - src_off[i]);
+        const zb_batch_params &q = params[n_params == 1 ? 0 : i];
+        MemberParams mp;
+        if (!batch_member_params(q.level, q.strategy, q.window_bits, q.mem_level, len, &mp)) {
+            snprintf(g_err, sizeof g_err, "deflate_batch_params: item %u: level %d, strategy %d, window_bits %d, mem_level %d is not a "
+                     "deflateInit2 parameter set", i, q.level, q.strategy, q.window_bits, q.mem_level);
+            return ZB_E_PARAM;
+        }
+        h_mp[i] = mp; // by input order for now
+        total += len;
+        bound += stream_bound(len);
+    }
+    if (total > kBatchMaxBytes) { snprintf(g_err, sizeof g_err, "deflate_batch_params: %llu bytes in all (at most 2^31)", (unsigned long long)total); return ZB_E_PARAM; }
+    if (total && !src) { snprintf(g_err, sizeof g_err, "deflate_batch_params: null source"); return ZB_E_PARAM; }
+    res->exact_parity = 1;
+    res->bits_used = 8;
+    dst_off[0] = 0;
+    if (nm == 0) return ZB_OK;
+    uint32_t cbeg[kClasses + 1]; // class c: staged members [cbeg[c], cbeg[c + 1])
+    batch_class_order(h_mp, nm, cbeg, h_morder);
+    // the staged table: member m = morder[i] is item i; its record, offset, length, slots and the lengths its checks cover
+    std::vector<MemberParams> byin(h_mp, h_mp + nm);
+    bool any_z = false, any_g = false;
+    for (uint32_t i = 0; i < nm; i++) {
+        const uint32_t m = h_morder[i], len = (uint32_t)(src_off[i + 1] - src_off[i]);
+        h_mp[m] = byin[i];
+        h_mlen[m] = len;
+        h_soff[m] = src_off[i];
+        h_lz[m] = byin[i].wrap == 1 ? len : 0;
+        h_lg[m] = byin[i].wrap == 2 ? len : 0;
+        any_z |= byin[i].wrap == 1;
+        any_g |= byin[i].wrap == 2;
+    }
+    const uint64_t span = batch_params_layout(h_mp, h_mlen, nm, h_moff, h_mslot);
+    const uint32_t nslots = h_mslot[nm];
+    auto has = [&](uint32_t c) { return cbeg[c + 1] > cbeg[c]; };
+    const bool links = cbeg[kClassSlow9 + 1] > cbeg[kClassMedium], steps = cbeg[kClassRle + 1] > cbeg[kClassSlow];
+    CK(cudaSetDevice(device));
+    launches = 0;
+    const size_t out_cap = (bound + 15) & ~(size_t)15;
+    JobBufs jb;
+    BgzfJob bj;
+    uint32_t *d_freq;
+    if ((rc = members_alloc(jb, bj, nm, (uint32_t)span, span, out_cap, 0, nslots, nslots > 0, links, steps, &d_freq)) != ZB_OK) return rc;
+    // S_BATCH: soff | mp | mslot | morder | lz | lg | mcrc | a host source
+    const size_t a8 = ((size_t)nm * 8 + 63) & ~(size_t)63, a4 = ((size_t)nm * 4 + 4 + 63) & ~(size_t)63;
+    const size_t amp = ((size_t)nm * sizeof(MemberParams) + 63) & ~(size_t)63;
+    void *p;
+    if ((rc = reserve(S_BATCH, a8 + amp + 5 * a4 + (src_dev ? 0 : total), &p)) != ZB_OK) return rc;
+    uint8_t *t = static_cast<uint8_t *>(p);
+    uint64_t *d_soff = reinterpret_cast<uint64_t *>(t);
+    MemberParams *d_mp = reinterpret_cast<MemberParams *>(t + a8);
+    uint32_t *d_mslot = reinterpret_cast<uint32_t *>(t + a8 + amp), *d_morder = reinterpret_cast<uint32_t *>(t + a8 + amp + a4);
+    uint32_t *d_lz = reinterpret_cast<uint32_t *>(t + a8 + amp + 2 * a4), *d_lg = reinterpret_cast<uint32_t *>(t + a8 + amp + 3 * a4);
+    uint32_t *d_mcrc = reinterpret_cast<uint32_t *>(t + a8 + amp + 4 * a4);
+    const uint8_t *d_src = src_dev ? static_cast<const uint8_t *>(src) + src_off[0] : t + a8 + amp + 5 * a4;
+    bj.mp = d_mp;
+    bj.mslot = d_mslot;
+    bj.morder = d_morder;
+    bj.mcrc = d_mcrc;
+    const size_t mi_bytes = ((size_t)nm * sizeof(JobInfo) + 15) & ~(size_t)15;
+
+    CK(cudaEventRecord(ev0, st));
+    CK(cudaMemcpyAsync(bj.moff, h_moff, (size_t)nm * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(bj.mlen, h_mlen, (size_t)nm * 4, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_soff, h_soff, (size_t)nm * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_mp, h_mp, (size_t)nm * sizeof(MemberParams), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_mslot, h_mslot, ((size_t)nm + 1) * 4, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_morder, h_morder, (size_t)nm * 4, cudaMemcpyHostToDevice, st));
+    if (any_z) CK(cudaMemcpyAsync(d_lz, h_lz, (size_t)nm * 4, cudaMemcpyHostToDevice, st));
+    if (any_g) CK(cudaMemcpyAsync(d_lg, h_lg, (size_t)nm * 4, cudaMemcpyHostToDevice, st));
+    if (!src_dev && total) CK(cudaMemcpyAsync(const_cast<uint8_t *>(d_src), static_cast<const uint8_t *>(src) + src_off[0], total, cudaMemcpyHostToDevice, st));
+    // k_batch_stage reads member m at src + (soff[m] - soff[0]): shift the source so that this is the item's caller offset
+    k_batch_stage<<<nm, 256, 0, st>>>(d_src + (h_soff[0] - src_off[0]), d_soff, nullptr, bj, const_cast<uint8_t *>(jb.in), span);
+    CK(cudaMemsetAsync(const_cast<uint8_t *>(jb.in) + span, 0, kPad + 16, st));
+    CK(cudaMemsetAsync(bj.minfo, 0, mi_bytes + sizeof(BgzfCtl), st));
+    CK(cudaMemsetAsync(jb.out, 0, out_cap, st));
+    launches++;
+    // the items' checks: adler32 over the zlib members, crc32 over the gzip members (the others get segments of length 0)
+    CK(cudaMemsetAsync(bj.mcheck, 0, (size_t)nm * 4, st));
+    if (any_z) { CK(launch_adler32_segments(jb.in, bj.moff, d_lz, nm, bj.mcheck, st)); launches++; }
+    if (any_g) { CK(launch_crc32_segments(jb.in, bj.moff, d_lg, nm, d_mcrc, st)); launches++; }
+    // links over the staged range of a run of classes: the members' own coordinates are shift invariant
+    auto link_range = [&](uint32_t m0, uint32_t m1, bool roll) {
+        if (m1 <= m0) return;
+        JobBufs r = jb;
+        const uint64_t o0 = h_moff[m0], o1 = m1 < nm ? h_moff[m1] : span;
+        r.in += o0;
+        r.L += o0;
+        r.keys += o0;
+        r.N = (uint32_t)(o1 - o0);
+        const uint32_t nt = r.N / kLinkTile + 1;
+        if (roll) {
+            k_links2_roll<<<nt, 1024, kLinks2SmemBytes, st>>>(r, 0);
+            k_links_fix_roll<<<r.N / 256 + 1, 256, 0, st>>>(r);
+        } else {
+            k_links2_std<<<nt, 1024, kLinks2SmemBytes, st>>>(r, 0);
+            k_links_fix_std<<<r.N / 256 + 1, 256, 0, st>>>(r);
+        }
+        launches += 2;
+    };
+    link_range(cbeg[kClassMedium], cbeg[kClassSlow9], false); // levels 3..8: standard hash
+    link_range(cbeg[kClassSlow9], cbeg[kClassRle], true);     // level 9: rolling hash
+    // the parsers, each over its class's members (a view of the member tables from the class's first member)
+    auto view = [&](uint32_t c0, uint32_t c1) {
+        BgzfJob v = bj;
+        const uint32_t m0 = cbeg[c0];
+        v.nm = cbeg[c1] - m0;
+        v.moff += m0;
+        v.mlen += m0;
+        v.minfo += m0;
+        v.mp += m0;
+        v.mslot += m0;
+        return v;
+    };
+    if (has(kClassQuick)) {
+        JobBufs q = jb;
+        q.serial_mode = 1;
+        const BgzfJob v = view(kClassQuick, kClassQuick + 1);
+        k_serial_low_members<<<v.nm, 32, kSerialSmemQuick, st>>>(q, v);
+        launches++;
+    }
+    if (has(kClassFast)) {
+        JobBufs q = jb;
+        q.serial_mode = 2;
+        const BgzfJob v = view(kClassFast, kClassFast + 1);
+        k_serial_low_members<<<v.nm, 32, kSerialSmemBytes, st>>>(q, v);
+        launches++;
+    }
+    if (has(kClassMedium)) {
+        const BgzfJob v = view(kClassMedium, kClassMedium + 1);
+        k_bgzf_medium<<<v.nm, 32, 0, st>>>(jb, v);
+        launches++;
+    }
+    if (cbeg[kClassRle] > cbeg[kClassSlow]) { // levels 7..9
+        const BgzfJob v = view(kClassSlow, kClassRle);
+        k_bgzf_slow_steps<<<v.nm * (kMemberMax / 256), 256, 0, st>>>(jb, v);
+        k_bgzf_slow_walk<<<(v.nm + 31) / 32, 32, 0, st>>>(jb, v);
+        launches += 2;
+    }
+    if (has(kClassRle)) {
+        const BgzfJob v = view(kClassRle, kClassRle + 1);
+        k_bgzf_rle_steps<<<v.nm * (kMemberMax / 256), 256, 0, st>>>(jb, v);
+        k_bgzf_slow_walk<<<(v.nm + 31) / 32, 32, 0, st>>>(jb, v);
+        launches += 2;
+    }
+    if (has(kClassHuff)) {
+        const BgzfJob v = view(kClassHuff, kClassHuff + 1);
+        k_bgzf_literals<<<v.nm * (kMemberMax / 256), 256, 0, st>>>(jb, v);
+        launches++;
+    }
+    if ((rc = members_blocks(jb, bj, nslots > 0, nslots, d_freq)) != ZB_OK) return rc;
+    CK(cudaMemcpyAsync(h_ctl, bj.ctl, sizeof(BgzfCtl), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(h_mout, bj.mout, (size_t)nm * 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(h_adler, bj.mcheck, (size_t)nm * 4, cudaMemcpyDeviceToHost, st));
+    if (any_g) CK(cudaMemcpyAsync(h_crc, d_mcrc, (size_t)nm * 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (h_ctl->error) { snprintf(g_err, sizeof g_err, "engine error flags 0x%x (batch_params)", h_ctl->error); return ZB_E_INTERNAL; }
+    const uint64_t out_bytes = h_ctl->out_bytes;
+    if (out_bytes > dst_cap) {
+        res->out_bytes = out_bytes;
+        return ZB_E_BUF;
+    }
+    CK(cudaMemcpyAsync(dst, jb.out, out_bytes, dst_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
+    CK(cudaEventRecord(ev1, st));
+    CK(cudaStreamSynchronize(st));
+    float ms = 0;
+    CK(cudaEventElapsedTime(&ms, ev0, ev1));
+    for (uint32_t i = 0; i < nm; i++) {
+        const uint32_t m = h_morder[i];
+        dst_off[i] = h_mout[m];
+        if (checks) checks[i] = byin[i].wrap == 1 ? h_adler[m] : byin[i].wrap == 2 ? h_crc[m] : 0u;
+    }
+    dst_off[nm] = out_bytes;
+    res->out_bytes = out_bytes;
+    res->data_type = (int32_t)h_ctl->data_type;
+    res->iterations = nslots > 0 ? 1 : 0;
     res->n_symbols = h_ctl->n_syms;
     res->n_blocks = h_ctl->n_blocks;
     res->gpu_launches = launches;
@@ -1327,6 +1577,14 @@ int zb_deflate_flushed(zb_engine *z, const void *src, const uint64_t *seg_off, s
     if (!z) return ZB_E_NODEVICE;
     z->e.shard.phase = 0; // a range job in progress is gone (its buffers are reused)
     return z->e.deflate_flushed(src, seg_off, n_segs, src_dev != 0, dst, cap, dst_dev != 0, level, strategy, window_bits, flags, restart, res);
+}
+
+int zb_deflate_batch_params(zb_engine *z, const void *src, const uint64_t *src_off, size_t n_items, int src_dev, const zb_batch_params *params,
+                            size_t n_params, void *dst, size_t cap, int dst_dev, uint64_t *dst_off, uint32_t *checks, zb_deflate_result *res)
+{
+    if (!z) return ZB_E_NODEVICE;
+    z->e.shard.phase = 0; // a range job in progress is gone (its buffers are reused)
+    return z->e.deflate_batch_params(src, src_off, n_items, src_dev != 0, params, n_params, dst, cap, dst_dev != 0, dst_off, checks, res);
 }
 
 size_t zb_deflate_flushed_bound(const uint64_t *seg_off, size_t n_segs)

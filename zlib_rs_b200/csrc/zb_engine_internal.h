@@ -111,6 +111,12 @@ struct Engine {
     int members_reserve(JobBufs &jb, BgzfJob &bj, uint32_t nm, uint32_t S, size_t span, int level, size_t out_cap, uint32_t wrap,
                         uint32_t **d_freq);
     int members_launch(JobBufs &jb, BgzfJob &bj, int level, uint32_t *d_freq);
+    int members_alloc(JobBufs &jb, BgzfJob &bj, uint32_t nm, uint32_t S, size_t span, size_t out_cap, uint32_t wrap, uint32_t nslots,
+                      bool parse, bool links, bool slow, uint32_t **d_freq);
+    int members_blocks(JobBufs &jb, BgzfJob &bj, bool blocks, uint32_t nslots, uint32_t *d_freq);
+    int deflate_batch_params(const void *src, const uint64_t *src_off, size_t n_items, bool src_dev, const zb_batch_params *params,
+                             size_t n_params, void *dst, size_t dst_cap, bool dst_dev, uint64_t *dst_off, uint32_t *checks,
+                             zb_deflate_result *res);
     int inflate(const void *src, size_t n, bool src_dev, void *dst, size_t dst_cap, bool dst_dev, int window_bits,
                 zb_inflate_result *res, uint32_t flags = 0, IdxBuild *ib = nullptr);
     int inflate_stream(const uint8_t *d_src, size_t n, uint8_t *d_dst, size_t dst_cap, int window_bits, uint32_t flags,

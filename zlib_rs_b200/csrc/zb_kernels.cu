@@ -1849,19 +1849,22 @@ __global__ void __launch_bounds__(1024) k_encode(JobBufs jb)
 
 // ------------------------------------------------------------------------------------------------
 // Members of a BGZF file or a batch (zb_bgzf.h, zb_bgzf.cu): the block kernels above over every member at once, one CTA per block
-// slot m * kBgzfMaxBlocks + k.  Positions and symbols are member-relative (a dictionary's bytes included, so block_start and
+// slot slot0(m) + k (m * kBgzfMaxBlocks but for a batch with parameters per item).  Positions and symbols are member-relative (a dictionary's bytes included, so block_start and
 // have_window see the window as the single stream with a dictionary does); in_start and sym_begin point into the staged buffers.
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) k_bgzf_hist(JobBufs jb, BgzfJob bj, uint32_t *freq)
 {
-    const uint32_t b = blockIdx.x, m = b / kBgzfMaxBlocks, k = b % kBgzfMaxBlocks;
+    const uint32_t b = blockIdx.x;
+    uint32_t m, k;
+    bj.slot_member(b, m, k);
     const JobInfo &mi = bj.minfo[m];
     const uint32_t nsyms = mi.n_syms, nblocks = mi.n_blocks;
     if (k >= nblocks) return;
     const uint32_t base = (uint32_t)bj.moff[m], len = bj.pstart + bj.mlen[m]; // the member's end: dictionary and item
     const Sym *syms = jb.syms + base;
-    const uint32_t begin = k * jb.block_syms;
-    const uint32_t count = k + 1 < nblocks ? jb.block_syms : nsyms - begin;
+    const uint32_t bs = bj.mp ? bj.mp[m].bs : jb.block_syms;
+    const uint32_t begin = k * bs;
+    const uint32_t count = k + 1 < nblocks ? bs : nsyms - begin;
     block_hist_body(syms, begin, count, freq + (size_t)b * 320);
     if (threadIdx.x == 0) {
         BlockDesc &bd = jb.blocks[b];
@@ -1874,26 +1877,36 @@ __global__ void __launch_bounds__(256) k_bgzf_hist(JobBufs jb, BgzfJob bj, uint3
         bd.in_start = base + start;
         bd.in_len = end - start;
         uint32_t Bf;
+        // the parse's class: the call's, or the member's own (zb_deflate_batch_params)
+        const uint32_t cls = bj.mp ? bj.mp[m].cls : jb.slow_mode ? (uint32_t)kClassSlow : (uint32_t)kClassMedium;
+        const uint32_t w = bj.mp ? bj.mp[m].wsize : jb.wsize;
+        const uint32_t q = last ? 0u : syms[begin + count - 1].pos; // a block that is not the last holds bs >= 1 symbols
         if (last) Bf = mi.final_base;
-        else if (jb.slow_mode) Bf = base_at(syms[begin + count - 1].pos + 1, len, jb.wsize); // as k_block_hist
-        else Bf = jb.block_base[b]; // recorded by the parse at the flush (unused by deflate_quick's pieces)
+        else if (cls == kClassSlow || cls == kClassSlow9) Bf = base_at(q + 1, len, w); // as k_block_hist
+        else if (cls == kClassRle) Bf = base_at(q, len, w);
+        else if (cls == kClassHuff) Bf = q < 2 * w ? 0 : w * (1 + (q - 2 * w) / w);
+        else Bf = jb.block_base[bj.slot0(m) + k]; // recorded by the parse at the flush (unused by deflate_quick's pieces)
         bd.have_window = start >= Bf;
     }
 }
 
 __global__ void __launch_bounds__(32) k_bgzf_build(JobBufs jb, BgzfJob bj, const uint32_t *freq)
 {
-    const uint32_t b = blockIdx.x, m = b / kBgzfMaxBlocks, k = b % kBgzfMaxBlocks;
+    const uint32_t b = blockIdx.x;
+    uint32_t m, k;
+    bj.slot_member(b, m, k);
     const uint32_t nblocks = bj.minfo[m].n_blocks;
     if (k >= nblocks) return;
-    build_blocks_body(&jb.blocks[b], freq + (size_t)b * 320, jb.serial_mode == 1, k == 0, k + 1 == nblocks, !bj.flushed || m + 1 == bj.nm,
-                      false);
+    const bool quick = bj.mp ? bj.mp[m].cls == kClassQuick : jb.serial_mode == 1, fixed = bj.mp && bj.mp[m].fixed;
+    build_blocks_body(&jb.blocks[b], freq + (size_t)b * 320, quick, k == 0, k + 1 == nblocks, !bj.flushed || m + 1 == bj.nm, fixed);
 }
 
 // bit_base is absolute here (k_bgzf_scan); a member written stored has no blocks to encode
 __global__ void __launch_bounds__(1024) k_bgzf_encode(JobBufs jb, BgzfJob bj)
 {
-    const uint32_t b = blockIdx.x, m = b / kBgzfMaxBlocks, k = b % kBgzfMaxBlocks;
+    const uint32_t b = blockIdx.x;
+    uint32_t m, k;
+    bj.slot_member(b, m, k);
     if (bj.ctl->error || k >= bj.minfo[m].n_blocks || bj.mstored[m]) return;
     encode_body(jb.blocks[b], jb.syms, jb.in, jb.out, &bj.ctl->error);
 }
@@ -2019,7 +2032,7 @@ struct WriterMembers {
         if (eof(m)) return WriterUnits{nullptr, nullptr, 0, 0, bj.ctl->out_bytes - kBgzfEofLen + kBgzfHeader, 1, 1};
         const uint32_t len = bj.mlen[m];
         if (bj.mstored[m]) return WriterUnits{nullptr, nullptr, 0, len, bj.mout[m] + kBgzfHeader, 0, (uint32_t)stored_blocks(len)};
-        return WriterUnits{jb.blocks + m * kBgzfMaxBlocks, jb.syms, bj.moff[m], len, 0, 0, bj.minfo[m].n_blocks};
+        return WriterUnits{jb.blocks + bj.slot0((uint32_t)m), jb.syms, bj.moff[m], len, 0, 0, bj.minfo[m].n_blocks};
     }
     __device__ uint64_t n_units(uint64_t m) const { return units(m).nb; }
     __device__ IdxPick pick(uint64_t m, uint64_t T) const

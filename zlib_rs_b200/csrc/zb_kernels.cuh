@@ -117,8 +117,8 @@ struct JobBufs {
 };
 
 // One member call (zb_bgzf.h): a BGZF file (ZB_FLAG_BGZF) or a batch of streams (zb_deflate_batch).  Member m is staged at
-// moff[m] of JobBufs::in, its symbols start at syms[moff[m]], its deflate blocks are blocks[m * kBgzfMaxBlocks + k] and the
-// window bases of their flushes block_base[m * kBgzfMaxBlocks + k].
+// moff[m] of JobBufs::in, its symbols start at syms[moff[m]], its deflate blocks are blocks[slot0(m) + k] and the window bases
+// of their flushes block_base[slot0(m) + k] (slot0(m) = m * kBgzfMaxBlocks unless the members have their own slot table).
 struct BgzfCtl {
     uint32_t count;     // members (k_crc_join)
     uint32_t error;     // non-zero: internal invariant violated
@@ -146,6 +146,27 @@ struct BgzfJob {
                         // frames the stream, member 0 has the header, the last the trailer, every other one the empty stored block
     uint32_t *fcheck;   // flushed: the check of the whole input, joined from mcheck
     uint32_t isize;     // flushed: the input length mod 2^32 (gzip's ISIZE)
+    // zb_deflate_batch_params (zb_bgzf.h, DESIGN.md §2o); all nullptr for the other member calls, whose members share the call's
+    // parameters and kBgzfMaxBlocks block slots each
+    const MemberParams *mp;  // member m's parameters
+    const uint32_t *mslot;   // nm + 1 entries: member m's block slots are [mslot[m], mslot[m + 1])
+    const uint32_t *morder;  // input order: item i is staged as member morder[i]
+    uint32_t *mcrc;          // crc32 of the gzip members (mcheck holds the adler32 of the zlib members)
+    ZB_HD uint32_t slot0(uint32_t m) const { return mslot ? mslot[m] : m * kBgzfMaxBlocks; }
+    ZB_HD uint32_t nslots(uint32_t m) const { return mslot ? mslot[m + 1] - mslot[m] : kBgzfMaxBlocks; }
+    ZB_HD uint32_t wrap_of(uint32_t m) const { return mp ? mp[m].wrap : wrap; }
+    // the member and block of block slot b
+    ZB_HD void slot_member(uint32_t b, uint32_t &m, uint32_t &k) const
+    {
+        if (!mslot) { m = b / kBgzfMaxBlocks; k = b % kBgzfMaxBlocks; return; }
+        uint32_t lo = 0, hi = nm; // the last m with mslot[m] <= b (members without slots are skipped)
+        while (hi - lo > 1) {
+            const uint32_t mid = (lo + hi) / 2;
+            if (mslot[mid] <= b) lo = mid; else hi = mid;
+        }
+        m = lo;
+        k = b - mslot[lo];
+    }
 };
 
 // zb_deflate_index (DESIGN.md §2l): k_deflate_points runs one warp per slot, the targets k * span (k = 1..K) and then the first

@@ -106,8 +106,9 @@ __global__ void __launch_bounds__(32) k_serial_low_members(JobBufs jb, BgzfJob b
     mj.in = jb.in + base;
     mj.N = bj.mlen[m];
     mj.syms = jb.syms + base;
-    mj.block_base = jb.block_base + m * kBgzfMaxBlocks;
+    mj.block_base = jb.block_base + bj.slot0(m);
     mj.info = bj.minfo + m;
+    if (bj.mp) { mj.wsize = bj.mp[m].wsize; mj.block_syms = bj.mp[m].bs; } // zb_deflate_batch_params: the member's window and memLevel
     if (jb.serial_mode == 1) serial_low_body<kRingQuick, false>(mj, smem);
     else serial_low_body<kRingFast, true>(mj, smem);
 }

@@ -556,21 +556,10 @@ __global__ void __launch_bounds__(256) k_rle(JobBufs jb)
 {
     const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x, N = jb.N;
     if (p >= N) return;
-    const uint8_t *d = jb.in;
-    const uint32_t B = base_at(p, N, jb.wsize), la = lookahead_at(p, B, N, jb.wsize);
-    uint32_t len = 0;
-    if (la >= 3 && p > 0 && d[p - 1] == d[p] && d[p] == d[p + 1]) {
-        const uint32_t c = d[p - 1];
-        uint32_t n = 0;
-        while (n < 256 && p + 2 + n < N + kPad - 8 && d[p + 2 + n] == c) n++; // bytes behind the input: the clamp below decides
-        len = n + 2;
-        if (len > la) len = la;
-        if (len > kMaxMatch) len = kMaxMatch;
-        if (len < 3) len = 0;
-    }
-    const uint32_t next = p + (len ? len : 1u);
+    const SlowStep s = rle_step(jb.in, p, N, jb.wsize, N + kPad - 8); // bytes behind the input: the clamp decides
+    const uint32_t next = s.next;
     jb.nxt[p] = ((next - p) & 0xffffu) | (1u << 16) | (next >= N ? kNxtTail : 0u);
-    jb.M[p] = len ? pack_step(SlowStep{next, 0, len, 1}) : pack_step(SlowStep{next, 1, 0, 0});
+    jb.M[p] = pack_step(s);
 }
 
 __device__ __forceinline__ uint32_t emit_step(const JobBufs &jb, uint32_t p, Sym *out)

@@ -183,6 +183,25 @@ ZB_HD uint32_t pack_step(const SlowStep &s)
     return (s.nlit << 24) | (s.len ? ((s.len - 3u) << 16) | 0x8000u | (s.dist - 1u) : 0u);
 }
 
+// Z_RLE's step at p (deflate/algorithm/rle.rs): a match is a run of the previous byte (distance 1), clamped to the lookahead and
+// 258 bytes, so it depends on the data only.  Bytes are read up to `lim` (exclusive): what the run does beyond the lookahead does
+// not change the clamped length.
+ZB_HD SlowStep rle_step(const uint8_t *d, uint32_t p, uint32_t N, uint32_t w, uint32_t lim)
+{
+    const uint32_t B = base_at(p, N, w), la = lookahead_at(p, B, N, w);
+    uint32_t len = 0;
+    if (la >= 3 && p > 0 && d[p - 1] == d[p] && d[p] == d[p + 1]) {
+        const uint32_t c = d[p - 1];
+        uint32_t n = 0;
+        while (n < 256 && p + 2 + n < lim && d[p + 2 + n] == c) n++;
+        len = n + 2;
+        if (len > la) len = la;
+        if (len > kMaxMatch) len = kMaxMatch;
+        if (len < 3) len = 0;
+    }
+    return len ? SlowStep{p + len, 0, len, 1} : SlowStep{p + 1, 1, 0, 0};
+}
+
 // Search at loop-top q with prev_length pl (slow.rs:56-82).  Returns the new match_len (2 = none) and start.
 template <class A>
 ZB_HD Match slow_search(const A &a, uint32_t q, uint32_t pl, uint32_t ms, uint32_t B, uint32_t N, const SlowParams &sp)
