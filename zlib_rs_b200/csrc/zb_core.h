@@ -331,8 +331,15 @@ struct SerialAcc {
     const SA &a;
     uint32_t ins_base, ins_words;
     uint32_t *ins; // bitmap for positions >= ins_base: 1 = inserted
+    uint32_t base = 0; // the window base in force: a link to it or below reads window index 0, which the reference never matches
     ZB_HD uint32_t byte(uint32_t y) const { return a.byte(y); }
-    ZB_HD uint32_t link(uint32_t y) const { return a.link(y); }
+    ZB_HD uint32_t link(uint32_t y) const
+    {
+        // Only once the input is exhausted can a loop-top stand w - 262 past a base above 0 (fill_window slides at strstart >=
+        // w + max_dist, deflate.rs:1776-1806): its head at distance max_dist is window index 0, NIL (medium.rs:76).
+        const uint32_t d = a.link(y);
+        return d && base && y - d <= base ? 0u : d;
+    }
     ZB_HD bool inserted(uint32_t y) const
     {
         if (y < ins_base) return a.inserted(y);
@@ -362,12 +369,14 @@ ZB_HDN uint32_t serial_medium(const SA &a0, uint32_t N, uint32_t p0, uint32_t *i
     uint32_t B = p0 == 0 ? 0 : wbase_w(wn, p0 - 1);
     uint32_t F = (uint64_t)B + 2 * kW < N ? B + 2 * kW : N;
     uint32_t p = p0;
+    a.base = B;
     PMatch cur{0, 0, 0, 0}, next{0, 0, 0, 0};
     for (;;) {
         uint32_t lookahead = F - p;
         if (lookahead < kMinLookahead) {
             // fill_window (deflate.rs:1776-1861)
             if (p - B >= kW + kMD) B += kW;
+            a.base = B;
             if (F < N) {
                 F = (uint64_t)B + 2 * kW < N ? B + 2 * kW : N;
                 // quick_insert_string(strstart-1) (deflate.rs:1836-1838).  p-1 is the last byte of the previous
