@@ -139,7 +139,33 @@ ZB_API int zb_deflate_batch_dict(zb_engine *e, const void *dict, size_t dict_len
                                  size_t n_items, int src_on_device, void *dst, size_t dst_cap, int dst_on_device, int level, int strategy,
                                  int window_bits, uint32_t flags, uint64_t *dst_off, uint32_t *checks, zb_deflate_result *res);
 
-/* zb_deflate_batch_params: a batch whose items each carry their own deflateInit2 parameters (DESIGN.md §2o).  params holds 1 entry,
+/* zb_deflate_batch_dicts / zb_inflate_batch_dicts: batches whose items each name their own preset dictionary (DESIGN.md §2p).  The
+ * dictionaries form one table: dictionary j is dicts[dict_off[j], dict_off[j+1]) (dict_off: a host array of n_dicts + 1 offsets;
+ * dicts a host pointer, or a device pointer with src_on_device).  which (host, n_items entries) names item i's dictionary: an index
+ * below n_dicts, ZB_DICT_NONE, or on inflate ZB_DICT_BY_ID.
+ * Deflate: item i's stream is byte for byte zb_deflate_batch_dict(dictionary which[i], {item i}) -- deflateInit2 +
+ * deflateSetDictionary + deflate(Z_FINISH) of that item alone -- and an item with ZB_DICT_NONE or an empty dictionary gets
+ * zb_deflate_batch's bytes.  A zlib item whose dictionary put bytes in the window gets FDICT and DICTID = the adler32 of its whole
+ * dictionary.  The rules and limits are zb_deflate_batch_dict's (window_bits 15 / -15, Z_DEFAULT_STRATEGY, memLevel 8, levels -1,
+ * 0, 3..9, every item staged behind its own copy of its dictionary's window bytes and the staged bytes at most 2^31), and n_dicts
+ * <= 65535, at most 2^31 dictionary bytes in all, every which[i] in range; anything else is ZB_E_PARAM with a zb_last_error() text
+ * naming the item or the dictionary.  zb_deflate_batch_bound is enough.  Launches: zb_deflate_batch's, one more for DICTID when a
+ * zlib item names a non-empty dictionary, one more at levels 3..8 when an item's window holds at least 3 dictionary bytes.
+ * Inflate: which may be NULL (every item ZB_DICT_BY_ID).  items[i] gets what zb_inflate_batch_dict(d, {item i}) gives: with an
+ * index j, d is dictionary j (a raw item decodes with it as its window, a zlib FDICT item only when its DICTID is adler32(j), else
+ * "need dictionary"); with ZB_DICT_BY_ID a zlib FDICT item takes the lowest-index dictionary whose adler32 is its DICTID ("need
+ * dictionary" when none is; a header cut inside its DICTID is truncated, as with any dictionary) and a raw item none; with
+ * ZB_DICT_NONE no dictionary.  gzip items and zlib items without FDICT decode as with zb_inflate_batch, +32 auto-detection too.
+ * The limits are zb_inflate_batch's, n_dicts <= 2^20 and at most 2^31 dictionary bytes.  Launches: zb_inflate_batch's 4, and one
+ * for the adler32 of every dictionary when n_dicts > 0. */
+#define ZB_DICT_NONE 0xffffffffu  /* the item uses no dictionary */
+#define ZB_DICT_BY_ID 0xfffffffeu /* inflate only: a zlib FDICT item takes the lowest-index dictionary whose adler32 is its DICTID */
+ZB_API int zb_deflate_batch_dicts(zb_engine *e, const void *dicts, const uint64_t *dict_off, size_t n_dicts, const uint32_t *which,
+                                  const void *src, const uint64_t *src_off, size_t n_items, int src_on_device, void *dst,
+                                  size_t dst_cap, int dst_on_device, int level, int strategy, int window_bits, uint32_t flags,
+                                  uint64_t *dst_off, uint32_t *checks, zb_deflate_result *res);
+
+/* zb_deflate_batch_params:a batch whose items each carry their own deflateInit2 parameters (DESIGN.md §2o).  params holds 1 entry,
  * used for every item, or n_items entries, one per item; any other n_params is ZB_E_PARAM.  An entry is accepted exactly when
  * deflateInit2 accepts it: level -1..9, strategy 0..4 (Z_DEFAULT_STRATEGY, Z_FILTERED, Z_HUFFMAN_ONLY, Z_RLE, Z_FIXED), window_bits
  * 8..15 (zlib; 8 is 9 with CINFO 1), -9..-15 (raw) or 25..31 (gzip), mem_level 1..9.  Item i's stream is byte for byte what
@@ -243,6 +269,10 @@ ZB_API int zb_inflate_batch(zb_engine *e, const void *src, const uint64_t *src_o
 ZB_API int zb_inflate_batch_dict(zb_engine *e, const void *dict, size_t dict_len, const void *src, const uint64_t *src_off,
                                  size_t n_items, int src_on_device, void *dst, const uint64_t *dst_off, int dst_on_device, int window_bits,
                                  zb_inflate_result *items);
+/* zb_inflate_batch_dicts: a dictionary per item, see zb_deflate_batch_dicts above (DESIGN.md §2p). */
+ZB_API int zb_inflate_batch_dicts(zb_engine *e, const void *dicts, const uint64_t *dict_off, size_t n_dicts, const uint32_t *which,
+                                  const void *src, const uint64_t *src_off, size_t n_items, int src_on_device, void *dst,
+                                  const uint64_t *dst_off, int dst_on_device, int window_bits, zb_inflate_result *items);
 
 /* zb_inflate_flushed: decode any set of segments of a stream written with full flushes, each from its restart point with an empty
  * window (DESIGN.md §2m).  Segment k is src[restart[k], restart[k+1]) (restart: host, n_segs + 1 entries, as zb_deflate_flushed

@@ -18,6 +18,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("ZB_LIB_PATH") or os.path.join(_HERE, "libz_b200.so")  # ZB_LIB_PATH: another build of the library, e.g. a baseline for scripts/gpu_ab.sh
 
 Z_OK, Z_STREAM_END, Z_NEED_DICT = 0, 1, 2
+DICT_NONE, DICT_BY_ID = 0xFFFFFFFF, 0xFFFFFFFE  # ZB_DICT_NONE, ZB_DICT_BY_ID of Engine.deflate_batch_dicts / inflate_batch_dicts
 Z_ERRNO, Z_STREAM_ERROR, Z_DATA_ERROR, Z_MEM_ERROR, Z_BUF_ERROR, Z_VERSION_ERROR = -1, -2, -3, -4, -5, -6
 Z_NO_FLUSH, Z_PARTIAL_FLUSH, Z_SYNC_FLUSH, Z_FULL_FLUSH, Z_FINISH, Z_BLOCK = 0, 1, 2, 3, 4, 5
 Z_DEFAULT_STRATEGY, Z_FILTERED, Z_HUFFMAN_ONLY, Z_RLE, Z_FIXED = 0, 1, 2, 3, 4
@@ -183,6 +184,10 @@ def lib():
         if hasattr(L, "zb_deflate_batch_dict"):
             L.zb_deflate_batch_dict.argtypes = [vp, vp, sz] + L.zb_deflate_batch.argtypes[1:]
             L.zb_inflate_batch_dict.argtypes = [vp, vp, sz] + L.zb_inflate_batch.argtypes[1:]
+        if hasattr(L, "zb_deflate_batch_dicts"):
+            u64p = ctypes.POINTER(u64)
+            L.zb_deflate_batch_dicts.argtypes = [vp, vp, u64p, sz, ctypes.POINTER(u32)] + L.zb_deflate_batch.argtypes[1:]
+            L.zb_inflate_batch_dicts.argtypes = [vp, vp, u64p, sz, ctypes.POINTER(u32)] + L.zb_inflate_batch.argtypes[1:]
         L.zb_adler32.argtypes = [vp, u32, vp, sz, ci, ctypes.POINTER(u32), ctypes.POINTER(ctypes.c_float)]
         L.zb_crc32.argtypes = [vp, u32, vp, sz, ci, ctypes.POINTER(u32), ctypes.POINTER(ctypes.c_float)]
         L.zb_engine_set_profile.argtypes = [vp, ci]
@@ -249,6 +254,26 @@ def _dictionary(dictionary, on_device):
     data = bytes(dictionary)
     keep = (ctypes.c_char * max(len(data), 1)).from_buffer_copy(data or b"\0")
     return ctypes.addressof(keep), len(data), keep
+
+
+def _dictionaries(dictionaries, dict_off, on_device):
+    """(pointer, offsets, n, keep-alive) of a dictionary table: a list of bytes-like objects on the host; with on_device a device
+    pointer with `dict_off` (n + 1 offsets into it), or a (pointer, dict_off) pair."""
+    if on_device:
+        if isinstance(dictionaries, tuple):
+            dictionaries, dict_off = dictionaries
+        off = (ctypes.c_uint64 * len(dict_off))(*dict_off)
+        return dictionaries, off, len(dict_off) - 1, None
+    keep, off = _gather(dictionaries)
+    return ctypes.addressof(keep), off, len(off) - 1, keep
+
+
+def _which(which, n):
+    """The dictionary index of every item as a uint32 array: None is DICT_NONE."""
+    w = [DICT_NONE if x is None else int(x) for x in which]
+    if len(w) != n:
+        raise ValueError("which has %d entries for %d items" % (len(w), n))
+    return (ctypes.c_uint32 * max(n, 1))(*w)
 
 
 def deflate_batch_bound(lengths):
@@ -633,6 +658,77 @@ class Engine:
         raw = own.raw if own is not None else None
         outs = [raw[offs[i]:offs[i + 1]] for i in range(n)] if own is not None else None
         return outs, offs, list(checks)[:n], res
+
+    def deflate_batch_dicts(self, items, dictionaries, which, level=-1, window_bits=15, src_on_device=False, src_off=None,
+                            dict_off=None, dst=None, dst_cap=0, dst_on_device=False):
+        """Deflate every item as its own stream after deflateSetDictionary of its own dictionary, in one call
+        (zb_deflate_batch_dicts).  `dictionaries`: a list of bytes-like objects, or with src_on_device a device pointer with
+        `dict_off` (or a (pointer, dict_off) pair).  which[i] is item i's dictionary index, or None for no dictionary.  Item i's
+        stream is byte for byte deflate_batch([item i], dictionary=its dictionary)'s.  Items, `dst` and the result are as in
+        deflate_batch: (list of bytes or None, offsets (n + 1), checks, DeflateResult).  Raises ZlibError."""
+        res = DeflateResult()
+        keep = None
+        if src_on_device:
+            off = (ctypes.c_uint64 * len(src_off))(*src_off)
+            src = items
+        else:
+            keep, off = _gather(items)
+            src = ctypes.addressof(keep)
+        n = len(off) - 1
+        dptr, doff, nd, dkeep = _dictionaries(dictionaries, dict_off, src_on_device)
+        w = _which(which, n)
+        own = None
+        if dst is None:
+            dst_cap = lib().zb_deflate_batch_bound(off, n) + 64
+            own = ctypes.create_string_buffer(dst_cap)
+            dst = ctypes.addressof(own)
+            dst_on_device = False
+        dst_off = (ctypes.c_uint64 * (n + 1))()
+        checks = (ctypes.c_uint32 * max(n, 1))()
+        rc = lib().zb_deflate_batch_dicts(self.h, dptr, doff, nd, w, src, off, n, int(src_on_device), dst, dst_cap, int(dst_on_device),
+                                          level, 0, window_bits, 0, dst_off, checks, ctypes.byref(res))
+        if rc != 0:
+            e = ZlibError(rc, lib().zb_last_error().decode())
+            e.needed = res.out_bytes
+            raise e
+        offs = list(dst_off)
+        raw = own.raw if own is not None else None
+        outs = [raw[offs[i]:offs[i + 1]] for i in range(n)] if own is not None else None
+        return outs, offs, list(checks)[:n], res
+
+    def inflate_batch_dicts(self, items, out_caps, dictionaries, which=None, window_bits=15, src_on_device=False, src_off=None,
+                            dict_off=None, dst=None, dst_off=None, dst_on_device=False):
+        """Inflate every item into its own slot in one call, each with its own preset dictionary (zb_inflate_batch_dicts).
+        `dictionaries` as in deflate_batch_dicts.  which[i]: a dictionary index, None (no dictionary) or DICT_BY_ID (a zlib FDICT
+        item takes the lowest-index dictionary whose adler32 is its DICTID); which=None is DICT_BY_ID for every item.  Items,
+        `dst` and the result are as in inflate_batch: (rc, list of bytes or None, list of InflateResult)."""
+        keep = None
+        if src_on_device:
+            off = (ctypes.c_uint64 * len(src_off))(*src_off)
+            src = items
+        else:
+            keep, off = _gather(items)
+            src = ctypes.addressof(keep)
+        n = len(off) - 1
+        dptr, doffs, nd, dkeep = _dictionaries(dictionaries, dict_off, src_on_device)
+        w = _which(which, n) if which is not None else None
+        own = None
+        if dst is None:
+            doff = _offsets(list(out_caps))
+            own = ctypes.create_string_buffer(max(doff[n], 1))
+            dst = ctypes.addressof(own)
+            dst_on_device = False
+        else:
+            doff = (ctypes.c_uint64 * len(dst_off))(*dst_off)
+        res = (InflateResult * max(n, 1))()
+        rc = lib().zb_inflate_batch_dicts(self.h, dptr, doffs, nd, w, src, off, n, int(src_on_device), dst, doff, int(dst_on_device),
+                                          window_bits, res)
+        results = list(res)[:n]
+        outs = None
+        if own is not None:
+            raw = own.raw
+            outs = [raw[doff[i]:doff[i] + results[i].out_bytes] for i in range(n)]
+        return rc, outs, results
 
     def deflate_batch_params(self, items, params, src_on_device=False, src_off=None, dst=None, dst_cap=0, dst_on_device=False):
         """Deflate every item as its own stream with its own deflateInit2 parameters in one call (zb_deflate_batch_params).

@@ -17,13 +17,15 @@ __global__ void __launch_bounds__(256) k_bgzf_setup(BgzfJob bj, uint64_t n)
 }
 
 // Batch staging: item m of the contiguous source `src` (item m at src[soff[m] - soff[0]], the member table filled by the host) goes
-// to its staged offset behind its own copy of the dictionary's window bytes dict[0, bj.pstart), and the gap behind it up to the next
-// item's offset (or `span`) is zeroed.  One CTA per item.
+// to its staged offset behind its own copy of its dictionary's window bytes dict[mdsrc[m], mdsrc[m] + D'), and the gap behind it up
+// to the next item's offset (or `span`) is zeroed.  One CTA per item.
 __global__ void __launch_bounds__(256) k_batch_stage(const uint8_t *__restrict__ src, const uint64_t *__restrict__ soff,
-                                                     const uint8_t *__restrict__ dict, BgzfJob bj, uint8_t *__restrict__ in, uint64_t span)
+                                                     const uint8_t *__restrict__ dict, const uint64_t *__restrict__ mdsrc, BgzfJob bj,
+                                                     uint8_t *__restrict__ in, uint64_t span)
 {
-    const uint32_t m = blockIdx.x, D = bj.pstart;
+    const uint32_t m = blockIdx.x, D = bj.pstart_of(m);
     const uint8_t *s = src + (soff[m] - soff[0]);
+    if (D) dict += mdsrc[m];
     uint8_t *d = in + bj.moff[m];
     const uint32_t len = bj.mlen[m];
     const uint64_t end = (m + 1 < bj.nm ? bj.moff[m + 1] : span) - bj.moff[m];
@@ -37,7 +39,7 @@ __global__ void __launch_bounds__(256) k_batch_stage(const uint8_t *__restrict__
 __global__ void __launch_bounds__(256) k_batch_dict_ghost(JobBufs jb, BgzfJob bj)
 {
     __shared__ uint32_t first;
-    const uint32_t m = blockIdx.x, D = bj.pstart, N = D + bj.mlen[m];
+    const uint32_t m = blockIdx.x, D = bj.pstart_of(m), N = D + bj.mlen[m];
     if (D < 3 || N == D) return;
     const uint8_t *d = jb.in + bj.moff[m];
     const uint32_t g = D - 3;
@@ -65,7 +67,7 @@ __global__ void __launch_bounds__(32) k_bgzf_medium(JobBufs jb, BgzfJob bj)
 {
     __shared__ uint32_t ins[kMemberMax / 32];
     if (threadIdx.x != 0) return;
-    const uint32_t m = blockIdx.x, base = (uint32_t)bj.moff[m], p0 = bj.pstart, len = p0 + bj.mlen[m];
+    const uint32_t m = blockIdx.x, base = (uint32_t)bj.moff[m], p0 = bj.pstart_of(m), len = p0 + bj.mlen[m];
     const uint32_t bs = bj.mp ? bj.mp[m].bs : jb.block_syms, w = bj.mp ? bj.mp[m].wsize : kWSize;
     const LevelParams lp = bj.mp ? level_params(bj.mp[m].level) : jb.lp;
     const BgzfAcc a{jb.in + base, jb.L + base, len, 4u, w, w - kMinLookahead};
@@ -92,7 +94,7 @@ __global__ void __launch_bounds__(256) k_bgzf_slow_steps(JobBufs jb, BgzfJob bj)
     const uint32_t m = blockIdx.x / (kMemberMax / 256), i = (blockIdx.x % (kMemberMax / 256)) * 256 + threadIdx.x;
     if (m >= bj.nm) return;
     if (i >= bj.mlen[m]) return;
-    const uint32_t y = bj.pstart + i, len = bj.pstart + bj.mlen[m];
+    const uint32_t p0 = bj.pstart_of(m), y = p0 + i, len = p0 + bj.mlen[m];
     const uint32_t base = (uint32_t)bj.moff[m], x = base + y;
     SlowParams sp = jb.sp;
     if (bj.mp) { sp = slow_params(bj.mp[m].level); sp.filtered = bj.mp[m].filtered; sp.wsize = bj.mp[m].wsize; }
@@ -142,14 +144,14 @@ __global__ void __launch_bounds__(32) k_bgzf_slow_walk(JobBufs jb, BgzfJob bj)
 {
     const uint32_t m = blockIdx.x * 32 + threadIdx.x;
     if (m >= bj.nm) return;
-    const uint32_t base = (uint32_t)bj.moff[m], len = bj.pstart + bj.mlen[m];
+    const uint32_t base = (uint32_t)bj.moff[m], p0 = bj.pstart_of(m), len = p0 + bj.mlen[m];
     const uint32_t bs = bj.mp ? bj.mp[m].bs : jb.block_syms, w = bj.mp ? bj.mp[m].wsize : jb.wsize;
     const bool lazy = bj.mp ? bj.mp[m].cls != kClassRle : jb.slow_mode == 1;
     const uint8_t *d = jb.in + base;
     const uint32_t *M = jb.M + base, *nxt = jb.nxt + base;
     Sym *syms = jb.syms + base;
     uint32_t n = 0;
-    for (uint32_t p = bj.pstart; p < len;) {
+    for (uint32_t p = p0; p < len;) {
         const uint32_t v = M[p], nlit = v >> 24;
         for (uint32_t i = 0; i < nlit; i++) syms[n++] = Sym{0, d[p + i], p + i};
         if (v & 0x8000u) syms[n++] = Sym{(uint16_t)((v & 0x7fffu) + 1u), (uint16_t)((v >> 16) & 0xffu), p + nlit};
@@ -197,7 +199,7 @@ __global__ void __launch_bounds__(256) k_bgzf_size(JobBufs jb, BgzfJob bj)
     atomicAdd(&bj.ctl->n_blocks, nb);
     bj.mstored[m] = stored;
     bj.mbytes[m] = bj.flushed ? flush_header_len(bj.wrap, m) + (uint32_t)payload + flush_trailer_len(bj.wrap, m, bj.nm)
-                              : member_header_len(wrap, bj.fdict) + (uint32_t)payload + member_trailer_len(wrap);
+                              : member_header_len(wrap, bj.fdict_of(m)) + (uint32_t)payload + member_trailer_len(wrap);
 }
 
 // One CTA: the members' offsets in the output (exclusive scan of their lengths, in input order), the blocks' absolute bit
@@ -222,7 +224,7 @@ __global__ void __launch_bounds__(1024, 1) k_bgzf_scan(JobBufs jb, BgzfJob bj)
     for (uint32_t j = beg; j < end; j++) {
         const uint32_t i = bj.morder ? bj.morder[j] : j;
         bj.mout[i] = off;
-        const uint32_t hl = bj.flushed ? flush_header_len(bj.wrap, i) : member_header_len(bj.wrap_of(i), bj.fdict);
+        const uint32_t hl = bj.flushed ? flush_header_len(bj.wrap, i) : member_header_len(bj.wrap_of(i), bj.fdict_of(i));
         if (!bj.mstored[i]) {
             const uint32_t nb = bj.minfo[i].n_blocks;
             for (uint32_t k = 0; k < nb; k++) jb.blocks[bj.slot0(i) + k].bit_base += 8ull * (off + hl);
@@ -266,21 +268,23 @@ __global__ void __launch_bounds__(256) k_bgzf_frame(JobBufs jb, BgzfJob bj)
         }
         return;
     }
-    const uint32_t wrap = bj.wrap_of(m), hl = member_header_len(wrap, bj.fdict);
+    const uint32_t wrap = bj.wrap_of(m), hl = member_header_len(wrap, bj.fdict_of(m));
     if (tid == 0) {
         if (wrap == kWrapBgzf) bgzf_header(o, bytes);
         else if (bj.mp) { // the item's own framing (zb_bgzf.h)
             const MemberParams &mp = bj.mp[m];
             stream_header(o, wrap, mp.lflags, mp.cinfo, mp.xfl);
-        } else stream_header(o, wrap, zlib_level_flags(jb.level, false), 7, gzip_xfl((int)jb.level, 0), bj.fdict != 0,
-                             bj.fdict ? *bj.dictid : 0u);
+        } else {
+            const bool fd = bj.fdict_of(m);
+            stream_header(o, wrap, zlib_level_flags(jb.level, false), 7, gzip_xfl((int)jb.level, 0), fd, fd ? bj.dictid_of(m) : 0u);
+        }
         const uint32_t tw = wrap == kWrapBgzf ? 2u : wrap; // BGZF's trailer is gzip's
         stream_trailer(o + bytes - member_trailer_len(wrap), tw, wrap == 2 && bj.mcrc ? bj.mcrc[m] : bj.mcheck[m], len);
     }
     if (stored) {
         const uint32_t nb = (uint32_t)stored_blocks(len);
         if (tid < nb) stored_header(o + hl + tid * (kStoredMax + 5), min(kStoredMax, len - tid * kStoredMax), tid + 1 == nb);
-        const uint8_t *src = jb.in + bj.moff[m] + bj.pstart; // the item's bytes only
+        const uint8_t *src = jb.in + bj.moff[m] + bj.pstart_of(m); // the item's bytes only
         for (uint32_t i = tid; i < len; i += 256) o[hl + 5 * (i / kStoredMax + 1) + i] = src[i];
     }
 }

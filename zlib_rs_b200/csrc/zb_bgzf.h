@@ -23,9 +23,14 @@
 // Batch with a preset dictionary (zb_deflate_batch_dict, DESIGN.md §2j).  Item i becomes what the reference writes after
 // deflateSetDictionary(dict): the single-stream rule of a dictionary (Engine::deflate) applied to every member.  The window holds
 // D' bytes of the dictionary (all of it, or its last 32 KiB when it is 64 KiB or longer, deflate.rs:517-531), so member m is staged
-// as D' ++ item and its parse starts at the parse start D' (BgzfJob::pstart, one value per call).  A zlib item gets the 6-byte
-// header with FDICT and DICTID (adler32 of the whole dictionary) whenever D' > 0; its trailer and checks[i] cover the item alone.
-// Level 0 writes stored blocks of the item bytes only (a dictionary does not enter stored blocks).
+// as D' ++ item and its parse starts at the parse start D' (BgzfJob::pstart_of).  A zlib item gets the 6-byte header with FDICT
+// and DICTID (adler32 of the whole dictionary) whenever D' > 0; its trailer and checks[i] cover the item alone.  Level 0 writes
+// stored blocks of the item bytes only (a dictionary does not enter stored blocks).
+//
+// Batch with a dictionary per item (zb_deflate_batch_dicts, DESIGN.md §2p).  The same rule with item i's own dictionary: member i is
+// staged as D'_i ++ item i and parsed from D'_i, its own prefix length (batch_dicts_layout below).  Nothing in the member's parse
+// depends on what its neighbours are staged behind: every argument below is made in the member's own coordinates, so it holds
+// with a prefix of any length.  zb_deflate_batch_dict is the case of a one-dictionary table that every item names.
 //
 // Staging.  Member m is staged at moff[m] of the engine's input buffer with at least kMemberGap zero bytes behind it: BGZF at
 // m * kBgzfStride, a batch packed by batch_stage_next() (with a dictionary, the member is its dictionary copy and the item).  The link kernels of the single-stream path run over the whole staged
@@ -108,6 +113,40 @@ ZB_HD uint64_t batch_stage_next(uint64_t off, uint64_t len) { return (off + len 
 // stored + framing, which this covers for every memLevel.  With a dictionary the zlib header grows by the 4 bytes of DICTID: the 18 +
 // 64 bytes of slack beyond stored + 6 + 4 still cover it, so zb_deflate_batch_bound bounds zb_deflate_batch_dict too.
 ZB_HD uint64_t stream_bound(uint64_t n) { return n + ((n + 7) >> 3) + ((n + 63) >> 6) + 5 + 18 + 64; }
+
+// Batches with preset dictionaries (zb_deflate_batch_dict, zb_deflate_batch_dicts).  The window's part D' of a dictionary: all of
+// it, or its last w_size bytes when it is 64 KiB or longer (deflate.rs:517-531).
+constexpr uint32_t kDictNone = 0xffffffffu;  // ZB_DICT_NONE: the item has no dictionary (or, in mdx, no FDICT)
+constexpr uint32_t kDictById = 0xfffffffeu;  // ZB_DICT_BY_ID (inflate): the dictionary a zlib item's DICTID names
+constexpr uint64_t kBatchMaxDicts = 65535;   // dictionaries of a deflate call
+ZB_HD uint32_t dict_prefix_len(uint64_t dict_len) { return dict_len >= 2 * (uint64_t)kWSize ? kWSize : (uint32_t)dict_len; }
+// The staging of a batch with a dictionary per item, which the engine and tests/batchdictsmodel share.  Item i names dictionary
+// which[i] of the table dict_off (n_dicts + 1 offsets; which == nullptr: every item names dictionary 0; kDictNone: none) and is
+// staged at moff[i] as its dictionary's last mps[i] = D'_i bytes, which start at dict_off[0] + mdsrc[i] of the table, followed by
+// the item.  mdx[i] is the dictionary whose adler32 is the item's DICTID, or kDictNone when its header has no FDICT (raw items,
+// D' = 0).  The caller has checked which[] against n_dicts.  Returns the staged span: every member 64-byte aligned with at least
+// kMemberGap zero bytes behind it (batch_stage_next over D'_i + len_i).
+ZB_HD uint64_t batch_dicts_layout(const uint64_t *src_off, uint32_t n, const uint64_t *dict_off, const uint32_t *which, uint32_t wrap,
+                                  uint64_t *moff, uint32_t *mps, uint64_t *mdsrc, uint32_t *mdx)
+{
+    uint64_t span = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        const uint32_t j = which ? which[i] : 0u;
+        uint32_t D = 0;
+        uint64_t from = 0;
+        if (j != kDictNone) {
+            const uint64_t dl = dict_off[j + 1] - dict_off[j];
+            D = dict_prefix_len(dl);
+            from = dict_off[j] + dl - D - dict_off[0];
+        }
+        moff[i] = span;
+        mps[i] = D;
+        mdsrc[i] = from;
+        mdx[i] = wrap == 1 && D > 0 ? j : kDictNone; // FDICT whenever the dictionary put bytes in the window (deflate.rs:1578-1581)
+        span = batch_stage_next(span, D + (src_off[i + 1] - src_off[i]));
+    }
+    return span;
+}
 
 // Member m of a staged input, in its own coordinates: position y reads in[moff[m] + y].  Behind the member's `n` bytes it
 // reads what the reference's window buffer holds behind a one-shot input of n bytes (zeros up to 64 KiB, then the bytes one window

@@ -75,7 +75,7 @@ __global__ void k_bgzf_size(JobBufs, BgzfJob);
 __global__ void k_bgzf_scan(JobBufs, BgzfJob);
 __global__ void k_bgzf_encode(JobBufs, BgzfJob);
 __global__ void k_bgzf_frame(JobBufs, BgzfJob);
-__global__ void k_batch_stage(const uint8_t *, const uint64_t *, const uint8_t *, BgzfJob, uint8_t *, uint64_t);
+__global__ void k_batch_stage(const uint8_t *, const uint64_t *, const uint8_t *, const uint64_t *, BgzfJob, uint8_t *, uint64_t);
 __global__ void k_batch_dict_ghost(JobBufs, BgzfJob);
 __global__ void k_flush_blocks(JobBufs, BgzfJob);
 __global__ void k_deflate_points(JobBufs, BgzfJob, IdxWriteJob); // zb_deflate_index (zb_kernels.cu)
@@ -748,8 +748,8 @@ int Engine::members_alloc(JobBufs &jb, BgzfJob &bj, uint32_t nm, uint32_t S, siz
     uint8_t *t = static_cast<uint8_t *>(p);
     bj.nm = nm;
     bj.wrap = wrap;
-    bj.pstart = 0;
-    bj.fdict = 0;
+    bj.mps = nullptr;
+    bj.mdx = nullptr;
     bj.dictid = nullptr;
     bj.flushed = 0;
     bj.fcheck = nullptr;
@@ -769,8 +769,9 @@ int Engine::members_alloc(JobBufs &jb, BgzfJob &bj, uint32_t nm, uint32_t S, siz
     return ZB_OK;
 }
 
-// ... and its launches behind the staging: links, parse, blocks, sizes and offsets, encoding, framing.
-int Engine::members_launch(JobBufs &jb, BgzfJob &bj, int level, uint32_t *d_freq)
+// ... and its launches behind the staging: links, parse, blocks, sizes and offsets, encoding, framing.  `ghost`: some member is
+// staged behind at least 3 dictionary bytes (k_batch_dict_ghost).
+int Engine::members_launch(JobBufs &jb, BgzfJob &bj, int level, uint32_t *d_freq, bool ghost)
 {
     const uint32_t nm = bj.nm, S = jb.N, nmt = S / kLinkTile + 1;
     const bool links = level >= 3, slow = level >= 7;
@@ -782,7 +783,7 @@ int Engine::members_launch(JobBufs &jb, BgzfJob &bj, int level, uint32_t *d_freq
             } else {
                 k_links2_std<<<nmt, 1024, kLinks2SmemBytes, st>>>(jb, 0);
                 k_links_fix_std<<<S / 256 + 1, 256, 0, st>>>(jb);
-                if (bj.pstart >= 3) { k_batch_dict_ghost<<<nm, 256, 0, st>>>(jb, bj); launches++; } // zb_bgzf.cu
+                if (ghost) { k_batch_dict_ghost<<<nm, 256, 0, st>>>(jb, bj); launches++; } // zb_bgzf.cu
             }
             launches += 2;
         }
@@ -904,56 +905,108 @@ int Engine::deflate_bgzf(const void *src, size_t n, bool src_dev, void *dst, siz
 // zb_deflate_batch (zb_bgzf.h, DESIGN.md §2i): item i is deflated alone and framed as its own zlib / gzip / raw stream, byte for
 // byte what zb_deflate gives for it.  The items are packed into the staged buffer by the host's member table and go through the
 // member core of BGZF; a call costs a fixed number of launches and two host syncs whatever the number and lengths of its items.
-// With a preset dictionary (zb_deflate_batch_dict, DESIGN.md §2j) every item is staged behind its own copy of the dictionary's
-// window bytes and parsed from there: item i is what deflateSetDictionary(dict) + deflate(Z_FINISH) writes for it.  `dict` is
-// nullptr for zb_deflate_batch.
-int Engine::deflate_batch(const void *dict, size_t dict_len, const void *src, const uint64_t *src_off, size_t n_items, bool src_dev,
-                          void *dst, size_t dst_cap, bool dst_dev, int level, int strategy, int window_bits, uint32_t flags,
-                          uint64_t *dst_off, uint32_t *checks, zb_deflate_result *res)
+// With preset dictionaries (zb_deflate_batch_dict, DESIGN.md §2j; zb_deflate_batch_dicts, §2p) every item is staged behind its own
+// copy of its dictionary's window bytes and parsed from there: item i is what deflateSetDictionary(its dictionary) +
+// deflate(Z_FINISH) writes for it.  The shared dictionary of zb_deflate_batch_dict is a table of one that every item names.
+int Engine::deflate_batch(const DictTable &dt, const void *src, const uint64_t *src_off, size_t n_items, bool src_dev, void *dst,
+                          size_t dst_cap, bool dst_dev, int level, int strategy, int window_bits, uint32_t flags, uint64_t *dst_off,
+                          uint32_t *checks, zb_deflate_result *res)
 {
-    if (!res || !dst_off || (n_items && (!src_off || !dst))) { snprintf(g_err, sizeof g_err, "deflate_batch: null argument"); return ZB_E_PARAM; }
+    const bool per_item = dt.kind == DictTable::kPerItem, with_dict = dt.kind != DictTable::kNone;
+    // the names in the messages: the shared-dictionary call keeps its own
+    const char *gn = per_item ? "deflate_batch_dicts" : "deflate_batch", *dn = per_item ? "deflate_batch_dicts" : "deflate_batch_dict";
+    if (!res || !dst_off || (n_items && (!src_off || !dst))) { snprintf(g_err, sizeof g_err, "%s: null argument", gn); return ZB_E_PARAM; }
     memset(res, 0, sizeof *res);
-    const bool with_dict = dict != nullptr || dict_len != 0;
     const uint32_t ml = (flags >> 8) & 15u;
     uint32_t wrap;
     if (window_bits == 15) wrap = 1;
     else if (window_bits == 31 && !with_dict) wrap = 2;
     else if (window_bits == -15) wrap = 0;
-    else if (window_bits == 31) { snprintf(g_err, sizeof g_err, "deflate_batch_dict: a gzip stream takes no dictionary"); return ZB_E_PARAM; }
+    else if (window_bits == 31) { snprintf(g_err, sizeof g_err, "%s: a gzip stream takes no dictionary", dn); return ZB_E_PARAM; }
+    else if (per_item) { snprintf(g_err, sizeof g_err, "deflate_batch_dicts takes window_bits 15 or -15"); return ZB_E_PARAM; }
     else { snprintf(g_err, sizeof g_err, "deflate_batch takes window_bits 15, -15 or 31"); return ZB_E_PARAM; }
     if ((flags & ~ZB_FLAG_MEMLEVEL(15)) || (ml && ml != 8) || strategy != 0 || level < -1 || level > 9) {
-        snprintf(g_err, sizeof g_err, "deflate_batch takes Z_DEFAULT_STRATEGY, level -1..9, memLevel 8 and no flag");
+        snprintf(g_err, sizeof g_err, "%s takes Z_DEFAULT_STRATEGY, level -1..9, memLevel 8 and no flag", gn);
         return ZB_E_PARAM;
     }
     if (with_dict && (level == 1 || level == 2)) {
         // the one-warp parsers of levels 1/2 take no dictionary (zb_deflate_dict runs the level-3 kernels there, not the reference's
         // bytes); a batch returns the reference's bytes or nothing
-        snprintf(g_err, sizeof g_err, "deflate_batch_dict: levels 1 and 2 have no exact parser with a dictionary (use 0 or 3..9)");
+        snprintf(g_err, sizeof g_err, "%s: levels 1 and 2 have no exact parser with a dictionary (use 0 or 3..9)", dn);
         return ZB_E_PARAM;
     }
-    if (with_dict && !dict) { snprintf(g_err, sizeof g_err, "deflate_batch_dict: null dictionary of %zu bytes", dict_len); return ZB_E_PARAM; }
-    if (dict_len > 0xffffffffull) { snprintf(g_err, sizeof g_err, "deflate_batch_dict: dictionary of 4 GiB or more"); return ZB_E_PARAM; }
-    // the window's part of the dictionary (deflate.rs:517-531): all of it, or its last w_size bytes when it would fill the window
-    const uint32_t D = dict_len >= 2 * (size_t)kWSize ? kWSize : (uint32_t)dict_len;
-    if (n_items > kBatchMaxItems) { snprintf(g_err, sizeof g_err, "deflate_batch: %zu items (at most %llu)", n_items, (unsigned long long)kBatchMaxItems); return ZB_E_PARAM; }
-    // the member table, on the host: items at 64-byte aligned staged offsets, each behind its dictionary copy, with a zero gap behind
+    const uint32_t nd = (uint32_t)dt.n;
+    uint64_t dict_bytes = 0;
+    if (dt.kind == DictTable::kShared) {
+        dict_bytes = dt.off[1] - dt.off[0];
+        if (dict_bytes > 0xffffffffull) { snprintf(g_err, sizeof g_err, "deflate_batch_dict: dictionary of 4 GiB or more"); return ZB_E_PARAM; }
+    } else if (per_item) {
+        if (n_items && (!dt.off || !dt.which)) { snprintf(g_err, sizeof g_err, "deflate_batch_dicts: null dictionary table"); return ZB_E_PARAM; }
+        if (dt.n > kBatchMaxDicts) { snprintf(g_err, sizeof g_err, "deflate_batch_dicts: %zu dictionaries (at most %llu)", dt.n, (unsigned long long)kBatchMaxDicts); return ZB_E_PARAM; }
+        for (uint32_t j = 0; j < nd; j++)
+            if (dt.off[j + 1] < dt.off[j]) { snprintf(g_err, sizeof g_err, "deflate_batch_dicts: offsets of dictionary %u decrease", j); return ZB_E_PARAM; }
+        dict_bytes = nd ? dt.off[nd] - dt.off[0] : 0;
+        if (dict_bytes > kBatchMaxBytes) { snprintf(g_err, sizeof g_err, "deflate_batch_dicts: %llu dictionary bytes (at most 2^31)", (unsigned long long)dict_bytes); return ZB_E_PARAM; }
+        if (dict_bytes && !dt.data) { snprintf(g_err, sizeof g_err, "deflate_batch_dicts: null dictionaries of %llu bytes", (unsigned long long)dict_bytes); return ZB_E_PARAM; }
+        for (size_t i = 0; i < n_items; i++)
+            if (dt.which[i] >= nd && dt.which[i] != kDictNone) {
+                snprintf(g_err, sizeof g_err, "deflate_batch_dicts: item %zu names dictionary 0x%x (%u dictionaries; ZB_DICT_BY_ID is for inflate)",
+                         i, dt.which[i], nd);
+                return ZB_E_PARAM;
+            }
+    }
+    if (n_items > kBatchMaxItems) { snprintf(g_err, sizeof g_err, "%s: %zu items (at most %llu)", gn, n_items, (unsigned long long)kBatchMaxItems); return ZB_E_PARAM; }
     const uint32_t nm = (uint32_t)n_items;
-    uint64_t span = 0, bound = 0;
+    uint64_t bound = 0;
     for (uint32_t i = 0; i < nm; i++) {
         if (src_off[i + 1] < src_off[i] || src_off[i + 1] - src_off[i] > kMemberMax) {
-            snprintf(g_err, sizeof g_err, "deflate_batch: item %u is not 0..%u bytes", i, kMemberMax);
+            snprintf(g_err, sizeof g_err, "%s: item %u is not 0..%u bytes", gn, i, kMemberMax);
             return ZB_E_PARAM;
         }
-        span = batch_stage_next(span, D + (src_off[i + 1] - src_off[i]));
         bound += stream_bound(src_off[i + 1] - src_off[i]);
     }
     const uint64_t total = nm ? src_off[nm] - src_off[0] : 0;
-    if (total > kBatchMaxBytes) { snprintf(g_err, sizeof g_err, "deflate_batch: %llu bytes in all (at most 2^31)", (unsigned long long)total); return ZB_E_PARAM; }
-    if (D && span > kBatchMaxBytes) {
-        snprintf(g_err, sizeof g_err, "deflate_batch_dict: %llu staged bytes with the dictionary copies (at most 2^31)", (unsigned long long)span);
+    if (total > kBatchMaxBytes) { snprintf(g_err, sizeof g_err, "%s: %llu bytes in all (at most 2^31)", gn, (unsigned long long)total); return ZB_E_PARAM; }
+    // pinned staging: up the member table (moff | mlen | src_off; with dictionaries mps | mdx | mdsrc | the items' start | the
+    // dictionaries' offsets and lengths), down the control block, offsets and checks
+    const size_t t_dict = with_dict ? (size_t)nm * (4 + 4 + 8 + 8) + ((size_t)nd + 1) * 8 + (size_t)nd * 4 + 64 : 0;
+    const size_t t_up = (size_t)nm * 8 + (size_t)nm * 4 + ((size_t)nm + 1) * 8 + t_dict, t_down = sizeof(BgzfCtl) + (size_t)nm * 12 + 16;
+    int rc;
+    if ((rc = stage(t_up + t_down + 64)) != ZB_OK) return rc;
+    uint8_t *h = static_cast<uint8_t *>(h_stage);
+    uint64_t *h_moff = reinterpret_cast<uint64_t *>(h);
+    uint32_t *h_mlen = reinterpret_cast<uint32_t *>(h + (size_t)nm * 8);
+    uint64_t *h_soff = reinterpret_cast<uint64_t *>(h + (size_t)nm * 12);
+    uint64_t *h_mdsrc = h_soff + nm + 1, *h_mitem = h_mdsrc + nm, *h_doff = h_mitem + nm; // with dictionaries
+    uint32_t *h_mps = reinterpret_cast<uint32_t *>(h_doff + nd + 1), *h_mdx = h_mps + nm, *h_dlen = h_mdx + nm;
+    BgzfCtl *h_ctl = reinterpret_cast<BgzfCtl *>(h + ((t_up + 15) & ~(size_t)15));
+    uint64_t *h_mout = reinterpret_cast<uint64_t *>(h_ctl + 1);
+    uint32_t *h_chk = reinterpret_cast<uint32_t *>(h_mout + nm);
+    // the member table: items at 64-byte aligned staged offsets, each behind its dictionary copy, with a zero gap behind
+    uint64_t span = 0;
+    uint32_t maxD = 0;
+    bool fdict = false;
+    if (with_dict) {
+        span = batch_dicts_layout(src_off, nm, dt.off, dt.which, wrap, h_moff, h_mps, h_mdsrc, h_mdx);
+        for (uint32_t i = 0; i < nm; i++) {
+            maxD = std::max(maxD, h_mps[i]);
+            fdict |= h_mdx[i] != kDictNone;
+            h_mitem[i] = h_moff[i] + h_mps[i];
+        }
+        for (uint32_t j = 0; j <= nd; j++) h_doff[j] = dt.off[j] - dt.off[0];
+        for (uint32_t j = 0; j < nd; j++) h_dlen[j] = (uint32_t)(dt.off[j + 1] - dt.off[j]);
+    } else {
+        for (uint32_t i = 0; i < nm; i++) {
+            h_moff[i] = span;
+            span = batch_stage_next(span, src_off[i + 1] - src_off[i]);
+        }
+    }
+    for (uint32_t i = 0; i < nm; i++) h_mlen[i] = (uint32_t)(src_off[i + 1] - src_off[i]);
+    if (maxD && span > kBatchMaxBytes) {
+        snprintf(g_err, sizeof g_err, "%s: %llu staged bytes with the dictionary copies (at most 2^31)", dn, (unsigned long long)span);
         return ZB_E_PARAM;
     }
-    if (total && !src) { snprintf(g_err, sizeof g_err, "deflate_batch: null source"); return ZB_E_PARAM; }
+    if (total && !src) { snprintf(g_err, sizeof g_err, "%s: null source", gn); return ZB_E_PARAM; }
     if (level == -1) level = 6;
     res->exact_parity = 1;
     res->bits_used = 8;
@@ -966,71 +1019,69 @@ int Engine::deflate_batch(const void *dict, size_t dict_len, const void *src, co
     JobBufs jb;
     BgzfJob bj;
     uint32_t *d_freq;
-    int rc;
     if ((rc = members_reserve(jb, bj, nm, S, span, level, out_cap, wrap, &d_freq)) != ZB_OK) return rc;
-    bj.pstart = D;
-    bj.fdict = wrap == 1 && D > 0; // FDICT whenever the dictionary put bytes in the window (deflate.rs:1578-1581)
-    // pinned staging: the member table up (moff | mlen | src_off | the dictionary's offset and length for its adler32), the control
-    // block, offsets and checks down
-    const size_t t_up = (size_t)nm * 8 + (size_t)nm * 4 + ((size_t)nm + 1) * 8 + 16, t_down = sizeof(BgzfCtl) + (size_t)nm * 12 + 16;
-    if ((rc = stage(t_up + t_down + 64)) != ZB_OK) return rc;
-    uint8_t *h = static_cast<uint8_t *>(h_stage);
-    uint64_t *h_moff = reinterpret_cast<uint64_t *>(h);
-    uint32_t *h_mlen = reinterpret_cast<uint32_t *>(h + (size_t)nm * 8);
-    uint64_t *h_soff = reinterpret_cast<uint64_t *>(h + (size_t)nm * 12);
-    uint64_t *h_dseg = h_soff + nm + 1; // offset 0, then the dictionary's length
-    BgzfCtl *h_ctl = reinterpret_cast<BgzfCtl *>(h + ((t_up + 15) & ~(size_t)15));
-    uint64_t *h_mout = reinterpret_cast<uint64_t *>(h_ctl + 1);
-    uint32_t *h_chk = reinterpret_cast<uint32_t *>(h_mout + nm);
-    uint64_t off = 0;
-    for (uint32_t i = 0; i < nm; i++) {
-        h_moff[i] = off;
-        h_mlen[i] = (uint32_t)(src_off[i + 1] - src_off[i]);
-        off = batch_stage_next(off, D + h_mlen[i]);
-    }
     memcpy(h_soff, src_off, ((size_t)nm + 1) * 8);
-    h_dseg[0] = 0;
-    h_dseg[1] = dict_len;
-    // S_BATCH: the caller's offsets | the dictionary segment (offset, length, its adler32) | a host dictionary | a host source
-    const size_t a_soff = ((((size_t)nm + 1) * 8 + 63) & ~(size_t)63), a_dseg = 64;
-    const size_t a_dict = src_dev ? 0 : ((dict_len + 63) & ~(size_t)63);
+    // S_BATCH: the caller's offsets | with dictionaries: mdsrc | the items' start | the dictionaries' offsets | mps | mdx | the
+    // dictionaries' lengths | their adler32 | a host copy of the dictionaries | a host source
+    auto al = [](size_t b) { return (b + 63) & ~(size_t)63; };
+    const size_t a_soff = al(((size_t)nm + 1) * 8);
+    const size_t a_tab = with_dict ? 2 * al((size_t)nm * 8) + al(((size_t)nd + 1) * 8) + 2 * al((size_t)nm * 4) + 2 * al((size_t)nd * 4) : 0;
+    const size_t a_dict = src_dev ? 0 : al(dict_bytes);
     void *p;
-    if ((rc = reserve(S_BATCH, a_soff + a_dseg + a_dict + (src_dev ? 0 : total), &p)) != ZB_OK) return rc;
+    if ((rc = reserve(S_BATCH, a_soff + a_tab + a_dict + (src_dev ? 0 : total), &p)) != ZB_OK) return rc;
     uint8_t *t = static_cast<uint8_t *>(p);
     uint64_t *d_soff = reinterpret_cast<uint64_t *>(t);
-    uint64_t *d_dseg = reinterpret_cast<uint64_t *>(t + a_soff);
-    uint32_t *d_dictid = reinterpret_cast<uint32_t *>(t + a_soff + 32);
-    const uint8_t *d_dict = src_dev ? static_cast<const uint8_t *>(dict) : t + a_soff + a_dseg;
-    const uint8_t *d_src = src_dev ? static_cast<const uint8_t *>(src) + src_off[0] : t + a_soff + a_dseg + a_dict;
+    uint64_t *d_mdsrc = reinterpret_cast<uint64_t *>(t + a_soff), *d_mitem = reinterpret_cast<uint64_t *>(t + a_soff + al((size_t)nm * 8));
+    uint64_t *d_doff = reinterpret_cast<uint64_t *>(t + a_soff + 2 * al((size_t)nm * 8));
+    uint32_t *d_mps = reinterpret_cast<uint32_t *>(reinterpret_cast<uint8_t *>(d_doff) + al(((size_t)nd + 1) * 8));
+    uint32_t *d_mdx = reinterpret_cast<uint32_t *>(reinterpret_cast<uint8_t *>(d_mps) + al((size_t)nm * 4));
+    uint32_t *d_dlen = reinterpret_cast<uint32_t *>(reinterpret_cast<uint8_t *>(d_mdx) + al((size_t)nm * 4));
+    uint32_t *d_dictid = reinterpret_cast<uint32_t *>(reinterpret_cast<uint8_t *>(d_dlen) + al((size_t)nd * 4));
+    const uint8_t *d_dict = !with_dict ? nullptr
+                            : src_dev ? static_cast<const uint8_t *>(dt.data) + dt.off[0] : t + a_soff + a_tab;
+    const uint8_t *d_src = src_dev ? static_cast<const uint8_t *>(src) + src_off[0] : t + a_soff + a_tab + a_dict;
     const size_t mi_bytes = ((size_t)nm * sizeof(JobInfo) + 15) & ~(size_t)15;
-    bj.dictid = d_dictid;
+    if (with_dict) {
+        bj.mps = d_mps;
+        bj.mdx = d_mdx;
+        bj.dictid = d_dictid;
+    }
 
     CK(cudaEventRecord(ev0, st));
     CK(cudaMemcpyAsync(bj.moff, h_moff, (size_t)nm * 8, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(bj.mlen, h_mlen, (size_t)nm * 4, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_soff, h_soff, ((size_t)nm + 1) * 8, cudaMemcpyHostToDevice, st));
-    if (bj.fdict) CK(cudaMemcpyAsync(d_dseg, h_dseg, 16, cudaMemcpyHostToDevice, st));
-    // staging: one contiguous copy of a host source (and dictionary), then every item to its staged offset behind its dictionary copy,
-    // with the gap behind it zeroed
-    if (!src_dev && dict_len) CK(cudaMemcpyAsync(const_cast<uint8_t *>(d_dict), dict, dict_len, cudaMemcpyHostToDevice, st));
+    if (with_dict) {
+        CK(cudaMemcpyAsync(d_mdsrc, h_mdsrc, (size_t)nm * 8, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(d_mps, h_mps, (size_t)nm * 4, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(d_mdx, h_mdx, (size_t)nm * 4, cudaMemcpyHostToDevice, st));
+        if (wrap == 1) CK(cudaMemcpyAsync(d_mitem, h_mitem, (size_t)nm * 8, cudaMemcpyHostToDevice, st));
+        if (fdict) {
+            CK(cudaMemcpyAsync(d_doff, h_doff, ((size_t)nd + 1) * 8, cudaMemcpyHostToDevice, st));
+            CK(cudaMemcpyAsync(d_dlen, h_dlen, (size_t)nd * 4, cudaMemcpyHostToDevice, st));
+        }
+    }
+    // staging: one contiguous copy of a host source (and of the dictionaries), then every item to its staged offset behind its
+    // dictionary copy, with the gap behind it zeroed
+    if (!src_dev && dict_bytes)
+        CK(cudaMemcpyAsync(const_cast<uint8_t *>(d_dict), static_cast<const uint8_t *>(dt.data) + dt.off[0], dict_bytes, cudaMemcpyHostToDevice, st));
     if (!src_dev && total) CK(cudaMemcpyAsync(const_cast<uint8_t *>(d_src), static_cast<const uint8_t *>(src) + src_off[0], total, cudaMemcpyHostToDevice, st));
-    k_batch_stage<<<nm, 256, 0, st>>>(d_src, d_soff, D ? d_dict + (dict_len - D) : nullptr, bj, const_cast<uint8_t *>(jb.in), span);
+    k_batch_stage<<<nm, 256, 0, st>>>(d_src, d_soff, d_dict, with_dict ? d_mdsrc : nullptr, bj, const_cast<uint8_t *>(jb.in), span);
     CK(cudaMemsetAsync(const_cast<uint8_t *>(jb.in) + span, 0, kPad + 16, st));
     CK(cudaMemsetAsync(bj.minfo, 0, mi_bytes + sizeof(BgzfCtl), st));
     CK(cudaMemsetAsync(jb.out, 0, out_cap, st));
     launches++;
     // the items' checks, as zb_deflate returns them (the item's bytes only, behind its dictionary copy), and DICTID: the adler32 of
-    // the whole dictionary as passed (deflate.rs:507-510)
-    if (wrap == 1) CK(launch_adler32_segments(jb.in + D, bj.moff, bj.mlen, nm, bj.mcheck, st));
+    // every whole dictionary as passed (deflate.rs:507-510), one segment each
+    if (wrap == 1) CK(launch_adler32_segments(jb.in, with_dict ? d_mitem : bj.moff, bj.mlen, nm, bj.mcheck, st));
     else if (wrap == 2) CK(launch_crc32_segments(jb.in, bj.moff, bj.mlen, nm, bj.mcheck, st));
     else CK(cudaMemsetAsync(bj.mcheck, 0, (size_t)nm * 4, st));
     if (wrap) launches++;
-    if (bj.fdict) {
-        // one segment: [0, dict_len) of the dictionary, its length as a 32-bit word (the low half of h_dseg[1], little-endian)
-        CK(launch_adler32_segments(d_dict, d_dseg, reinterpret_cast<const uint32_t *>(d_dseg + 1), 1, d_dictid, st));
+    if (fdict) {
+        CK(launch_adler32_segments(d_dict, d_doff, d_dlen, nd, d_dictid, st));
         launches++;
     }
-    if ((rc = members_launch(jb, bj, level, d_freq)) != ZB_OK) return rc;
+    if ((rc = members_launch(jb, bj, level, d_freq, maxD >= 3)) != ZB_OK) return rc;
     CK(cudaMemcpyAsync(h_ctl, bj.ctl, sizeof(BgzfCtl), cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(h_mout, bj.mout, (size_t)nm * 8, cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(h_chk, bj.mcheck, (size_t)nm * 4, cudaMemcpyDeviceToHost, st));
@@ -1173,7 +1224,7 @@ int Engine::deflate_batch_params(const void *src, const uint64_t *src_off, size_
     if (any_g) CK(cudaMemcpyAsync(d_lg, h_lg, (size_t)nm * 4, cudaMemcpyHostToDevice, st));
     if (!src_dev && total) CK(cudaMemcpyAsync(const_cast<uint8_t *>(d_src), static_cast<const uint8_t *>(src) + src_off[0], total, cudaMemcpyHostToDevice, st));
     // k_batch_stage reads member m at src + (soff[m] - soff[0]): shift the source so that this is the item's caller offset
-    k_batch_stage<<<nm, 256, 0, st>>>(d_src + (h_soff[0] - src_off[0]), d_soff, nullptr, bj, const_cast<uint8_t *>(jb.in), span);
+    k_batch_stage<<<nm, 256, 0, st>>>(d_src + (h_soff[0] - src_off[0]), d_soff, nullptr, nullptr, bj, const_cast<uint8_t *>(jb.in), span);
     CK(cudaMemsetAsync(const_cast<uint8_t *>(jb.in) + span, 0, kPad + 16, st));
     CK(cudaMemsetAsync(bj.minfo, 0, mi_bytes + sizeof(BgzfCtl), st));
     CK(cudaMemsetAsync(jb.out, 0, out_cap, st));
@@ -1371,7 +1422,7 @@ int Engine::deflate_flushed(const void *src, const uint64_t *seg_off, size_t n_s
     CK(cudaMemcpyAsync(d_soff, h_soff, ((size_t)nm + 1) * 8, cudaMemcpyHostToDevice, st));
     if (!src_dev) CK(cudaMemcpyAsync(const_cast<uint8_t *>(d_src), static_cast<const uint8_t *>(src) + seg_off[0], total, cudaMemcpyHostToDevice, st));
     // staging: every segment at its offset with zeros behind it, as a batch item (zb_bgzf.h: the bytes behind a segment do not matter)
-    k_batch_stage<<<nm, 256, 0, st>>>(d_src, d_soff, nullptr, bj, const_cast<uint8_t *>(jb.in), span);
+    k_batch_stage<<<nm, 256, 0, st>>>(d_src, d_soff, nullptr, nullptr, bj, const_cast<uint8_t *>(jb.in), span);
     CK(cudaMemsetAsync(const_cast<uint8_t *>(jb.in) + span, 0, kPad + 16, st));
     launches++;
     CK(cudaMemsetAsync(bj.minfo, 0, mi_bytes + sizeof(BgzfCtl), st));
@@ -1557,8 +1608,21 @@ int zb_deflate_batch_dict(zb_engine *z, const void *dict, size_t dict_len, const
     z->e.shard.phase = 0; // a range job in progress is gone (its buffers are reused)
     // an empty dictionary still makes this the dictionary call (its rules on levels and framing), with the bytes of zb_deflate_batch
     static const uint8_t none = 0;
-    return z->e.deflate_batch(dict ? dict : &none, dict_len, src, src_off, n_items, src_dev != 0, dst, cap, dst_dev != 0, level, strategy,
-                              window_bits, flags, dst_off, checks, res);
+    const uint64_t off[2] = {0, dict_len};
+    zb::Engine::DictTable dt{zb::Engine::DictTable::kShared, dict ? dict : &none, off, 1, nullptr};
+    return z->e.deflate_batch(dt, src, src_off, n_items, src_dev != 0, dst, cap, dst_dev != 0, level, strategy, window_bits, flags, dst_off,
+                              checks, res);
+}
+
+int zb_deflate_batch_dicts(zb_engine *z, const void *dicts, const uint64_t *dict_off, size_t n_dicts, const uint32_t *which, const void *src,
+                           const uint64_t *src_off, size_t n_items, int src_dev, void *dst, size_t cap, int dst_dev, int level, int strategy,
+                           int window_bits, uint32_t flags, uint64_t *dst_off, uint32_t *checks, zb_deflate_result *res)
+{
+    if (!z) return ZB_E_NODEVICE;
+    z->e.shard.phase = 0; // a range job in progress is gone (its buffers are reused)
+    zb::Engine::DictTable dt{zb::Engine::DictTable::kPerItem, dicts, dict_off, n_dicts, which};
+    return z->e.deflate_batch(dt, src, src_off, n_items, src_dev != 0, dst, cap, dst_dev != 0, level, strategy, window_bits, flags, dst_off,
+                              checks, res);
 }
 
 int zb_deflate_batch(zb_engine *z, const void *src, const uint64_t *src_off, size_t n_items, int src_dev, void *dst, size_t cap,
@@ -1567,8 +1631,8 @@ int zb_deflate_batch(zb_engine *z, const void *src, const uint64_t *src_off, siz
 {
     if (!z) return ZB_E_NODEVICE;
     z->e.shard.phase = 0; // a range job in progress is gone (its buffers are reused)
-    return z->e.deflate_batch(nullptr, 0, src, src_off, n_items, src_dev != 0, dst, cap, dst_dev != 0, level, strategy, window_bits, flags,
-                              dst_off, checks, res);
+    return z->e.deflate_batch(zb::Engine::DictTable{}, src, src_off, n_items, src_dev != 0, dst, cap, dst_dev != 0, level, strategy,
+                              window_bits, flags, dst_off, checks, res);
 }
 
 int zb_deflate_flushed(zb_engine *z, const void *src, const uint64_t *seg_off, size_t n_segs, int src_dev, void *dst, size_t cap,
@@ -1609,8 +1673,19 @@ int zb_inflate_batch_dict(zb_engine *z, const void *dict, size_t dict_len, const
     if (!dict && dict_len) { snprintf(zb::g_err, sizeof zb::g_err, "inflate_batch_dict: null dictionary of %zu bytes", dict_len); return ZB_E_PARAM; }
     z->e.shard.phase = 0; // a range job in progress is gone (its buffers are reused)
     static const uint8_t none = 0; // an empty dictionary (id 1) is still a dictionary
-    return z->e.inflate_batch(dict ? dict : &none, dict_len, src, src_off, n_items, src_dev != 0, dst, dst_off, dst_dev != 0, window_bits,
-                              items);
+    const uint64_t off[2] = {0, dict_len};
+    zb::Engine::DictTable dt{zb::Engine::DictTable::kShared, dict ? dict : &none, off, 1, nullptr};
+    return z->e.inflate_batch(dt, src, src_off, n_items, src_dev != 0, dst, dst_off, dst_dev != 0, window_bits, items);
+}
+
+int zb_inflate_batch_dicts(zb_engine *z, const void *dicts, const uint64_t *dict_off, size_t n_dicts, const uint32_t *which, const void *src,
+                           const uint64_t *src_off, size_t n_items, int src_dev, void *dst, const uint64_t *dst_off, int dst_dev,
+                           int window_bits, zb_inflate_result *items)
+{
+    if (!z) return ZB_E_NODEVICE;
+    z->e.shard.phase = 0; // a range job in progress is gone (its buffers are reused)
+    zb::Engine::DictTable dt{zb::Engine::DictTable::kPerItem, dicts, dict_off, n_dicts, which};
+    return z->e.inflate_batch(dt, src, src_off, n_items, src_dev != 0, dst, dst_off, dst_dev != 0, window_bits, items);
 }
 
 int zb_inflate_batch(zb_engine *z, const void *src, const uint64_t *src_off, size_t n_items, int src_dev, void *dst, const uint64_t *dst_off,
@@ -1618,7 +1693,7 @@ int zb_inflate_batch(zb_engine *z, const void *src, const uint64_t *src_off, siz
 {
     if (!z) return ZB_E_NODEVICE;
     z->e.shard.phase = 0; // a range job in progress is gone (its buffers are reused)
-    return z->e.inflate_batch(nullptr, 0, src, src_off, n_items, src_dev != 0, dst, dst_off, dst_dev != 0, window_bits, items);
+    return z->e.inflate_batch(zb::Engine::DictTable{}, src, src_off, n_items, src_dev != 0, dst, dst_off, dst_dev != 0, window_bits, items);
 }
 
 int zb_inflate_flushed(zb_engine *z, const void *src, size_t src_len, int src_dev, const uint64_t *restart, size_t n_segs, const uint32_t *which,

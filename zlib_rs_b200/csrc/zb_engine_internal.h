@@ -101,7 +101,16 @@ struct Engine {
     int deflate_bgzf(const void *src, size_t n, bool src_dev, void *dst, size_t dst_cap, bool dst_dev, int level, zb_deflate_result *res,
                      IdxWrite *iw = nullptr);
     int index_written(const JobBufs &jb, const BgzfJob &bj, const IdxWriteJob &w, const IdxHeader &h, IdxWrite *iw);
-    int deflate_batch(const void *dict, size_t dict_len, const void *src, const uint64_t *src_off, size_t n_items, bool src_dev, void *dst,
+    // the dictionary table of a batch call: none (zb_deflate_batch / zb_inflate_batch), one that every item names
+    // (zb_*_batch_dict, which == nullptr) or one named item by item (zb_*_batch_dicts)
+    struct DictTable {
+        enum Kind { kNone, kShared, kPerItem } kind = kNone;
+        const void *data = nullptr;
+        const uint64_t *off = nullptr; // n + 1 offsets into data
+        size_t n = 0;
+        const uint32_t *which = nullptr;
+    };
+    int deflate_batch(const DictTable &dt, const void *src, const uint64_t *src_off, size_t n_items, bool src_dev, void *dst,
                       size_t dst_cap, bool dst_dev, int level, int strategy, int window_bits, uint32_t flags, uint64_t *dst_off,
                       uint32_t *checks, zb_deflate_result *res);
     int deflate_flushed(const void *src, const uint64_t *seg_off, size_t n_segs, bool src_dev, void *dst, size_t dst_cap, bool dst_dev,
@@ -110,7 +119,7 @@ struct Engine {
                         size_t n_which, void *dst, const uint64_t *dst_off, bool dst_dev, int window_bits, zb_inflate_result *items);
     int members_reserve(JobBufs &jb, BgzfJob &bj, uint32_t nm, uint32_t S, size_t span, int level, size_t out_cap, uint32_t wrap,
                         uint32_t **d_freq);
-    int members_launch(JobBufs &jb, BgzfJob &bj, int level, uint32_t *d_freq);
+    int members_launch(JobBufs &jb, BgzfJob &bj, int level, uint32_t *d_freq, bool ghost = false);
     int members_alloc(JobBufs &jb, BgzfJob &bj, uint32_t nm, uint32_t S, size_t span, size_t out_cap, uint32_t wrap, uint32_t nslots,
                       bool parse, bool links, bool slow, uint32_t **d_freq);
     int members_blocks(JobBufs &jb, BgzfJob &bj, bool blocks, uint32_t nslots, uint32_t *d_freq);
@@ -129,7 +138,7 @@ struct Engine {
     int index_bgzf(const void *src, size_t n, bool src_dev, zb_inflate_result *res, zb_index *x);
     int index_extract(const zb_index *x, const void *src, size_t src_len, bool src_dev, const uint64_t *offsets, size_t n_ranges,
                       void *dst, const uint64_t *dst_off, bool dst_dev, zb_inflate_result *items);
-    int inflate_batch(const void *dict, size_t dict_len, const void *src, const uint64_t *src_off, size_t n_items, bool src_dev, void *dst,
+    int inflate_batch(const DictTable &dt, const void *src, const uint64_t *src_off, size_t n_items, bool src_dev, void *dst,
                       const uint64_t *dst_off, bool dst_dev, int window_bits, zb_inflate_result *items);
     int inflate_blocks(const void *src, size_t n, uint64_t start_bit, const void *dict, size_t dict_len, void *dst, size_t dst_cap,
                        int check_kind, uint32_t check_start, zb_inflate_seg *out);

@@ -1480,13 +1480,54 @@ struct BatchResult {   // what comes back to the host per item
     uint32_t check, err; // err: InfErr, IE_OUTPUT_FULL is ZB_E_BUF
 };
 
+// The dictionaries of a batch (zb_inflate_batch_dict: one that every item names; zb_inflate_batch_dicts: a table named item by
+// item).  Dictionary j is data[off[j], off[j+1]) and id[j] its adler32; item i names which[i] (which == nullptr: `all` for every
+// item), an index, kDictById or kDictNone.  n = 0: no dictionary (zb_inflate_batch).
+struct InfDicts {
+    const uint8_t *data;
+    const uint64_t *off;
+    const uint32_t *id;
+    const uint32_t *which;
+    uint32_t n, all;
+};
+
+// kDictById: the dictionary an item's zlib header names, read by the whole warp before the decoder starts.  The decoder reads
+// DICTID at bytes 2..5 exactly when the stream is not raw, its first two bytes are not gzip's magic under auto-detection, gzip
+// alone is not asked for, and FDICT is set; otherwise it never looks at the dictionary, and no dictionary is as good as any.  The
+// lowest index whose adler32 is DICTID wins (a ballot per 32 ids; the scan stops at the first hit).  None: kDictNone, "need
+// dictionary".  A header cut inside its DICTID gets a dictionary too (the first), so it fails as truncated, as it does with any.
+__device__ __forceinline__ uint32_t dict_by_id(const InfDicts &dt, const uint8_t *src, uint64_t n, int window_bits)
+{
+    if (window_bits < 0 || n < 2 || (window_bits > 15 && window_bits < 32)) return kDictNone;
+    const uint32_t h = (uint32_t)src[0] | ((uint32_t)src[1] << 8);
+    if ((window_bits > 15 && h == 0x8b1f) || !(h & 0x2000)) return kDictNone;
+    if (n < 6) return 0;
+    const uint32_t want = ((uint32_t)src[2] << 24) | ((uint32_t)src[3] << 16) | ((uint32_t)src[4] << 8) | src[5];
+    for (uint32_t b = 0; b < dt.n; b += 32) {
+        const uint32_t j = b + threadIdx.x;
+        const uint32_t hit = __ballot_sync(0xffffffffu, j < dt.n && dt.id[j] == want);
+        if (hit) return b + __ffs(hit) - 1;
+    }
+    return kDictNone;
+}
+
 __global__ void __launch_bounds__(32) k_batch_members(const uint8_t *__restrict__ src, const BatchItem *items, uint8_t *__restrict__ dst,
                                                       int window_bits, InfState *ist, uint64_t *out_off, uint32_t *crc_len,
-                                                      uint32_t *adler_len, InfDict pd)
+                                                      uint32_t *adler_len, InfDicts dt)
 {
     extern __shared__ __align__(16) uint8_t smem_raw[];
     const uint32_t i = blockIdx.x;
     const BatchItem it = items[i];
+    InfDict pd{nullptr, nullptr, 0, 0};
+    if (dt.n) {
+        uint32_t j = dt.which ? dt.which[i] : dt.all;
+        if (j == kDictById) j = dict_by_id(dt, src + it.in_off, it.in_len, window_bits);
+        if (j < dt.n) {
+            const uint64_t b = dt.off[j], len = dt.off[j + 1] - b;
+            const uint32_t w = len > kWSize ? kWSize : (uint32_t)len; // the window keeps the dictionary's last 32 KiB
+            pd = InfDict{dt.data + b + (len - w), dt.id + j, w, 1};
+        }
+    }
     inflate_warp(*reinterpret_cast<InfShared *>(smem_raw), src + it.in_off, it.in_len, dst + it.out_off, it.out_cap, window_bits, ist + i,
                  InfSeg{0, nullptr, 0, 0}, pd);
     __syncwarp();
@@ -1931,14 +1972,35 @@ int Engine::inflate_stream(const uint8_t *d_src, size_t n, uint8_t *d_dst, size_
 }
 
 // zb_inflate_batch: item i of src[src_off[i], src_off[i+1]) into dst[dst_off[i], dst_off[i+1]), each as zb_inflate_ex decodes it
-// alone.  Fixed launches (k_batch_members, the two checksum kernels, k_batch_verdict) and one host sync.  With a preset dictionary
-// (zb_inflate_batch_dict, `dict` not nullptr) one more launch gives its adler32, the id an FDICT header must name; the decoder
-// preloads the dictionary's last 32 KiB as the window of the raw items and of the zlib items that name it.
-int Engine::inflate_batch(const void *dict, size_t dict_len, const void *src, const uint64_t *src_off, size_t n_items, bool src_dev,
-                          void *dst, const uint64_t *dst_off, bool dst_dev, int window_bits, zb_inflate_result *items)
+// alone.  Fixed launches (k_batch_members, the two checksum kernels, k_batch_verdict) and one host sync.  With preset dictionaries
+// (zb_inflate_batch_dict: one that every item names; zb_inflate_batch_dicts: a table named item by item, DESIGN.md §2p) one more
+// launch gives the adler32 of every dictionary, the ids an FDICT header must name; the decoder preloads the last 32 KiB of the
+// item's dictionary as the window of a raw item and of a zlib item that names it.
+int Engine::inflate_batch(const DictTable &dt, const void *src, const uint64_t *src_off, size_t n_items, bool src_dev, void *dst,
+                          const uint64_t *dst_off, bool dst_dev, int window_bits, zb_inflate_result *items)
 {
-    if (n_items && (!src_off || !dst_off || !items)) { snprintf(g_err, sizeof g_err, "inflate_batch: null argument"); return ZB_E_PARAM; }
-    if (dict_len > 0xffffffffull) { snprintf(g_err, sizeof g_err, "inflate_batch_dict: dictionary of 4 GiB or more"); return ZB_E_PARAM; }
+    const bool per_item = dt.kind == DictTable::kPerItem;
+    const char *gn = per_item ? "inflate_batch_dicts" : "inflate_batch";
+    if (n_items && (!src_off || !dst_off || !items)) { snprintf(g_err, sizeof g_err, "%s: null argument", gn); return ZB_E_PARAM; }
+    const uint32_t nd = (uint32_t)dt.n;
+    uint64_t dict_bytes = 0;
+    if (dt.kind == DictTable::kShared) {
+        dict_bytes = dt.off[1] - dt.off[0];
+        if (dict_bytes > 0xffffffffull) { snprintf(g_err, sizeof g_err, "inflate_batch_dict: dictionary of 4 GiB or more"); return ZB_E_PARAM; }
+    } else if (per_item) {
+        if (dt.n && !dt.off) { snprintf(g_err, sizeof g_err, "inflate_batch_dicts: null dictionary table"); return ZB_E_PARAM; }
+        if (dt.n > kBatchMaxInflateItems) { snprintf(g_err, sizeof g_err, "inflate_batch_dicts: %zu dictionaries (at most 2^20)", dt.n); return ZB_E_PARAM; }
+        for (uint32_t j = 0; j < nd; j++)
+            if (dt.off[j + 1] < dt.off[j]) { snprintf(g_err, sizeof g_err, "inflate_batch_dicts: offsets of dictionary %u decrease", j); return ZB_E_PARAM; }
+        dict_bytes = nd ? dt.off[nd] - dt.off[0] : 0;
+        if (dict_bytes > kBatchMaxBytes) { snprintf(g_err, sizeof g_err, "inflate_batch_dicts: %llu dictionary bytes (at most 2^31)", (unsigned long long)dict_bytes); return ZB_E_PARAM; }
+        if (dict_bytes && !dt.data) { snprintf(g_err, sizeof g_err, "inflate_batch_dicts: null dictionaries of %llu bytes", (unsigned long long)dict_bytes); return ZB_E_PARAM; }
+        for (size_t i = 0; dt.which && i < n_items; i++)
+            if (dt.which[i] >= nd && dt.which[i] != kDictNone && dt.which[i] != kDictById) {
+                snprintf(g_err, sizeof g_err, "inflate_batch_dicts: item %zu names dictionary %u of %u", i, dt.which[i], nd);
+                return ZB_E_PARAM;
+            }
+    }
     if (window_bits < 0) { if (window_bits < -15 || window_bits > -8) return ZB_E_PARAM; }
     else if (window_bits != 0 && ((window_bits & 15) < 8)) return ZB_E_PARAM;
     if (window_bits > 47) return ZB_E_PARAM;
@@ -1962,9 +2024,12 @@ int Engine::inflate_batch(const void *dict, size_t dict_len, const void *src, co
     // S_BATCH: item table | results | output offsets | the two checksum length tables and their checks | decoder states
     const size_t a_items = ((size_t)nm * sizeof(BatchItem) + 63) & ~(size_t)63, a_res = ((size_t)nm * sizeof(BatchResult) + 63) & ~(size_t)63;
     const size_t a4 = ((size_t)nm * 4 + 63) & ~(size_t)63, a8 = ((size_t)nm * 8 + 63) & ~(size_t)63;
-    // ... | the dictionary segment (offset, length, id) | a host dictionary
-    const size_t a_ist = ((size_t)nm * sizeof(InfState) + 63) & ~(size_t)63, a_dict = (dict && !src_dev) ? ((dict_len + 63) & ~(size_t)63) : 0;
-    if ((rc = reserve(S_BATCH, a_items + a_res + a8 + 4 * a4 + a_ist + 64 + a_dict, &p)) != ZB_OK) return rc;
+    // ... | the dictionaries' offsets (n_dicts + 1), lengths and ids | the items' dictionaries | a host copy of the dictionaries
+    const bool with_dict = dt.kind != DictTable::kNone && nd > 0, item_which = with_dict && per_item && dt.which;
+    const size_t a_ist = ((size_t)nm * sizeof(InfState) + 63) & ~(size_t)63;
+    const size_t a_doff = with_dict ? (((size_t)nd + 1) * 8 + 63) & ~(size_t)63 : 0, a_d4 = with_dict ? ((size_t)nd * 4 + 63) & ~(size_t)63 : 0;
+    const size_t a_which = item_which ? a4 : 0, a_dict = (with_dict && !src_dev) ? ((dict_bytes + 63) & ~(size_t)63) : 0;
+    if ((rc = reserve(S_BATCH, a_items + a_res + a8 + 4 * a4 + a_ist + a_doff + 2 * a_d4 + a_which + a_dict, &p)) != ZB_OK) return rc;
     uint8_t *t = static_cast<uint8_t *>(p);
     BatchItem *d_items = reinterpret_cast<BatchItem *>(t);
     BatchResult *d_res = reinterpret_cast<BatchResult *>(t + a_items);
@@ -1972,15 +2037,21 @@ int Engine::inflate_batch(const void *dict, size_t dict_len, const void *src, co
     uint32_t *d_clen = reinterpret_cast<uint32_t *>(t + a_items + a_res + a8), *d_alen = d_clen + a4 / 4;
     uint32_t *d_crc = d_alen + a4 / 4, *d_adler = d_crc + a4 / 4;
     InfState *d_ist = reinterpret_cast<InfState *>(d_adler + a4 / 4);
-    uint64_t *d_dseg = reinterpret_cast<uint64_t *>(reinterpret_cast<uint8_t *>(d_ist) + a_ist);
-    uint32_t *d_dictid = reinterpret_cast<uint32_t *>(d_dseg + 2);
-    const uint8_t *d_dict = src_dev ? static_cast<const uint8_t *>(dict) : reinterpret_cast<const uint8_t *>(d_dseg) + 64;
-    if ((rc = stage(a_items + a_res + 64 + 16)) != ZB_OK) return rc;
+    uint64_t *d_doff = reinterpret_cast<uint64_t *>(reinterpret_cast<uint8_t *>(d_ist) + a_ist);
+    uint32_t *d_dlen = reinterpret_cast<uint32_t *>(reinterpret_cast<uint8_t *>(d_doff) + a_doff), *d_dictid = d_dlen + a_d4 / 4;
+    uint32_t *d_which = d_dictid + a_d4 / 4;
+    const uint8_t *d_dict = !with_dict ? nullptr
+                            : src_dev ? static_cast<const uint8_t *>(dt.data) + dt.off[0] : reinterpret_cast<const uint8_t *>(d_which) + a_which;
+    if ((rc = stage(a_items + a_res + 64 + a_doff + 2 * a_d4 + a_which)) != ZB_OK) return rc;
     BatchItem *h_items = static_cast<BatchItem *>(h_stage);
     BatchResult *h_res = reinterpret_cast<BatchResult *>(static_cast<uint8_t *>(h_stage) + a_items);
-    uint64_t *h_dseg = reinterpret_cast<uint64_t *>(static_cast<uint8_t *>(h_stage) + a_items + a_res + 64);
-    h_dseg[0] = 0;
-    h_dseg[1] = dict_len;
+    uint64_t *h_doff = reinterpret_cast<uint64_t *>(static_cast<uint8_t *>(h_stage) + a_items + a_res + 64);
+    uint32_t *h_dlen = reinterpret_cast<uint32_t *>(reinterpret_cast<uint8_t *>(h_doff) + a_doff), *h_which = h_dlen + 2 * (a_d4 / 4);
+    if (with_dict) {
+        for (uint32_t j = 0; j <= nd; j++) h_doff[j] = dt.off[j] - dt.off[0];
+        for (uint32_t j = 0; j < nd; j++) h_dlen[j] = (uint32_t)(dt.off[j + 1] - dt.off[j]);
+        if (item_which) memcpy(h_which, dt.which, (size_t)nm * 4);
+    }
     for (uint32_t i = 0; i < nm; i++)
         h_items[i] = BatchItem{src_off[i] - src_off[0], src_off[i + 1] - src_off[i], dst_off[i] - dst_off[0], dst_off[i + 1] - dst_off[i]};
     // the item offsets index the caller's buffers: a host buffer is copied (or staged) as one range
@@ -1998,17 +2069,19 @@ int Engine::inflate_batch(const void *dict, size_t dict_len, const void *src, co
         CKI(cudaMemsetAsync(d_dst, 0, out_total, st)); // the slots go back whole: what lies behind an item's output is zeros
     }
     CKI(cudaMemcpyAsync(d_items, h_items, (size_t)nm * sizeof(BatchItem), cudaMemcpyHostToDevice, st));
-    InfDict pd{nullptr, nullptr, 0, 0};
-    if (dict) {
-        // the dictionary's id: the adler32 of all of it (an empty one has id 1), as inflateSetDictionary checks it
-        CKI(cudaMemcpyAsync(d_dseg, h_dseg, 16, cudaMemcpyHostToDevice, st));
-        if (!src_dev && dict_len) CKI(cudaMemcpyAsync(const_cast<uint8_t *>(d_dict), dict, dict_len, cudaMemcpyHostToDevice, st));
-        CKI(launch_adler32_segments(d_dict, d_dseg, reinterpret_cast<const uint32_t *>(d_dseg + 1), 1, d_dictid, st));
+    InfDicts idt{nullptr, nullptr, nullptr, nullptr, 0, 0};
+    if (with_dict) {
+        // the dictionaries' ids: the adler32 of each whole dictionary (an empty one has id 1), as inflateSetDictionary checks it
+        CKI(cudaMemcpyAsync(d_doff, h_doff, a_doff + a_d4, cudaMemcpyHostToDevice, st));
+        if (item_which) CKI(cudaMemcpyAsync(d_which, h_which, (size_t)nm * 4, cudaMemcpyHostToDevice, st));
+        if (!src_dev && dict_bytes)
+            CKI(cudaMemcpyAsync(const_cast<uint8_t *>(d_dict), static_cast<const uint8_t *>(dt.data) + dt.off[0], dict_bytes,
+                                cudaMemcpyHostToDevice, st));
+        CKI(launch_adler32_segments(d_dict, d_doff, d_dlen, nd, d_dictid, st));
         launches++;
-        const uint32_t w = dict_len > kWSize ? kWSize : (uint32_t)dict_len; // the window keeps the dictionary's last 32 KiB
-        pd = InfDict{d_dict + (dict_len - w), d_dictid, w, 1};
+        idt = InfDicts{d_dict, d_doff, d_dictid, item_which ? d_which : nullptr, nd, per_item ? kDictById : 0u};
     }
-    k_batch_members<<<nm, 32, sizeof(InfShared), st>>>(d_src, d_items, d_dst, window_bits, d_ist, d_ooff, d_clen, d_alen, pd);
+    k_batch_members<<<nm, 32, sizeof(InfShared), st>>>(d_src, d_items, d_dst, window_bits, d_ist, d_ooff, d_clen, d_alen, idt);
     CKI(launch_crc32_segments(d_dst, d_ooff, d_clen, nm, d_crc, st));
     CKI(launch_adler32_segments(d_dst, d_ooff, d_alen, nm, d_adler, st));
     k_batch_verdict<<<(nm + 255) / 256, 256, 0, st>>>(d_ist, d_crc, d_adler, nm, d_res);

@@ -1860,7 +1860,7 @@ __global__ void __launch_bounds__(256) k_bgzf_hist(JobBufs jb, BgzfJob bj, uint3
     const JobInfo &mi = bj.minfo[m];
     const uint32_t nsyms = mi.n_syms, nblocks = mi.n_blocks;
     if (k >= nblocks) return;
-    const uint32_t base = (uint32_t)bj.moff[m], len = bj.pstart + bj.mlen[m]; // the member's end: dictionary and item
+    const uint32_t base = (uint32_t)bj.moff[m], p0 = bj.pstart_of(m), len = p0 + bj.mlen[m]; // the member's end: dictionary and item
     const Sym *syms = jb.syms + base;
     const uint32_t bs = bj.mp ? bj.mp[m].bs : jb.block_syms;
     const uint32_t begin = k * bs;
@@ -1872,7 +1872,7 @@ __global__ void __launch_bounds__(256) k_bgzf_hist(JobBufs jb, BgzfJob bj, uint3
         bd.sym_begin = base + begin;
         bd.sym_count = count;
         bd.last = last && (!bj.flushed || m + 1 == bj.nm); // a segment of a flushed stream ends its stream only if it is the last
-        const uint32_t start = begin == 0 ? bj.pstart : sym_end(syms[begin - 1]);
+        const uint32_t start = begin == 0 ? p0 : sym_end(syms[begin - 1]);
         const uint32_t end = last ? len : sym_end(syms[begin + count - 1]);
         bd.in_start = base + start;
         bd.in_len = end - start;

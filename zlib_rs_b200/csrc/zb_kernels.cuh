@@ -139,10 +139,12 @@ struct BgzfJob {
     uint32_t *mstored;  // 1: written as stored blocks (level 0, or a BGZF payload that does not fit 64 KiB)
     JobInfo *minfo;     // n_syms, n_blocks and final_base of its parse, as a single-stream parse reports them
     BgzfCtl *ctl;
-    uint32_t pstart;    // parse start of every member: the dictionary's bytes D' staged in front of each item (0: none)
-    uint32_t fdict;     // zlib items get FDICT and DICTID = *dictid (a batch with a preset dictionary)
-    const uint32_t *dictid;
-    uint32_t flushed;   // 1: the members are the segments of one stream written with Z_FULL_FLUSH (zb_deflate_flushed): `wrap`
+    // batches with preset dictionaries (zb_deflate_batch_dict / _dicts, zb_bgzf.h batch_dicts_layout); all nullptr for the other
+    // member calls, whose members start parsing at 0 and have no FDICT
+    const uint32_t *mps;    // member m's parse start: its dictionary's bytes D' staged in front of the item
+    const uint32_t *mdx;    // the dictionary whose adler32 is member m's DICTID, or kDictNone (no FDICT)
+    const uint32_t *dictid; // adler32 of every dictionary of the table
+    uint32_t flushed;  // 1: the members are the segments of one stream written with Z_FULL_FLUSH (zb_deflate_flushed): `wrap`
                         // frames the stream, member 0 has the header, the last the trailer, every other one the empty stored block
     uint32_t *fcheck;   // flushed: the check of the whole input, joined from mcheck
     uint32_t isize;     // flushed: the input length mod 2^32 (gzip's ISIZE)
@@ -155,6 +157,9 @@ struct BgzfJob {
     ZB_HD uint32_t slot0(uint32_t m) const { return mslot ? mslot[m] : m * kBgzfMaxBlocks; }
     ZB_HD uint32_t nslots(uint32_t m) const { return mslot ? mslot[m + 1] - mslot[m] : kBgzfMaxBlocks; }
     ZB_HD uint32_t wrap_of(uint32_t m) const { return mp ? mp[m].wrap : wrap; }
+    ZB_HD uint32_t pstart_of(uint32_t m) const { return mps ? mps[m] : 0u; }
+    ZB_HD bool fdict_of(uint32_t m) const { return mdx && mdx[m] != kDictNone; }
+    ZB_HD uint32_t dictid_of(uint32_t m) const { return dictid[mdx[m]]; } // fdict_of(m) only
     // the member and block of block slot b
     ZB_HD void slot_member(uint32_t b, uint32_t &m, uint32_t &k) const
     {
