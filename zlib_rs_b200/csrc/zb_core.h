@@ -134,6 +134,25 @@ ZB_HD uint32_t wbase_w(const WN &wn, uint32_t p) { return p <= wn.t0() ? 0u : wn
 // fill_window check (deflate.rs:1776-1806): slides happen at the first loop-top beyond base+65274.
 ZB_HD uint32_t wbase(uint32_t p) { return p <= kT0 ? 0u : kWSize * (1u + (p - kT0 - 1u) / kWSize); }
 
+// The link of position i with the holes bridged (what k_skip stores in Lr[i]): the distance to the nearest predecessor of i on
+// its hash chain that is not a hole, or 0 when the chain ends, or that predecessor lies more than md back, before one is found.
+// L[i] itself is kept when it is 0 or leads to a position that is not a hole (i itself may be a hole: k_match starts walks there).
+// Only positions from i - md to i are read.  A walk that would cross more than max_hops holes stops with kBridgeUnbounded.
+constexpr uint32_t kBridgeUnbounded = 0xffffffffu;
+ZB_HD uint32_t bridged_link(const uint16_t *L, const uint32_t *holes, uint32_t i, uint32_t md, uint32_t max_hops = 0xffffffffu)
+{
+    uint32_t d = L[i];
+    for (uint32_t hops = 0;; hops++) {
+        if (d == 0 || d > i) return d; // no predecessor, or one before the first position of L
+        const uint32_t t = i - d;
+        if (!((holes[t >> 5] >> (t & 31)) & 1u)) return d;
+        if (hops == max_hops) return kBridgeUnbounded;
+        const uint32_t d2 = L[t];
+        if (d2 == 0 || d + d2 > md) return 0;
+        d += d2;
+    }
+}
+
 // ---------------------------------------------------------------------------------------------
 // Accessor concept used by the templates below:
 //   uint32_t byte(uint32_t y)   : window byte at absolute position y (stale bytes beyond N allowed)

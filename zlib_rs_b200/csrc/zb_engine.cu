@@ -31,7 +31,8 @@ static void set_err(const char *what, cudaError_t e)
 
 // kernels (zb_kernels.cu)
 __global__ void k_match(JobBufs);
-__global__ void k_skip(JobBufs);
+__global__ void k_skip(JobBufs, uint32_t);
+__global__ void k_skip_walk(JobBufs);
 __global__ void k_nxt(JobBufs);
 __global__ void k_path_tiles(JobBufs);
 __global__ void k_path_chain(JobBufs, uint32_t, uint32_t);
@@ -84,6 +85,7 @@ constexpr uint32_t kMatchSmemBytes = (kWSize + kMatchSub + 512) + (kWSize + kMat
 constexpr uint32_t kPathSmemBytes = kPathTile * 4 * 3;
 constexpr uint32_t kLinks2SmemBytes = 65536 * 2 + kLinkTile * 2 + kLinkTile + 64 + 2048;
 constexpr uint32_t kSkipSmemBytes = 2 * kWSize * 2 + 2 * (2 * kWSize / 32) * 4 + 8192 + 64; // links, hole + bucket-flag bitmaps, bucket map
+constexpr uint32_t kSkipWalkSmemBytes = (kWSize + kSkipSlice) * 2 + (kWSize + kSkipSlice) / 32 * 4 + 8192; // links, holes, bucket map
 constexpr uint32_t kSlowSubMax = 24576;
 constexpr uint32_t kSlowSmemBytes = (kWSize + kSlowSubMax + kSlowAhead) * 3;
 constexpr uint32_t kChainSmemBytes = kChainChunkTiles * kPathHead * 8;
@@ -113,6 +115,7 @@ int Engine::init(int dev)
     CK(upload_tables());
     CK(cudaFuncSetAttribute(k_match, cudaFuncAttributeMaxDynamicSharedMemorySize, kMatchSmemBytes));
     CK(cudaFuncSetAttribute(k_skip, cudaFuncAttributeMaxDynamicSharedMemorySize, kSkipSmemBytes));
+    CK(cudaFuncSetAttribute(k_skip_walk, cudaFuncAttributeMaxDynamicSharedMemorySize, kSkipWalkSmemBytes));
     CK(cudaFuncSetAttribute(k_links2_std, cudaFuncAttributeMaxDynamicSharedMemorySize, kLinks2SmemBytes));
     CK(cudaFuncSetAttribute(k_links2_roll, cudaFuncAttributeMaxDynamicSharedMemorySize, kLinks2SmemBytes));
     CK(cudaFuncSetAttribute(k_slow, cudaFuncAttributeMaxDynamicSharedMemorySize, kSlowSmemBytes));
@@ -286,7 +289,8 @@ int Engine::deflate(const void *src, size_t n_in, bool src_dev, void *dst, size_
     const uint32_t nlists = npt * (kPathTile / kPathSub);
     RES(S_LLIST, (size_t)nlists * kLongPerSub * 4, long_list, uint32_t *)
     RES(S_LCNT, (size_t)nlists * 4, long_cnt, uint32_t *)
-    RES(S_TDIRTY, (size_t)nmt + 16, tile_dirty, uint8_t *)
+    RES(S_TDIRTY, 2 * ((size_t)nmt + 16), tile_dirty, uint8_t *)
+    jb.skip_fall = jb.tile_dirty + nmt + 16; // the second half: k_skip_walk's per-tile flags
     RES(S_SYMS, ((size_t)N + 64) * sizeof(Sym), syms, Sym *)
     RES(S_SYMB, 40000 * 4, sym_base, uint32_t *)
     RES(S_BMAP, (size_t)nmt * 8192, bucket_map, uint32_t *) // one 65536-bit map per 32 KiB tile
@@ -484,6 +488,7 @@ int Engine::deflate(const void *src, size_t n_in, bool src_dev, void *dst, size_
             CK(cudaMemsetAsync(jb.holes, 0, (size_t)nwords * 4, st));
             CK(cudaMemsetAsync(jb.holes_new, 0, (size_t)nwords * 4, st));
             CK(cudaMemsetAsync(jb.tile_dirty, 1, nmt, st));
+            CK(cudaMemsetAsync(jb.skip_fall, 0, nmt, st));
             CK(cudaMemsetAsync(jb.tile_entry, 0xee, (size_t)npt * 4, st)); // "never seen": forces the first marking
             CK(cudaMemsetAsync(jb.M + N, 0, (size_t)kPad * 4, st));
             CK(cudaMemsetAsync(jb.L + N, 0, (size_t)kPad * 2, st));
@@ -562,11 +567,17 @@ int Engine::deflate(const void *src, size_t n_in, bool src_dev, void *dst, size_
                         n_ptiles = h_info->n_ptiles ? h_info->n_ptiles : 1;
                         first_ptile = h_info->first_ptile;
                         nsub = (n_dirty ? n_dirty : 1) * (kMatchTile / jb.match_sub);
-                        if (n_dirty) {
+                        if (n_dirty > kSkipWalkTiles) {
                             pbegin();
-                            k_skip<<<n_dirty, 1024, kSkipSmemBytes, st>>>(jb);
+                            k_skip<<<n_dirty, 1024, kSkipSmemBytes, st>>>(jb, 0);
                             pend(1, 1);
                             launches++;
+                        } else if (n_dirty) { // few tiles: one CTA per slice, k_skip only for the tiles whose walks gave up
+                            pbegin();
+                            k_skip_walk<<<n_dirty * (kMatchTile / kSkipSlice), 1024, kSkipWalkSmemBytes, st>>>(jb);
+                            k_skip<<<n_dirty, 1024, kSkipSmemBytes, st>>>(jb, 1);
+                            pend(1, 2);
+                            launches += 2;
                         }
                     }
                     // the dirty-bucket map and the changed-hole bitmaps are only staged from the second iteration on

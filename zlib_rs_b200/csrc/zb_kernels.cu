@@ -225,7 +225,7 @@ __global__ void __launch_bounds__(256) k_links_fix_roll(JobBufs jb) { links_fix_
 // partial jump along the same chain.
 // ------------------------------------------------------------------------------------------------
 constexpr uint32_t kSkipSpan = 2 * kWSize;
-__global__ void __launch_bounds__(1024) k_skip(JobBufs jb)
+__global__ void __launch_bounds__(1024) k_skip(JobBufs jb, uint32_t fallen_only)
 {
     extern __shared__ __align__(16) uint8_t smem[];
     uint16_t *sL = reinterpret_cast<uint16_t *>(smem);
@@ -235,6 +235,12 @@ __global__ void __launch_bounds__(1024) k_skip(JobBufs jb)
     const uint32_t tile = jb.skip_list ? jb.skip_list[blockIdx.x] : blockIdx.x;
     const uint32_t ts = tile * kMatchTile;
     if (ts >= jb.N) return;
+    if (fallen_only) { // after k_skip_walk: only the tiles one of whose walks gave up
+        const bool fell = jb.skip_fall[tile] != 0;
+        __syncthreads();
+        if (!fell) return;
+        if (threadIdx.x == 0) jb.skip_fall[tile] = 0;
+    }
     const uint32_t te = min(ts + kMatchTile, jb.N);
     const uint32_t ws = ts >= kWSize ? ts - kWSize : 0;
     const uint32_t span = te - ws, tid = threadIdx.x;
@@ -327,6 +333,50 @@ __global__ void __launch_bounds__(1024) k_skip(JobBufs jb)
         }
         jb.Lr[ws + i] = (uint16_t)d;
     }
+}
+
+// k_skip_walk: the same Lr entries as k_skip, for the later iterations, where a few dirty tiles would leave k_skip with one CTA
+// (latency-bound: its rounds cost the same at 2 tiles as at 14) on almost idle SMs.  Here every 4 KiB slice of a dirty tile has
+// its own CTA, which stages the links and holes of the slice and the 32 KiB before it and walks each in-play position of the
+// slice on its own with bridged_link() -- the value k_skip's sweep converges to (tests/test_skip_bridge_cpu.py).  A walk across
+// more than kSkipWalkHops holes (long runs of one byte) flags its tile, and k_skip, launched next over the same list, sweeps the
+// flagged tiles whole.
+__global__ void __launch_bounds__(1024) k_skip_walk(JobBufs jb)
+{
+    extern __shared__ __align__(16) uint8_t smem[];
+    constexpr uint32_t kSpan = kWSize + kSkipSlice;
+    uint16_t *sL = reinterpret_cast<uint16_t *>(smem);
+    uint32_t *sh = reinterpret_cast<uint32_t *>(smem + kSpan * 2);
+    uint32_t *sbm = sh + kSpan / 32;
+    __shared__ uint32_t s_fall;
+    const uint32_t tile = jb.skip_list[blockIdx.x / (kMatchTile / kSkipSlice)];
+    const uint32_t ts = tile * kMatchTile + (blockIdx.x % (kMatchTile / kSkipSlice)) * kSkipSlice;
+    if (ts >= jb.N) return;
+    const uint32_t te = min(ts + kSkipSlice, jb.N);
+    const uint32_t ws = ts >= kWSize ? ts - kWSize : 0; // a multiple of kSkipSlice: aligned for the 16-byte loads
+    const uint32_t span = te - ws, tid = threadIdx.x;
+    const uint32_t md = jb.wsize - kMinLookahead;
+    {
+        const uint4 *ls = reinterpret_cast<const uint4 *>(jb.L + ws);
+        uint4 *ld = reinterpret_cast<uint4 *>(sL);
+        for (uint32_t i = tid; i < (span + 7) / 8; i += 1024) ld[i] = ls[i];
+        for (uint32_t i = tid; i < (span + 31) / 32; i += 1024) sh[i] = jb.holes[(ws >> 5) + i];
+        const uint32_t *bm1 = jb.bucket_map + (size_t)tile * 2048, *bm0 = tile ? bm1 - 2048 : bm1;
+        for (uint32_t i = tid; i < 2048; i += 1024) sbm[i] = bm0[i] | bm1[i];
+        if (tid == 0) s_fall = 0;
+    }
+    __syncthreads();
+    bool fall = false;
+    for (uint32_t x = ts + tid; x < te; x += 1024) {
+        const uint32_t k = jb.keys[x];
+        if (!((sbm[k >> 5] >> (k & 31u)) & 1u)) continue; // its bucket is unchanged: Lr stands
+        const uint32_t v = bridged_link(sL, sh, x - ws, md, kSkipWalkHops);
+        if (v == kBridgeUnbounded) fall = true;
+        else jb.Lr[x] = (uint16_t)v;
+    }
+    if (fall) s_fall = 1;
+    __syncthreads();
+    if (tid == 0 && s_fall) jb.skip_fall[tile] = 1;
 }
 
 // ------------------------------------------------------------------------------------------------

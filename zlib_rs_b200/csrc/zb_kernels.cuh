@@ -24,6 +24,9 @@ constexpr uint32_t kNxtLong = 0x40000000u; // nxt flag: the macro step emits a m
 constexpr uint32_t kNxtLong258 = 0x20000000u; // ... and that match is 258 bytes long (levels 5/6: 257 otherwise)
 constexpr uint32_t kSymsPerThread = 16;
 constexpr uint32_t kSlowAhead = 1024;   // bytes/links staged behind the last position of a k_slow CTA (<= kPad)
+constexpr uint32_t kSkipSlice = 4096;    // output positions per k_skip_walk CTA
+constexpr uint32_t kSkipWalkHops = 256;  // holes one k_skip_walk walk may cross before its tile goes to k_skip's sweep
+constexpr uint32_t kSkipWalkTiles = 32;  // iterations with at most this many dirty tiles bridge by walks (k_skip_walk)
 
 // Explicit shared-space loads on 32-bit shared addresses (keeps address-space conversions out of the hot loops of k_match and
 // k_slow).
@@ -76,6 +79,7 @@ struct JobBufs {
     uint32_t *tile_entry; // path tiles: entry position (or 0xffffffff)
     uint32_t *tile_symbase;
     uint8_t *tile_dirty;  // match tiles
+    uint8_t *skip_fall;   // match tiles: a k_skip_walk walk hit kSkipWalkHops, k_skip sweeps the tile (and clears the flag)
     Sym *syms;            // N + 64
     uint32_t *sym_base;   // window base per symbol (tail symbols only; index relative to n_mid_syms)
     BlockDesc *blocks;
