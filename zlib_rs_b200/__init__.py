@@ -234,6 +234,40 @@ def _gather(items):
     return (ctypes.c_char * max(len(data), 1)).from_buffer_copy(data or b"\0"), _offsets([len(x) for x in items])
 
 
+def _items(items, src_on_device, src_off):
+    """(source pointer, offsets (n + 1), keep-alive) of batch items: a list of bytes-like objects gathered into one host buffer, or
+    a device pointer with `src_off`."""
+    if src_on_device:
+        return items, (ctypes.c_uint64 * len(src_off))(*src_off), None
+    keep, off = _gather(items)
+    return ctypes.addressof(keep), off, keep
+
+
+def _deflate_items(off, dst, dst_cap, dst_on_device, call):
+    """Runs a batch deflate `call(dst, dst_cap, dst_on_device, dst_off, checks, res)` into the caller's `dst`, or into a host buffer
+    of zb_deflate_batch_bound + 64 bytes.  Returns (list of bytes or None, offsets (n + 1), checks, DeflateResult); raises ZlibError
+    (.needed: the size a too small dst_cap would have to be)."""
+    n = len(off) - 1
+    res = DeflateResult()
+    own = None
+    if dst is None:
+        dst_cap = lib().zb_deflate_batch_bound(off, n) + 64
+        own = ctypes.create_string_buffer(dst_cap)
+        dst = ctypes.addressof(own)
+        dst_on_device = False
+    dst_off = (ctypes.c_uint64 * (n + 1))()
+    checks = (ctypes.c_uint32 * max(n, 1))()
+    rc = call(dst, dst_cap, int(dst_on_device), dst_off, checks, ctypes.byref(res))
+    if rc != 0:
+        e = ZlibError(rc, lib().zb_last_error().decode())
+        e.needed = res.out_bytes
+        raise e
+    offs = list(dst_off)
+    raw = own.raw if own is not None else None
+    outs = [raw[offs[i]:offs[i + 1]] for i in range(n)] if own is not None else None
+    return outs, offs, list(checks)[:n], res
+
+
 def _host_view(src):
     """(address, length, keep-alive) of a host buffer without copying it: bytes, or any writable contiguous buffer (bytearray,
     mmap, numpy array).  Other read-only buffers are copied once."""
@@ -625,39 +659,18 @@ class Engine:
         small dst_cap would have to be).
         With a `dictionary` (bytes-like, or (device pointer, length) with src_on_device) every item is deflated after
         deflateSetDictionary(dictionary) (zb_deflate_batch_dict): zlib items carry FDICT and its adler32 as DICTID."""
-        res = DeflateResult()
         flags |= (mem_level & 15) << 8
-        keep = None
-        if src_on_device:
-            off = (ctypes.c_uint64 * len(src_off))(*src_off)
-            src = items
-        else:
-            keep, off = _gather(items)
-            src = ctypes.addressof(keep)
+        src, off, keep = _items(items, src_on_device, src_off)
         n = len(off) - 1
-        own = None
-        if dst is None:
-            dst_cap = lib().zb_deflate_batch_bound(off, n) + 64
-            own = ctypes.create_string_buffer(dst_cap)
-            dst = ctypes.addressof(own)
-            dst_on_device = False
-        dst_off = (ctypes.c_uint64 * (n + 1))()
-        checks = (ctypes.c_uint32 * max(n, 1))()
-        args = (src, off, n, int(src_on_device), dst, dst_cap, int(dst_on_device), level, strategy, window_bits, flags, dst_off, checks,
-                ctypes.byref(res))
-        if dictionary is None:
-            rc = lib().zb_deflate_batch(self.h, *args)
-        else:
+
+        def call(dst, dst_cap, dst_on_device, dst_off, checks, res):
+            args = (src, off, n, int(src_on_device), dst, dst_cap, dst_on_device, level, strategy, window_bits, flags, dst_off, checks,
+                    res)
+            if dictionary is None:
+                return lib().zb_deflate_batch(self.h, *args)
             dptr, dlen, dkeep = _dictionary(dictionary, src_on_device)
-            rc = lib().zb_deflate_batch_dict(self.h, dptr, dlen, *args)
-        if rc != 0:
-            e = ZlibError(rc, lib().zb_last_error().decode())
-            e.needed = res.out_bytes
-            raise e
-        offs = list(dst_off)
-        raw = own.raw if own is not None else None
-        outs = [raw[offs[i]:offs[i + 1]] for i in range(n)] if own is not None else None
-        return outs, offs, list(checks)[:n], res
+            return lib().zb_deflate_batch_dict(self.h, dptr, dlen, *args)
+        return _deflate_items(off, dst, dst_cap, dst_on_device, call)
 
     def deflate_batch_dicts(self, items, dictionaries, which, level=-1, window_bits=15, src_on_device=False, src_off=None,
                             dict_off=None, dst=None, dst_cap=0, dst_on_device=False):
@@ -666,35 +679,13 @@ class Engine:
         `dict_off` (or a (pointer, dict_off) pair).  which[i] is item i's dictionary index, or None for no dictionary.  Item i's
         stream is byte for byte deflate_batch([item i], dictionary=its dictionary)'s.  Items, `dst` and the result are as in
         deflate_batch: (list of bytes or None, offsets (n + 1), checks, DeflateResult).  Raises ZlibError."""
-        res = DeflateResult()
-        keep = None
-        if src_on_device:
-            off = (ctypes.c_uint64 * len(src_off))(*src_off)
-            src = items
-        else:
-            keep, off = _gather(items)
-            src = ctypes.addressof(keep)
+        src, off, keep = _items(items, src_on_device, src_off)
         n = len(off) - 1
         dptr, doff, nd, dkeep = _dictionaries(dictionaries, dict_off, src_on_device)
         w = _which(which, n)
-        own = None
-        if dst is None:
-            dst_cap = lib().zb_deflate_batch_bound(off, n) + 64
-            own = ctypes.create_string_buffer(dst_cap)
-            dst = ctypes.addressof(own)
-            dst_on_device = False
-        dst_off = (ctypes.c_uint64 * (n + 1))()
-        checks = (ctypes.c_uint32 * max(n, 1))()
-        rc = lib().zb_deflate_batch_dicts(self.h, dptr, doff, nd, w, src, off, n, int(src_on_device), dst, dst_cap, int(dst_on_device),
-                                          level, 0, window_bits, 0, dst_off, checks, ctypes.byref(res))
-        if rc != 0:
-            e = ZlibError(rc, lib().zb_last_error().decode())
-            e.needed = res.out_bytes
-            raise e
-        offs = list(dst_off)
-        raw = own.raw if own is not None else None
-        outs = [raw[offs[i]:offs[i + 1]] for i in range(n)] if own is not None else None
-        return outs, offs, list(checks)[:n], res
+        return _deflate_items(off, dst, dst_cap, dst_on_device, lambda dst, dst_cap, dst_on_device, dst_off, checks, res:
+                              lib().zb_deflate_batch_dicts(self.h, dptr, doff, nd, w, src, off, n, int(src_on_device), dst, dst_cap,
+                                                           dst_on_device, level, 0, window_bits, 0, dst_off, checks, res))
 
     def inflate_batch_dicts(self, items, out_caps, dictionaries, which=None, window_bits=15, src_on_device=False, src_off=None,
                             dict_off=None, dst=None, dst_off=None, dst_on_device=False):
@@ -702,13 +693,7 @@ class Engine:
         `dictionaries` as in deflate_batch_dicts.  which[i]: a dictionary index, None (no dictionary) or DICT_BY_ID (a zlib FDICT
         item takes the lowest-index dictionary whose adler32 is its DICTID); which=None is DICT_BY_ID for every item.  Items,
         `dst` and the result are as in inflate_batch: (rc, list of bytes or None, list of InflateResult)."""
-        keep = None
-        if src_on_device:
-            off = (ctypes.c_uint64 * len(src_off))(*src_off)
-            src = items
-        else:
-            keep, off = _gather(items)
-            src = ctypes.addressof(keep)
+        src, off, keep = _items(items, src_on_device, src_off)
         n = len(off) - 1
         dptr, doffs, nd, dkeep = _dictionaries(dictionaries, dict_off, src_on_device)
         w = _which(which, n) if which is not None else None
@@ -736,35 +721,13 @@ class Engine:
         i's stream is byte for byte what Engine.deflate gives for it alone with its parameters.  Items, `dst` and the result are
         as in deflate_batch: (list of bytes or None, offsets (n + 1), checks, DeflateResult).  Raises ZlibError (.needed: the
         size a too small dst_cap would have to be)."""
-        res = DeflateResult()
-        keep = None
-        if src_on_device:
-            off = (ctypes.c_uint64 * len(src_off))(*src_off)
-            src = items
-        else:
-            keep, off = _gather(items)
-            src = ctypes.addressof(keep)
+        src, off, keep = _items(items, src_on_device, src_off)
         n = len(off) - 1
         plist = [tuple(params)] if params and not isinstance(params[0], (tuple, list)) else [tuple(p) for p in params]
         par = (BatchParams * max(len(plist), 1))(*[BatchParams(*p) for p in plist])
-        own = None
-        if dst is None:
-            dst_cap = lib().zb_deflate_batch_bound(off, n) + 64
-            own = ctypes.create_string_buffer(dst_cap)
-            dst = ctypes.addressof(own)
-            dst_on_device = False
-        dst_off = (ctypes.c_uint64 * (n + 1))()
-        checks = (ctypes.c_uint32 * max(n, 1))()
-        rc = lib().zb_deflate_batch_params(self.h, src, off, n, int(src_on_device), par, len(plist), dst, dst_cap, int(dst_on_device),
-                                           dst_off, checks, ctypes.byref(res))
-        if rc != 0:
-            e = ZlibError(rc, lib().zb_last_error().decode())
-            e.needed = res.out_bytes
-            raise e
-        offs = list(dst_off)
-        raw = own.raw if own is not None else None
-        outs = [raw[offs[i]:offs[i + 1]] for i in range(n)] if own is not None else None
-        return outs, offs, list(checks)[:n], res
+        return _deflate_items(off, dst, dst_cap, dst_on_device, lambda dst, dst_cap, dst_on_device, dst_off, checks, res:
+                              lib().zb_deflate_batch_params(self.h, src, off, n, int(src_on_device), par, len(plist), dst, dst_cap,
+                                                            dst_on_device, dst_off, checks, res))
 
     def inflate_batch(self, items, out_caps, window_bits=15, src_on_device=False, src_off=None, dst=None, dst_off=None,
                       dst_on_device=False, dictionary=None):
@@ -774,13 +737,7 @@ class Engine:
         Engine.inflate gives for that item alone.
         With a `dictionary` (bytes-like, or (device pointer, length) with src_on_device; zb_inflate_batch_dict) raw items decode
         with it as their window, and zlib items whose FDICT header names its adler32 too."""
-        keep = None
-        if src_on_device:
-            off = (ctypes.c_uint64 * len(src_off))(*src_off)
-            src = items
-        else:
-            keep, off = _gather(items)
-            src = ctypes.addressof(keep)
+        src, off, keep = _items(items, src_on_device, src_off)
         n = len(off) - 1
         own = None
         if dst is None:

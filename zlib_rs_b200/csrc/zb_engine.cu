@@ -5,6 +5,7 @@
 #include <stdlib.h>
 #include <string.h>
 #include <algorithm>
+#include <cassert>
 #include <new>
 #include "../../include/zb_engine.h"
 #include "zb_kernels.cuh"
@@ -701,29 +702,33 @@ int Engine::deflate(const void *src, size_t n_in, bool src_dev, void *dst, size_
     return ZB_OK;
 }
 
-// The member core of BGZF writing and the batch (zb_bgzf.h): buffers for `nm` members staged in `span` bytes, of which the link
-// kernels cover the first S, and the member tables.  The caller stages the members and fills moff / mlen / mcheck.
-int Engine::members_reserve(JobBufs &jb, BgzfJob &bj, uint32_t nm, uint32_t S, size_t span, int level, size_t out_cap, uint32_t wrap,
-                            uint32_t **d_freq)
+// A call of nm members that share one level, the link kernels over [0, N): the one class batch_member_params gives that level, and
+// kBgzfMaxBlocks block slots per member when they are parsed.
+MemberClasses MemberClasses::uniform(int level, uint32_t nm, uint32_t N)
 {
-    int rc;
-    if ((rc = members_alloc(jb, bj, nm, S, span, out_cap, wrap, nm * kBgzfMaxBlocks, level > 0, level >= 3, level >= 7, d_freq)) != ZB_OK)
-        return rc;
-    jb.level = (uint32_t)level;
-    jb.block_syms = kBlockSyms; // memLevel 8; deflate_quick's pieces have the same size
-    jb.serial_mode = level == 1 || level == 2 ? (uint32_t)level : 0u;
-    if (level >= 3 && level <= 6) jb.lp = level_params(level);
-    if (level >= 7) { jb.slow_mode = 1; jb.sp = slow_params(level); jb.sp.wsize = kWSize; }
-    return ZB_OK;
+    MemberParams mp;
+    batch_member_params(level, 0 /* Z_DEFAULT_STRATEGY */, 15, 8, 0, &mp);
+    MemberClasses mc;
+    mc.level = level;
+    mc.nslots = level > 0 ? nm * kBgzfMaxBlocks : 0u;
+    for (uint32_t c = mp.cls + 1; c <= kClasses; c++) {
+        mc.beg[c] = nm;
+        mc.off[c] = N;
+    }
+    return mc;
 }
 
-// ... the buffers alone: `nslots` block slots, symbols when the members are parsed, links and the steps of the lazy parsers when
-// they need them.  The tables of a batch with parameters per item (BgzfJob::mp ..) are left to the caller.
-int Engine::members_alloc(JobBufs &jb, BgzfJob &bj, uint32_t nm, uint32_t S, size_t span, size_t out_cap, uint32_t wrap, uint32_t nslots,
-                          bool parse, bool links, bool slow, uint32_t **d_freq)
+// The member core of BGZF writing, batches and flushed writing (zb_bgzf.h): buffers for `nm` members staged in `span` bytes, of which
+// the link kernels cover the first S, and the member tables.  The block slots of `mc`, symbols when some member is parsed, links and
+// the steps of the lazy parsers when a class needs them.  A call of one level gets that level's parameters for the whole job: the
+// block, size and frame kernels read them when bj.mp is null.  The caller stages the members and fills moff / mlen / mcheck, and the
+// tables of a batch with parameters per item (BgzfJob::mp ..).
+int Engine::members_alloc(JobBufs &jb, BgzfJob &bj, const MemberClasses &mc, uint32_t nm, uint32_t S, size_t span, size_t out_cap,
+                          uint32_t wrap, uint32_t **d_freq)
 {
-    const uint32_t nmt = S / kLinkTile + 1;
+    const uint32_t nmt = S / kLinkTile + 1, nslots = mc.nslots;
     memset(&jb, 0, sizeof jb);
+    bj = BgzfJob{};
     int rc;
     void *p;
 #define RES(slot, bytes, field, type)                                   \
@@ -735,19 +740,19 @@ int Engine::members_alloc(JobBufs &jb, BgzfJob &bj, uint32_t nm, uint32_t S, siz
     RES(S_OUT, out_cap + 16, out, uint8_t *)
     jb.out_cap = out_cap;
     *d_freq = nullptr;
-    if (parse && nm) {
+    if (nslots) {
         RES(S_SYMS, (span + 64) * sizeof(Sym), syms, Sym *)
         RES(S_BLOCKS, (size_t)nslots * sizeof(BlockDesc), blocks, BlockDesc *)
         RES(S_BBASE, (size_t)nslots * 4, block_base, uint32_t *)
         if ((rc = reserve(S_FREQ, (size_t)nslots * 320 * 4, &p)) != ZB_OK) return rc;
         *d_freq = static_cast<uint32_t *>(p);
     }
-    if (links && nm) {
+    if (mc.any(kClassMedium, kClassRle)) {
         RES(S_L, (span + kPad) * 2, L, uint16_t *)
         RES(S_KEYS, (span + kPad) * 2, keys, uint16_t *)
         RES(S_LLAST, (size_t)nmt * 65536 * 2, link_last, uint16_t *)
     }
-    if (slow && nm) {
+    if (mc.any(kClassSlow, kClassHuff)) {
         RES(S_M, span * 4, M, uint32_t *)
         RES(S_NXT, span * 4, nxt, uint32_t *)
     }
@@ -759,16 +764,6 @@ int Engine::members_alloc(JobBufs &jb, BgzfJob &bj, uint32_t nm, uint32_t S, siz
     uint8_t *t = static_cast<uint8_t *>(p);
     bj.nm = nm;
     bj.wrap = wrap;
-    bj.mps = nullptr;
-    bj.mdx = nullptr;
-    bj.dictid = nullptr;
-    bj.flushed = 0;
-    bj.fcheck = nullptr;
-    bj.isize = 0;
-    bj.mp = nullptr;
-    bj.mslot = nullptr;
-    bj.morder = nullptr;
-    bj.mcrc = nullptr;
     bj.moff = reinterpret_cast<uint64_t *>(t);
     bj.mout = reinterpret_cast<uint64_t *>(t + m8);
     bj.mlen = reinterpret_cast<uint32_t *>(t + 2 * m8);
@@ -777,48 +772,137 @@ int Engine::members_alloc(JobBufs &jb, BgzfJob &bj, uint32_t nm, uint32_t S, siz
     bj.mstored = reinterpret_cast<uint32_t *>(t + 2 * m8 + 3 * m4);
     bj.minfo = reinterpret_cast<JobInfo *>(t + 2 * m8 + 4 * m4);
     bj.ctl = reinterpret_cast<BgzfCtl *>(t + 2 * m8 + 4 * m4 + mi_bytes);
+    if (mc.level >= 0) {
+        const int level = mc.level;
+        jb.level = (uint32_t)level;
+        jb.block_syms = kBlockSyms; // memLevel 8; deflate_quick's pieces have the same size
+        jb.serial_mode = level == 1 || level == 2 ? (uint32_t)level : 0u;
+        if (level >= 3 && level <= 6) jb.lp = level_params(level);
+        if (level >= 7) { jb.slow_mode = 1; jb.sp = slow_params(level); jb.sp.wsize = kWSize; }
+    }
     return ZB_OK;
 }
 
-// ... and its launches behind the staging: links, parse, blocks, sizes and offsets, encoding, framing.  `ghost`: some member is
-// staged behind at least 3 dictionary bytes (k_batch_dict_ghost).
-int Engine::members_launch(JobBufs &jb, BgzfJob &bj, int level, uint32_t *d_freq, bool ghost)
+// The members' parse results and the control block behind them (members_alloc), zeroed before a member call's launches.
+static size_t result_bytes(const BgzfJob &bj)
 {
-    const uint32_t nm = bj.nm, S = jb.N, nmt = S / kLinkTile + 1;
-    const bool links = level >= 3, slow = level >= 7;
-    if (level > 0 && nm) {
-        if (links) {
-            if (jb.sp.slow) {
-                k_links2_roll<<<nmt, 1024, kLinks2SmemBytes, st>>>(jb, 0);
-                k_links_fix_roll<<<S / 256 + 1, 256, 0, st>>>(jb);
-            } else {
-                k_links2_std<<<nmt, 1024, kLinks2SmemBytes, st>>>(jb, 0);
-                k_links_fix_std<<<S / 256 + 1, 256, 0, st>>>(jb);
-                if (ghost) { k_batch_dict_ghost<<<nm, 256, 0, st>>>(jb, bj); launches++; } // zb_bgzf.cu
-            }
-            launches += 2;
-        }
-        if (jb.serial_mode) {
-            k_serial_low_members<<<nm, 32, jb.serial_mode == 2 ? kSerialSmemBytes : kSerialSmemQuick, st>>>(jb, bj);
-            launches++;
-        } else if (!slow) {
-            k_bgzf_medium<<<nm, 32, 0, st>>>(jb, bj);
-            launches++;
+    return reinterpret_cast<const uint8_t *>(bj.ctl + 1) - reinterpret_cast<const uint8_t *>(bj.minfo);
+}
+
+// The staging of batch items and flushed segments: the member table and the caller's offsets (n_soff of them; soff[0] is staged
+// member 0's caller offset, `base` that of the source's first byte) go up, a host source of `total` bytes goes to d_copy,
+// k_batch_stage spreads the source to the staged offsets behind the members' dictionary copies, and the pad behind the staged bytes,
+// the members' results and the output are zeroed.
+int Engine::members_stage(const JobBufs &jb, const BgzfJob &bj, const uint64_t *h_moff, const uint32_t *h_mlen, const uint64_t *h_soff,
+                          uint64_t *d_soff, size_t n_soff, const void *src, bool src_dev, uint64_t base, uint64_t total, uint8_t *d_copy,
+                          const uint8_t *d_dict, const uint64_t *d_mdsrc)
+{
+    const uint32_t nm = bj.nm;
+    CK(cudaMemcpyAsync(bj.moff, h_moff, (size_t)nm * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(bj.mlen, h_mlen, (size_t)nm * 4, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_soff, h_soff, n_soff * 8, cudaMemcpyHostToDevice, st));
+    if (!src_dev && total) CK(cudaMemcpyAsync(d_copy, static_cast<const uint8_t *>(src) + base, total, cudaMemcpyHostToDevice, st));
+    const uint8_t *d_src = src_dev ? static_cast<const uint8_t *>(src) + base : d_copy;
+    // k_batch_stage reads member m at src + (soff[m] - soff[0]): shift the source so that this is the member's caller offset
+    k_batch_stage<<<nm, 256, 0, st>>>(d_src + (h_soff[0] - base), d_soff, d_dict, d_mdsrc, bj, const_cast<uint8_t *>(jb.in), jb.N);
+    CK(cudaMemsetAsync(const_cast<uint8_t *>(jb.in) + jb.N, 0, kPad + 16, st));
+    CK(cudaMemsetAsync(bj.minfo, 0, result_bytes(bj), st));
+    CK(cudaMemsetAsync(jb.out, 0, jb.out_cap, st));
+    launches++;
+    return ZB_OK;
+}
+
+// The links and parsers of a member call, class by class (DESIGN.md §2o): the standard links once over the staged range of levels
+// 3..8, then k_batch_dict_ghost when `ghost` (some member is staged behind at least 3 dictionary bytes); the rolling links once over
+// level 9; every parser once over a view of its class's members; k_flush_blocks behind the parse of a flushed call outside
+// deflate_quick.  A call of one level is a call of one class.
+void Engine::members_parse(const JobBufs &jb, const BgzfJob &bj, const MemberClasses &mc, bool ghost)
+{
+    // the link kernels over the staged range of classes [c0, c1): the members' own coordinates are shift invariant
+    auto links = [&](uint32_t c0, uint32_t c1, bool roll) {
+        if (!mc.any(c0, c1)) return false;
+        JobBufs r = jb;
+        r.in += mc.off[c0];
+        r.L += mc.off[c0];
+        r.keys += mc.off[c0];
+        r.N = (uint32_t)(mc.off[c1] - mc.off[c0]);
+        const uint32_t nt = r.N / kLinkTile + 1;
+        if (roll) {
+            k_links2_roll<<<nt, 1024, kLinks2SmemBytes, st>>>(r, 0);
+            k_links_fix_roll<<<r.N / 256 + 1, 256, 0, st>>>(r);
         } else {
-            k_bgzf_slow_steps<<<nm * (kMemberMax / 256), 256, 0, st>>>(jb, bj);
-            k_bgzf_slow_walk<<<(nm + 31) / 32, 32, 0, st>>>(jb, bj);
-            launches += 2;
+            k_links2_std<<<nt, 1024, kLinks2SmemBytes, st>>>(r, 0);
+            k_links_fix_std<<<r.N / 256 + 1, 256, 0, st>>>(r);
         }
-        if (bj.flushed && jb.serial_mode != 1) { k_flush_blocks<<<nm / 256 + 1, 256, 0, st>>>(jb, bj); launches++; } // zb_bgzf.cu
+        launches += 2;
+        return true;
+    };
+    // the member tables from the first member of classes [c0, c1) on
+    auto view = [&](uint32_t c0, uint32_t c1) {
+        const uint32_t m0 = mc.beg[c0];
+        assert(m0 == 0 || bj.mslot); // without a slot table slot0() counts m * kBgzfMaxBlocks from the view's first member
+        const auto at = [m0](auto *t) { return t ? t + m0 : t; };
+        BgzfJob v = bj;
+        v.nm = mc.beg[c1] - m0;
+        v.moff = at(v.moff);
+        v.mlen = at(v.mlen);
+        v.minfo = at(v.minfo);
+        v.mp = at(v.mp);
+        v.mslot = at(v.mslot);
+        v.mps = at(v.mps);
+        v.mdx = at(v.mdx);
+        return v;
+    };
+    if (links(kClassMedium, kClassSlow9, false) && ghost) { // levels 3..8: standard hash
+        const BgzfJob v = view(kClassMedium, kClassSlow9);
+        k_batch_dict_ghost<<<v.nm, 256, 0, st>>>(jb, v); // zb_bgzf.cu
+        launches++;
     }
-    return members_blocks(jb, bj, level > 0 && nm, nm * kBgzfMaxBlocks, d_freq);
+    links(kClassSlow9, kClassRle, true); // level 9: rolling hash
+    if (mc.any(kClassQuick, kClassQuick + 1)) {
+        JobBufs q = jb;
+        q.serial_mode = 1;
+        const BgzfJob v = view(kClassQuick, kClassQuick + 1);
+        k_serial_low_members<<<v.nm, 32, kSerialSmemQuick, st>>>(q, v);
+        launches++;
+    }
+    if (mc.any(kClassFast, kClassFast + 1)) {
+        JobBufs q = jb;
+        q.serial_mode = 2;
+        const BgzfJob v = view(kClassFast, kClassFast + 1);
+        k_serial_low_members<<<v.nm, 32, kSerialSmemBytes, st>>>(q, v);
+        launches++;
+    }
+    if (mc.any(kClassMedium, kClassMedium + 1)) {
+        const BgzfJob v = view(kClassMedium, kClassMedium + 1);
+        k_bgzf_medium<<<v.nm, 32, 0, st>>>(jb, v);
+        launches++;
+    }
+    if (mc.any(kClassSlow, kClassRle)) { // levels 7..9
+        const BgzfJob v = view(kClassSlow, kClassRle);
+        k_bgzf_slow_steps<<<v.nm * (kMemberMax / 256), 256, 0, st>>>(jb, v);
+        k_bgzf_slow_walk<<<(v.nm + 31) / 32, 32, 0, st>>>(jb, v);
+        launches += 2;
+    }
+    if (mc.any(kClassRle, kClassRle + 1)) {
+        const BgzfJob v = view(kClassRle, kClassRle + 1);
+        k_bgzf_rle_steps<<<v.nm * (kMemberMax / 256), 256, 0, st>>>(jb, v);
+        k_bgzf_slow_walk<<<(v.nm + 31) / 32, 32, 0, st>>>(jb, v);
+        launches += 2;
+    }
+    if (mc.any(kClassHuff, kClassHuff + 1)) {
+        const BgzfJob v = view(kClassHuff, kClassHuff + 1);
+        k_bgzf_literals<<<v.nm * (kMemberMax / 256), 256, 0, st>>>(jb, v);
+        launches++;
+    }
+    if (bj.flushed && mc.any(kClassFast, kClasses)) { k_flush_blocks<<<bj.nm / 256 + 1, 256, 0, st>>>(jb, bj); launches++; } // zb_bgzf.cu
 }
 
 // ... from the parse on: the blocks of `nslots` block slots (when some member has any), sizes and offsets, encoding, framing.
-int Engine::members_blocks(JobBufs &jb, BgzfJob &bj, bool blocks, uint32_t nslots, uint32_t *d_freq)
+int Engine::members_blocks(JobBufs &jb, BgzfJob &bj, uint32_t nslots, uint32_t *d_freq)
 {
     const uint32_t nm = bj.nm;
-    if (blocks) {
+    if (nslots) {
         k_bgzf_hist<<<nslots, 256, 0, st>>>(jb, bj, d_freq);
         k_bgzf_build<<<nslots, 32, 0, st>>>(jb, bj, d_freq);
         launches += 2;
@@ -826,13 +910,47 @@ int Engine::members_blocks(JobBufs &jb, BgzfJob &bj, bool blocks, uint32_t nslot
     k_bgzf_size<<<nm / 256 + 1, 256, 0, st>>>(jb, bj);
     k_bgzf_scan<<<1, 1024, 0, st>>>(jb, bj);
     launches += 2;
-    if (blocks) {
+    if (nslots) {
         k_bgzf_encode<<<nslots, 1024, 0, st>>>(jb, bj);
         launches++;
     }
     k_bgzf_frame<<<nm + 1, 256, 0, st>>>(jb, bj);
     launches++;
     CK(cudaGetLastError());
+    return ZB_OK;
+}
+
+// ... and the end of the call: the control block and the tables of `back` come down with the first host sync; then the error flags
+// (`name` in the message), the length against dst_cap, `before_copy` (zb_deflate_index), the copy out, the second host sync and the
+// result fields every member call shares.  The caller fills the others.
+int Engine::members_finish(const char *name, const JobBufs &jb, const BgzfJob &bj, BgzfCtl *h_ctl, std::initializer_list<Readback> back,
+                           void *dst, size_t dst_cap, bool dst_dev, zb_deflate_result *res, const std::function<int(uint64_t)> &before_copy)
+{
+    CK(cudaMemcpyAsync(h_ctl, bj.ctl, sizeof(BgzfCtl), cudaMemcpyDeviceToHost, st));
+    for (const Readback &b : back)
+        if (b.bytes) CK(cudaMemcpyAsync(b.host, b.dev, b.bytes, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (h_ctl->error) { snprintf(g_err, sizeof g_err, "engine error flags 0x%x (%s)", h_ctl->error, name); return ZB_E_INTERNAL; }
+    const uint64_t out_bytes = h_ctl->out_bytes;
+    if (out_bytes > dst_cap) {
+        res->out_bytes = out_bytes;
+        return ZB_E_BUF;
+    }
+    int rc;
+    if (before_copy && (rc = before_copy(out_bytes)) != ZB_OK) return rc;
+    CK(cudaMemcpyAsync(dst, jb.out, out_bytes, dst_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
+    CK(cudaEventRecord(ev1, st));
+    CK(cudaStreamSynchronize(st));
+    float ms = 0;
+    CK(cudaEventElapsedTime(&ms, ev0, ev1));
+    res->out_bytes = out_bytes;
+    res->data_type = (int32_t)h_ctl->data_type;
+    res->n_symbols = h_ctl->n_syms;
+    res->n_blocks = h_ctl->n_blocks;
+    res->gpu_launches = launches;
+    res->exact_parity = 1;
+    res->gpu_ms = ms;
+    res->bits_used = 8;
     return ZB_OK;
 }
 
@@ -853,14 +971,20 @@ int Engine::deflate_bgzf(const void *src, size_t n, bool src_dev, void *dst, siz
     const uint32_t S = nm ? (nm - 1) * kBgzfStride + bgzf_member_len(n, nm - 1) : 0; // staged length: the link kernels' N
     const size_t span = (size_t)nm * kBgzfStride;
     const size_t out_cap = (bgzf_bound(n) + 15) & ~(size_t)15;
+    const MemberClasses mc = MemberClasses::uniform(level, nm, S);
     JobBufs jb;
     BgzfJob bj;
     uint32_t *d_freq;
     int rc;
-    if ((rc = members_reserve(jb, bj, nm, S, span, level, out_cap, kWrapBgzf, &d_freq)) != ZB_OK) return rc;
-    if ((rc = stage(sizeof(BgzfCtl) + 16)) != ZB_OK) return rc;
+    if ((rc = members_alloc(jb, bj, mc, nm, S, span, out_cap, kWrapBgzf, &d_freq)) != ZB_OK) return rc;
+    BgzfCtl *h_ctl;
+    uint32_t *h_crc;
+    if ((rc = carve(-1, [&](Carve &c) {
+             h_ctl = c.take<BgzfCtl>(1);
+             h_crc = c.take<uint32_t>(1);
+         })) != ZB_OK)
+        return rc;
     uint8_t *d_in = const_cast<uint8_t *>(jb.in);
-    const size_t mi_bytes = ((size_t)nm * sizeof(JobInfo) + 15) & ~(size_t)15;
 
     CK(cudaEventRecord(ev0, st));
     // staging: one pitched copy of the whole blocks, the short last one, zeros in the gaps and behind the last member
@@ -872,44 +996,24 @@ int Engine::deflate_bgzf(const void *src, size_t n, bool src_dev, void *dst, siz
     }
     if (nm) CK(cudaMemcpyAsync(d_in + (size_t)(nm - 1) * kBgzfStride, s8 + (size_t)(nm - 1) * kBgzfBlock, S - (nm - 1) * kBgzfStride, kind, st));
     CK(cudaMemsetAsync(d_in + S, 0, span - S + kPad + 16, st));
-    CK(cudaMemsetAsync(bj.minfo, 0, mi_bytes + sizeof(BgzfCtl), st));
+    CK(cudaMemsetAsync(bj.minfo, 0, result_bytes(bj), st));
     CK(cudaMemsetAsync(jb.out, 0, out_cap, st));
     k_bgzf_setup<<<nm / 256 + 1, 256, 0, st>>>(bj, (uint64_t)n);
     CK(launch_crc32_segments(d_in, bj.moff, bj.mlen, nm, bj.mcheck, st));
     CK(launch_crc32_join(bj.mcheck, bj.mlen, &bj.ctl->count, d_check, st));
     launches += 3;
-    if ((rc = members_launch(jb, bj, level, d_freq)) != ZB_OK) return rc;
-    BgzfCtl *h_ctl = static_cast<BgzfCtl *>(h_stage);
-    uint32_t *h_crc = reinterpret_cast<uint32_t *>(h_ctl + 1);
-    CK(cudaMemcpyAsync(h_ctl, bj.ctl, sizeof(BgzfCtl), cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(h_crc, d_check, 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    if (h_ctl->error) { snprintf(g_err, sizeof g_err, "engine error flags 0x%x (bgzf)", h_ctl->error); return ZB_E_INTERNAL; }
-    const uint64_t out_bytes = h_ctl->out_bytes;
-    if (out_bytes > dst_cap) {
-        res->out_bytes = out_bytes;
-        return ZB_E_BUF;
-    }
-    if (iw) { // zb_deflate_index: the index of zb_index_build with window_bits 31 and ZB_INF_MEMBERS, the end-of-file member included
+    members_parse(jb, bj, mc);
+    if ((rc = members_blocks(jb, bj, mc.nslots, d_freq)) != ZB_OK) return rc;
+    // zb_deflate_index: the index of zb_index_build with window_bits 31 and ZB_INF_MEMBERS, the end-of-file member included
+    const auto index = [&](uint64_t out_bytes) {
+        if (!iw) return (int)ZB_OK;
         IdxWriteJob w{iw->span, zbi_targets(n, iw->span), n, nm + 1, 1, 0, 0, nullptr, nullptr};
         const IdxHeader h{kIdxMagic, kIdxVersion, iw->span, n, out_bytes, *h_crc, 31, 0, 0, 0};
-        if ((rc = index_written(jb, bj, w, h, iw)) != ZB_OK) return rc;
-    }
-    CK(cudaMemcpyAsync(dst, jb.out, out_bytes, dst_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
-    CK(cudaEventRecord(ev1, st));
-    CK(cudaStreamSynchronize(st));
-    float ms = 0;
-    CK(cudaEventElapsedTime(&ms, ev0, ev1));
-    res->out_bytes = out_bytes;
+        return index_written(jb, bj, w, h, iw);
+    };
+    if ((rc = members_finish("bgzf", jb, bj, h_ctl, {{h_crc, d_check, 4}}, dst, dst_cap, dst_dev, res, index)) != ZB_OK) return rc;
     res->check = *h_crc;
-    res->data_type = (int32_t)h_ctl->data_type;
     res->iterations = level > 0 ? 1 : 0;
-    res->n_symbols = h_ctl->n_syms;
-    res->n_blocks = h_ctl->n_blocks;
-    res->gpu_launches = launches;
-    res->exact_parity = 1;
-    res->gpu_ms = ms;
-    res->bits_used = 8;
     return ZB_OK;
 }
 
@@ -978,21 +1082,29 @@ int Engine::deflate_batch(const DictTable &dt, const void *src, const uint64_t *
     }
     const uint64_t total = nm ? src_off[nm] - src_off[0] : 0;
     if (total > kBatchMaxBytes) { snprintf(g_err, sizeof g_err, "%s: %llu bytes in all (at most 2^31)", gn, (unsigned long long)total); return ZB_E_PARAM; }
-    // pinned staging: up the member table (moff | mlen | src_off; with dictionaries mps | mdx | mdsrc | the items' start | the
-    // dictionaries' offsets and lengths), down the control block, offsets and checks
-    const size_t t_dict = with_dict ? (size_t)nm * (4 + 4 + 8 + 8) + ((size_t)nd + 1) * 8 + (size_t)nd * 4 + 64 : 0;
-    const size_t t_up = (size_t)nm * 8 + (size_t)nm * 4 + ((size_t)nm + 1) * 8 + t_dict, t_down = sizeof(BgzfCtl) + (size_t)nm * 12 + 16;
+    // pinned staging: up the member table (moff | mlen | src_off; with dictionaries mdsrc | the items' start | the dictionaries'
+    // offsets | mps | mdx | the dictionaries' lengths), down the control block, offsets and checks
+    uint64_t *h_moff, *h_soff, *h_mdsrc = nullptr, *h_mitem = nullptr, *h_doff = nullptr, *h_mout;
+    uint32_t *h_mlen, *h_mps = nullptr, *h_mdx = nullptr, *h_dlen = nullptr, *h_chk;
+    BgzfCtl *h_ctl;
     int rc;
-    if ((rc = stage(t_up + t_down + 64)) != ZB_OK) return rc;
-    uint8_t *h = static_cast<uint8_t *>(h_stage);
-    uint64_t *h_moff = reinterpret_cast<uint64_t *>(h);
-    uint32_t *h_mlen = reinterpret_cast<uint32_t *>(h + (size_t)nm * 8);
-    uint64_t *h_soff = reinterpret_cast<uint64_t *>(h + (size_t)nm * 12);
-    uint64_t *h_mdsrc = h_soff + nm + 1, *h_mitem = h_mdsrc + nm, *h_doff = h_mitem + nm; // with dictionaries
-    uint32_t *h_mps = reinterpret_cast<uint32_t *>(h_doff + nd + 1), *h_mdx = h_mps + nm, *h_dlen = h_mdx + nm;
-    BgzfCtl *h_ctl = reinterpret_cast<BgzfCtl *>(h + ((t_up + 15) & ~(size_t)15));
-    uint64_t *h_mout = reinterpret_cast<uint64_t *>(h_ctl + 1);
-    uint32_t *h_chk = reinterpret_cast<uint32_t *>(h_mout + nm);
+    if ((rc = carve(-1, [&](Carve &c) {
+             h_moff = c.take<uint64_t>(nm);
+             h_mlen = c.take<uint32_t>(nm);
+             h_soff = c.take<uint64_t>((size_t)nm + 1);
+             if (with_dict) {
+                 h_mdsrc = c.take<uint64_t>(nm);
+                 h_mitem = c.take<uint64_t>(nm);
+                 h_doff = c.take<uint64_t>((size_t)nd + 1);
+                 h_mps = c.take<uint32_t>(nm);
+                 h_mdx = c.take<uint32_t>(nm);
+                 h_dlen = c.take<uint32_t>(nd);
+             }
+             h_ctl = c.take<BgzfCtl>(1);
+             h_mout = c.take<uint64_t>(nm);
+             h_chk = c.take<uint32_t>(nm);
+         })) != ZB_OK)
+        return rc;
     // the member table: items at 64-byte aligned staged offsets, each behind its dictionary copy, with a zero gap behind
     uint64_t span = 0;
     uint32_t maxD = 0;
@@ -1027,41 +1139,38 @@ int Engine::deflate_batch(const DictTable &dt, const void *src, const uint64_t *
     launches = 0;
     const uint32_t S = (uint32_t)span; // the link kernels run over the gaps too: their links are cut like any other crossing link
     const size_t out_cap = (bound + 15) & ~(size_t)15;
+    const MemberClasses mc = MemberClasses::uniform(level, nm, S);
     JobBufs jb;
     BgzfJob bj;
     uint32_t *d_freq;
-    if ((rc = members_reserve(jb, bj, nm, S, span, level, out_cap, wrap, &d_freq)) != ZB_OK) return rc;
+    if ((rc = members_alloc(jb, bj, mc, nm, S, span, out_cap, wrap, &d_freq)) != ZB_OK) return rc;
     memcpy(h_soff, src_off, ((size_t)nm + 1) * 8);
     // S_BATCH: the caller's offsets | with dictionaries: mdsrc | the items' start | the dictionaries' offsets | mps | mdx | the
     // dictionaries' lengths | their adler32 | a host copy of the dictionaries | a host source
-    auto al = [](size_t b) { return (b + 63) & ~(size_t)63; };
-    const size_t a_soff = al(((size_t)nm + 1) * 8);
-    const size_t a_tab = with_dict ? 2 * al((size_t)nm * 8) + al(((size_t)nd + 1) * 8) + 2 * al((size_t)nm * 4) + 2 * al((size_t)nd * 4) : 0;
-    const size_t a_dict = src_dev ? 0 : al(dict_bytes);
-    void *p;
-    if ((rc = reserve(S_BATCH, a_soff + a_tab + a_dict + (src_dev ? 0 : total), &p)) != ZB_OK) return rc;
-    uint8_t *t = static_cast<uint8_t *>(p);
-    uint64_t *d_soff = reinterpret_cast<uint64_t *>(t);
-    uint64_t *d_mdsrc = reinterpret_cast<uint64_t *>(t + a_soff), *d_mitem = reinterpret_cast<uint64_t *>(t + a_soff + al((size_t)nm * 8));
-    uint64_t *d_doff = reinterpret_cast<uint64_t *>(t + a_soff + 2 * al((size_t)nm * 8));
-    uint32_t *d_mps = reinterpret_cast<uint32_t *>(reinterpret_cast<uint8_t *>(d_doff) + al(((size_t)nd + 1) * 8));
-    uint32_t *d_mdx = reinterpret_cast<uint32_t *>(reinterpret_cast<uint8_t *>(d_mps) + al((size_t)nm * 4));
-    uint32_t *d_dlen = reinterpret_cast<uint32_t *>(reinterpret_cast<uint8_t *>(d_mdx) + al((size_t)nm * 4));
-    uint32_t *d_dictid = reinterpret_cast<uint32_t *>(reinterpret_cast<uint8_t *>(d_dlen) + al((size_t)nd * 4));
-    const uint8_t *d_dict = !with_dict ? nullptr
-                            : src_dev ? static_cast<const uint8_t *>(dt.data) + dt.off[0] : t + a_soff + a_tab;
-    const uint8_t *d_src = src_dev ? static_cast<const uint8_t *>(src) + src_off[0] : t + a_soff + a_tab + a_dict;
-    const size_t mi_bytes = ((size_t)nm * sizeof(JobInfo) + 15) & ~(size_t)15;
-    if (with_dict) {
-        bj.mps = d_mps;
-        bj.mdx = d_mdx;
-        bj.dictid = d_dictid;
-    }
+    uint64_t *d_soff, *d_mdsrc = nullptr, *d_mitem = nullptr, *d_doff = nullptr;
+    uint32_t *d_mps = nullptr, *d_mdx = nullptr, *d_dlen = nullptr, *d_dictid = nullptr;
+    uint8_t *d_hdict, *d_copy;
+    if ((rc = carve(S_BATCH, [&](Carve &c) {
+             d_soff = c.take<uint64_t>((size_t)nm + 1);
+             if (with_dict) {
+                 d_mdsrc = c.take<uint64_t>(nm);
+                 d_mitem = c.take<uint64_t>(nm);
+                 d_doff = c.take<uint64_t>((size_t)nd + 1);
+                 d_mps = c.take<uint32_t>(nm);
+                 d_mdx = c.take<uint32_t>(nm);
+                 d_dlen = c.take<uint32_t>(nd);
+                 d_dictid = c.take<uint32_t>(nd);
+             }
+             d_hdict = c.take<uint8_t>(src_dev ? 0 : dict_bytes);
+             d_copy = c.take<uint8_t>(src_dev ? 0 : total);
+         })) != ZB_OK)
+        return rc;
+    const uint8_t *d_dict = !with_dict ? nullptr : src_dev ? static_cast<const uint8_t *>(dt.data) + dt.off[0] : d_hdict;
+    bj.mps = d_mps;
+    bj.mdx = d_mdx;
+    bj.dictid = d_dictid;
 
     CK(cudaEventRecord(ev0, st));
-    CK(cudaMemcpyAsync(bj.moff, h_moff, (size_t)nm * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(bj.mlen, h_mlen, (size_t)nm * 4, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_soff, h_soff, ((size_t)nm + 1) * 8, cudaMemcpyHostToDevice, st));
     if (with_dict) {
         CK(cudaMemcpyAsync(d_mdsrc, h_mdsrc, (size_t)nm * 8, cudaMemcpyHostToDevice, st));
         CK(cudaMemcpyAsync(d_mps, h_mps, (size_t)nm * 4, cudaMemcpyHostToDevice, st));
@@ -1075,13 +1184,10 @@ int Engine::deflate_batch(const DictTable &dt, const void *src, const uint64_t *
     // staging: one contiguous copy of a host source (and of the dictionaries), then every item to its staged offset behind its
     // dictionary copy, with the gap behind it zeroed
     if (!src_dev && dict_bytes)
-        CK(cudaMemcpyAsync(const_cast<uint8_t *>(d_dict), static_cast<const uint8_t *>(dt.data) + dt.off[0], dict_bytes, cudaMemcpyHostToDevice, st));
-    if (!src_dev && total) CK(cudaMemcpyAsync(const_cast<uint8_t *>(d_src), static_cast<const uint8_t *>(src) + src_off[0], total, cudaMemcpyHostToDevice, st));
-    k_batch_stage<<<nm, 256, 0, st>>>(d_src, d_soff, d_dict, with_dict ? d_mdsrc : nullptr, bj, const_cast<uint8_t *>(jb.in), span);
-    CK(cudaMemsetAsync(const_cast<uint8_t *>(jb.in) + span, 0, kPad + 16, st));
-    CK(cudaMemsetAsync(bj.minfo, 0, mi_bytes + sizeof(BgzfCtl), st));
-    CK(cudaMemsetAsync(jb.out, 0, out_cap, st));
-    launches++;
+        CK(cudaMemcpyAsync(d_hdict, static_cast<const uint8_t *>(dt.data) + dt.off[0], dict_bytes, cudaMemcpyHostToDevice, st));
+    if ((rc = members_stage(jb, bj, h_moff, h_mlen, h_soff, d_soff, (size_t)nm + 1, src, src_dev, src_off[0], total, d_copy, d_dict,
+                            d_mdsrc)) != ZB_OK)
+        return rc;
     // the items' checks, as zb_deflate returns them (the item's bytes only, behind its dictionary copy), and DICTID: the adler32 of
     // every whole dictionary as passed (deflate.rs:507-510), one segment each
     if (wrap == 1) CK(launch_adler32_segments(jb.in, with_dict ? d_mitem : bj.moff, bj.mlen, nm, bj.mcheck, st));
@@ -1092,32 +1198,15 @@ int Engine::deflate_batch(const DictTable &dt, const void *src, const uint64_t *
         CK(launch_adler32_segments(d_dict, d_doff, d_dlen, nd, d_dictid, st));
         launches++;
     }
-    if ((rc = members_launch(jb, bj, level, d_freq, maxD >= 3)) != ZB_OK) return rc;
-    CK(cudaMemcpyAsync(h_ctl, bj.ctl, sizeof(BgzfCtl), cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(h_mout, bj.mout, (size_t)nm * 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(h_chk, bj.mcheck, (size_t)nm * 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    if (h_ctl->error) { snprintf(g_err, sizeof g_err, "engine error flags 0x%x (batch)", h_ctl->error); return ZB_E_INTERNAL; }
-    const uint64_t out_bytes = h_ctl->out_bytes;
-    if (out_bytes > dst_cap) {
-        res->out_bytes = out_bytes;
-        return ZB_E_BUF;
-    }
-    CK(cudaMemcpyAsync(dst, jb.out, out_bytes, dst_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
-    CK(cudaEventRecord(ev1, st));
-    CK(cudaStreamSynchronize(st));
-    float ms = 0;
-    CK(cudaEventElapsedTime(&ms, ev0, ev1));
+    members_parse(jb, bj, mc, maxD >= 3);
+    if ((rc = members_blocks(jb, bj, mc.nslots, d_freq)) != ZB_OK) return rc;
+    if ((rc = members_finish("batch", jb, bj, h_ctl, {{h_mout, bj.mout, (size_t)nm * 8}, {h_chk, bj.mcheck, (size_t)nm * 4}}, dst,
+                             dst_cap, dst_dev, res)) != ZB_OK)
+        return rc;
     for (uint32_t i = 0; i < nm; i++) dst_off[i] = h_mout[i];
-    dst_off[nm] = out_bytes;
+    dst_off[nm] = res->out_bytes;
     if (checks) memcpy(checks, h_chk, (size_t)nm * 4);
-    res->out_bytes = out_bytes;
-    res->data_type = (int32_t)h_ctl->data_type;
     res->iterations = level > 0 ? 1 : 0;
-    res->n_symbols = h_ctl->n_syms;
-    res->n_blocks = h_ctl->n_blocks;
-    res->gpu_launches = launches;
-    res->gpu_ms = ms;
     return ZB_OK;
 }
 
@@ -1141,20 +1230,27 @@ int Engine::deflate_batch_params(const void *src, const uint64_t *src_off, size_
     }
     if (n_items > kBatchMaxItems) { snprintf(g_err, sizeof g_err, "deflate_batch_params: %zu items (at most %llu)", n_items, (unsigned long long)kBatchMaxItems); return ZB_E_PARAM; }
     const uint32_t nm = (uint32_t)n_items;
-    // pinned staging: up moff | mlen | soff | mp | mslot | morder | lz | lg, down the control block | mout | adler32 | crc32
-    const size_t t_up = (size_t)nm * (8 + 4 + 8 + sizeof(MemberParams) + 4 + 4 + 4 + 4) + 4 + 64;
-    const size_t t_down = sizeof(BgzfCtl) + (size_t)nm * 16 + 16;
+    // pinned staging: up moff | soff | mp | mlen | morder | lz | lg | mslot, down the control block | mout | adler32 | crc32
+    uint64_t *h_moff, *h_soff, *h_mout;
+    MemberParams *h_mp;
+    uint32_t *h_mlen, *h_morder, *h_lz, *h_lg, *h_mslot, *h_adler, *h_crc;
+    BgzfCtl *h_ctl;
     int rc;
-    if ((rc = stage(t_up + t_down + 64)) != ZB_OK) return rc;
-    uint8_t *h = static_cast<uint8_t *>(h_stage);
-    uint64_t *h_moff = reinterpret_cast<uint64_t *>(h);
-    uint64_t *h_soff = h_moff + nm;
-    MemberParams *h_mp = reinterpret_cast<MemberParams *>(h_soff + nm);
-    uint32_t *h_mlen = reinterpret_cast<uint32_t *>(h_mp + nm);
-    uint32_t *h_morder = h_mlen + nm, *h_lz = h_morder + nm, *h_lg = h_lz + nm, *h_mslot = h_lg + nm; // mslot: nm + 1
-    BgzfCtl *h_ctl = reinterpret_cast<BgzfCtl *>(h + ((t_up + 15) & ~(size_t)15));
-    uint64_t *h_mout = reinterpret_cast<uint64_t *>(h_ctl + 1);
-    uint32_t *h_adler = reinterpret_cast<uint32_t *>(h_mout + nm), *h_crc = h_adler + nm;
+    if ((rc = carve(-1, [&](Carve &c) {
+             h_moff = c.take<uint64_t>(nm);
+             h_soff = c.take<uint64_t>(nm);
+             h_mp = c.take<MemberParams>(nm);
+             h_mlen = c.take<uint32_t>(nm);
+             h_morder = c.take<uint32_t>(nm);
+             h_lz = c.take<uint32_t>(nm);
+             h_lg = c.take<uint32_t>(nm);
+             h_mslot = c.take<uint32_t>((size_t)nm + 1);
+             h_ctl = c.take<BgzfCtl>(1);
+             h_mout = c.take<uint64_t>(nm);
+             h_adler = c.take<uint32_t>(nm);
+             h_crc = c.take<uint32_t>(nm);
+         })) != ZB_OK)
+        return rc;
     // every item's record (deflateInit2_'s rules), then a stable counting sort by class
     uint64_t total = 0, bound = 0;
     for (uint32_t i = 0; i < nm; i++) {
@@ -1180,8 +1276,8 @@ int Engine::deflate_batch_params(const void *src, const uint64_t *src_off, size_
     res->bits_used = 8;
     dst_off[0] = 0;
     if (nm == 0) return ZB_OK;
-    uint32_t cbeg[kClasses + 1]; // class c: staged members [cbeg[c], cbeg[c + 1])
-    batch_class_order(h_mp, nm, cbeg, h_morder);
+    MemberClasses mc;
+    batch_class_order(h_mp, nm, mc.beg, h_morder);
     // the staged table: member m = morder[i] is item i; its record, offset, length, slots and the lengths its checks cover
     std::vector<MemberParams> byin(h_mp, h_mp + nm);
     bool any_z = false, any_g = false;
@@ -1196,153 +1292,61 @@ int Engine::deflate_batch_params(const void *src, const uint64_t *src_off, size_
         any_g |= byin[i].wrap == 2;
     }
     const uint64_t span = batch_params_layout(h_mp, h_mlen, nm, h_moff, h_mslot);
-    const uint32_t nslots = h_mslot[nm];
-    auto has = [&](uint32_t c) { return cbeg[c + 1] > cbeg[c]; };
-    const bool links = cbeg[kClassSlow9 + 1] > cbeg[kClassMedium], steps = cbeg[kClassRle + 1] > cbeg[kClassSlow];
+    mc.nslots = h_mslot[nm];
+    for (uint32_t c = 0; c <= kClasses; c++) mc.off[c] = mc.beg[c] < nm ? h_moff[mc.beg[c]] : span;
     CK(cudaSetDevice(device));
     launches = 0;
     const size_t out_cap = (bound + 15) & ~(size_t)15;
     JobBufs jb;
     BgzfJob bj;
     uint32_t *d_freq;
-    if ((rc = members_alloc(jb, bj, nm, (uint32_t)span, span, out_cap, 0, nslots, nslots > 0, links, steps, &d_freq)) != ZB_OK) return rc;
+    if ((rc = members_alloc(jb, bj, mc, nm, (uint32_t)span, span, out_cap, 0, &d_freq)) != ZB_OK) return rc;
     // S_BATCH: soff | mp | mslot | morder | lz | lg | mcrc | a host source
-    const size_t a8 = ((size_t)nm * 8 + 63) & ~(size_t)63, a4 = ((size_t)nm * 4 + 4 + 63) & ~(size_t)63;
-    const size_t amp = ((size_t)nm * sizeof(MemberParams) + 63) & ~(size_t)63;
-    void *p;
-    if ((rc = reserve(S_BATCH, a8 + amp + 5 * a4 + (src_dev ? 0 : total), &p)) != ZB_OK) return rc;
-    uint8_t *t = static_cast<uint8_t *>(p);
-    uint64_t *d_soff = reinterpret_cast<uint64_t *>(t);
-    MemberParams *d_mp = reinterpret_cast<MemberParams *>(t + a8);
-    uint32_t *d_mslot = reinterpret_cast<uint32_t *>(t + a8 + amp), *d_morder = reinterpret_cast<uint32_t *>(t + a8 + amp + a4);
-    uint32_t *d_lz = reinterpret_cast<uint32_t *>(t + a8 + amp + 2 * a4), *d_lg = reinterpret_cast<uint32_t *>(t + a8 + amp + 3 * a4);
-    uint32_t *d_mcrc = reinterpret_cast<uint32_t *>(t + a8 + amp + 4 * a4);
-    const uint8_t *d_src = src_dev ? static_cast<const uint8_t *>(src) + src_off[0] : t + a8 + amp + 5 * a4;
+    uint64_t *d_soff;
+    MemberParams *d_mp;
+    uint32_t *d_mslot, *d_morder, *d_lz, *d_lg, *d_mcrc;
+    uint8_t *d_copy;
+    if ((rc = carve(S_BATCH, [&](Carve &c) {
+             d_soff = c.take<uint64_t>(nm);
+             d_mp = c.take<MemberParams>(nm);
+             d_mslot = c.take<uint32_t>((size_t)nm + 1);
+             d_morder = c.take<uint32_t>(nm);
+             d_lz = c.take<uint32_t>(nm);
+             d_lg = c.take<uint32_t>(nm);
+             d_mcrc = c.take<uint32_t>(nm);
+             d_copy = c.take<uint8_t>(src_dev ? 0 : total);
+         })) != ZB_OK)
+        return rc;
     bj.mp = d_mp;
     bj.mslot = d_mslot;
     bj.morder = d_morder;
     bj.mcrc = d_mcrc;
-    const size_t mi_bytes = ((size_t)nm * sizeof(JobInfo) + 15) & ~(size_t)15;
 
     CK(cudaEventRecord(ev0, st));
-    CK(cudaMemcpyAsync(bj.moff, h_moff, (size_t)nm * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(bj.mlen, h_mlen, (size_t)nm * 4, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_soff, h_soff, (size_t)nm * 8, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_mp, h_mp, (size_t)nm * sizeof(MemberParams), cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_mslot, h_mslot, ((size_t)nm + 1) * 4, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_morder, h_morder, (size_t)nm * 4, cudaMemcpyHostToDevice, st));
     if (any_z) CK(cudaMemcpyAsync(d_lz, h_lz, (size_t)nm * 4, cudaMemcpyHostToDevice, st));
     if (any_g) CK(cudaMemcpyAsync(d_lg, h_lg, (size_t)nm * 4, cudaMemcpyHostToDevice, st));
-    if (!src_dev && total) CK(cudaMemcpyAsync(const_cast<uint8_t *>(d_src), static_cast<const uint8_t *>(src) + src_off[0], total, cudaMemcpyHostToDevice, st));
-    // k_batch_stage reads member m at src + (soff[m] - soff[0]): shift the source so that this is the item's caller offset
-    k_batch_stage<<<nm, 256, 0, st>>>(d_src + (h_soff[0] - src_off[0]), d_soff, nullptr, nullptr, bj, const_cast<uint8_t *>(jb.in), span);
-    CK(cudaMemsetAsync(const_cast<uint8_t *>(jb.in) + span, 0, kPad + 16, st));
-    CK(cudaMemsetAsync(bj.minfo, 0, mi_bytes + sizeof(BgzfCtl), st));
-    CK(cudaMemsetAsync(jb.out, 0, out_cap, st));
-    launches++;
+    if ((rc = members_stage(jb, bj, h_moff, h_mlen, h_soff, d_soff, nm, src, src_dev, src_off[0], total, d_copy, nullptr, nullptr)) != ZB_OK)
+        return rc;
     // the items' checks: adler32 over the zlib members, crc32 over the gzip members (the others get segments of length 0)
     CK(cudaMemsetAsync(bj.mcheck, 0, (size_t)nm * 4, st));
     if (any_z) { CK(launch_adler32_segments(jb.in, bj.moff, d_lz, nm, bj.mcheck, st)); launches++; }
     if (any_g) { CK(launch_crc32_segments(jb.in, bj.moff, d_lg, nm, d_mcrc, st)); launches++; }
-    // links over the staged range of a run of classes: the members' own coordinates are shift invariant
-    auto link_range = [&](uint32_t m0, uint32_t m1, bool roll) {
-        if (m1 <= m0) return;
-        JobBufs r = jb;
-        const uint64_t o0 = h_moff[m0], o1 = m1 < nm ? h_moff[m1] : span;
-        r.in += o0;
-        r.L += o0;
-        r.keys += o0;
-        r.N = (uint32_t)(o1 - o0);
-        const uint32_t nt = r.N / kLinkTile + 1;
-        if (roll) {
-            k_links2_roll<<<nt, 1024, kLinks2SmemBytes, st>>>(r, 0);
-            k_links_fix_roll<<<r.N / 256 + 1, 256, 0, st>>>(r);
-        } else {
-            k_links2_std<<<nt, 1024, kLinks2SmemBytes, st>>>(r, 0);
-            k_links_fix_std<<<r.N / 256 + 1, 256, 0, st>>>(r);
-        }
-        launches += 2;
-    };
-    link_range(cbeg[kClassMedium], cbeg[kClassSlow9], false); // levels 3..8: standard hash
-    link_range(cbeg[kClassSlow9], cbeg[kClassRle], true);     // level 9: rolling hash
-    // the parsers, each over its class's members (a view of the member tables from the class's first member)
-    auto view = [&](uint32_t c0, uint32_t c1) {
-        BgzfJob v = bj;
-        const uint32_t m0 = cbeg[c0];
-        v.nm = cbeg[c1] - m0;
-        v.moff += m0;
-        v.mlen += m0;
-        v.minfo += m0;
-        v.mp += m0;
-        v.mslot += m0;
-        return v;
-    };
-    if (has(kClassQuick)) {
-        JobBufs q = jb;
-        q.serial_mode = 1;
-        const BgzfJob v = view(kClassQuick, kClassQuick + 1);
-        k_serial_low_members<<<v.nm, 32, kSerialSmemQuick, st>>>(q, v);
-        launches++;
-    }
-    if (has(kClassFast)) {
-        JobBufs q = jb;
-        q.serial_mode = 2;
-        const BgzfJob v = view(kClassFast, kClassFast + 1);
-        k_serial_low_members<<<v.nm, 32, kSerialSmemBytes, st>>>(q, v);
-        launches++;
-    }
-    if (has(kClassMedium)) {
-        const BgzfJob v = view(kClassMedium, kClassMedium + 1);
-        k_bgzf_medium<<<v.nm, 32, 0, st>>>(jb, v);
-        launches++;
-    }
-    if (cbeg[kClassRle] > cbeg[kClassSlow]) { // levels 7..9
-        const BgzfJob v = view(kClassSlow, kClassRle);
-        k_bgzf_slow_steps<<<v.nm * (kMemberMax / 256), 256, 0, st>>>(jb, v);
-        k_bgzf_slow_walk<<<(v.nm + 31) / 32, 32, 0, st>>>(jb, v);
-        launches += 2;
-    }
-    if (has(kClassRle)) {
-        const BgzfJob v = view(kClassRle, kClassRle + 1);
-        k_bgzf_rle_steps<<<v.nm * (kMemberMax / 256), 256, 0, st>>>(jb, v);
-        k_bgzf_slow_walk<<<(v.nm + 31) / 32, 32, 0, st>>>(jb, v);
-        launches += 2;
-    }
-    if (has(kClassHuff)) {
-        const BgzfJob v = view(kClassHuff, kClassHuff + 1);
-        k_bgzf_literals<<<v.nm * (kMemberMax / 256), 256, 0, st>>>(jb, v);
-        launches++;
-    }
-    if ((rc = members_blocks(jb, bj, nslots > 0, nslots, d_freq)) != ZB_OK) return rc;
-    CK(cudaMemcpyAsync(h_ctl, bj.ctl, sizeof(BgzfCtl), cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(h_mout, bj.mout, (size_t)nm * 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(h_adler, bj.mcheck, (size_t)nm * 4, cudaMemcpyDeviceToHost, st));
-    if (any_g) CK(cudaMemcpyAsync(h_crc, d_mcrc, (size_t)nm * 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    if (h_ctl->error) { snprintf(g_err, sizeof g_err, "engine error flags 0x%x (batch_params)", h_ctl->error); return ZB_E_INTERNAL; }
-    const uint64_t out_bytes = h_ctl->out_bytes;
-    if (out_bytes > dst_cap) {
-        res->out_bytes = out_bytes;
-        return ZB_E_BUF;
-    }
-    CK(cudaMemcpyAsync(dst, jb.out, out_bytes, dst_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
-    CK(cudaEventRecord(ev1, st));
-    CK(cudaStreamSynchronize(st));
-    float ms = 0;
-    CK(cudaEventElapsedTime(&ms, ev0, ev1));
+    members_parse(jb, bj, mc);
+    if ((rc = members_blocks(jb, bj, mc.nslots, d_freq)) != ZB_OK) return rc;
+    if ((rc = members_finish("batch_params", jb, bj, h_ctl,
+                             {{h_mout, bj.mout, (size_t)nm * 8}, {h_adler, bj.mcheck, (size_t)nm * 4}, {h_crc, d_mcrc, any_g ? (size_t)nm * 4 : 0}},
+                             dst, dst_cap, dst_dev, res)) != ZB_OK)
+        return rc;
     for (uint32_t i = 0; i < nm; i++) {
         const uint32_t m = h_morder[i];
         dst_off[i] = h_mout[m];
         if (checks) checks[i] = byin[i].wrap == 1 ? h_adler[m] : byin[i].wrap == 2 ? h_crc[m] : 0u;
     }
-    dst_off[nm] = out_bytes;
-    res->out_bytes = out_bytes;
-    res->data_type = (int32_t)h_ctl->data_type;
-    res->iterations = nslots > 0 ? 1 : 0;
-    res->n_symbols = h_ctl->n_syms;
-    res->n_blocks = h_ctl->n_blocks;
-    res->gpu_launches = launches;
-    res->gpu_ms = ms;
+    dst_off[nm] = res->out_bytes;
+    res->iterations = mc.nslots > 0 ? 1 : 0;
     return ZB_OK;
 }
 
@@ -1391,24 +1395,28 @@ int Engine::deflate_flushed(const void *src, const uint64_t *seg_off, size_t n_s
     launches = 0;
     const uint32_t S = (uint32_t)span; // 2^31 input bytes + at most 127 bytes of gap and alignment per segment: below 2^32
     const size_t out_cap = (bound + 15) & ~(size_t)15;
+    const MemberClasses mc = MemberClasses::uniform(level, nm, S);
     JobBufs jb;
     BgzfJob bj;
     uint32_t *d_freq;
     int rc;
-    if ((rc = members_reserve(jb, bj, nm, S, span, level, out_cap, wrap, &d_freq)) != ZB_OK) return rc;
+    if ((rc = members_alloc(jb, bj, mc, nm, S, span, out_cap, wrap, &d_freq)) != ZB_OK) return rc;
     bj.flushed = 1;
     bj.isize = (uint32_t)total;
-    // pinned staging: the member table up (moff | mlen | seg_off | count), the control block and offsets down
-    const size_t t_up = (size_t)nm * 8 + (size_t)nm * 8 + ((size_t)nm + 1) * 8 + 16, t_down = sizeof(BgzfCtl) + (size_t)nm * 8 + 16;
-    if ((rc = stage(t_up + t_down + 64)) != ZB_OK) return rc;
-    uint8_t *h = static_cast<uint8_t *>(h_stage);
-    uint64_t *h_moff = reinterpret_cast<uint64_t *>(h);
-    uint32_t *h_mlen = reinterpret_cast<uint32_t *>(h + (size_t)nm * 8);
-    uint64_t *h_soff = reinterpret_cast<uint64_t *>(h + (size_t)nm * 16);
-    uint32_t *h_count = reinterpret_cast<uint32_t *>(h_soff + nm + 1);
-    BgzfCtl *h_ctl = reinterpret_cast<BgzfCtl *>(h + ((t_up + 15) & ~(size_t)15));
-    uint64_t *h_mout = reinterpret_cast<uint64_t *>(h_ctl + 1);
-    uint32_t *h_check = reinterpret_cast<uint32_t *>(h_mout + nm);
+    // pinned staging: the member table up (moff | mlen | seg_off | count), the control block, offsets and the check down
+    uint64_t *h_moff, *h_soff, *h_mout;
+    uint32_t *h_mlen, *h_count, *h_check;
+    BgzfCtl *h_ctl;
+    if ((rc = carve(-1, [&](Carve &c) {
+             h_moff = c.take<uint64_t>(nm);
+             h_mlen = c.take<uint32_t>(nm);
+             h_soff = c.take<uint64_t>((size_t)nm + 1);
+             h_count = c.take<uint32_t>(1);
+             h_ctl = c.take<BgzfCtl>(1);
+             h_mout = c.take<uint64_t>(nm);
+             h_check = c.take<uint32_t>(1);
+         })) != ZB_OK)
+        return rc;
     uint64_t off = 0;
     for (uint32_t i = 0; i < nm; i++) {
         h_moff[i] = off;
@@ -1418,27 +1426,21 @@ int Engine::deflate_flushed(const void *src, const uint64_t *seg_off, size_t n_s
     memcpy(h_soff, seg_off, ((size_t)nm + 1) * 8);
     *h_count = nm;
     // S_BATCH: the caller's offsets | the joined check | a host source
-    const size_t a_soff = (((size_t)nm + 1) * 8 + 63) & ~(size_t)63;
-    void *p;
-    if ((rc = reserve(S_BATCH, a_soff + 64 + (src_dev ? 0 : total), &p)) != ZB_OK) return rc;
-    uint8_t *t = static_cast<uint8_t *>(p);
-    uint64_t *d_soff = reinterpret_cast<uint64_t *>(t);
-    bj.fcheck = reinterpret_cast<uint32_t *>(t + a_soff);
-    const uint8_t *d_src = src_dev ? static_cast<const uint8_t *>(src) + seg_off[0] : t + a_soff + 64;
-    const size_t mi_bytes = ((size_t)nm * sizeof(JobInfo) + 15) & ~(size_t)15;
+    uint64_t *d_soff;
+    uint8_t *d_copy;
+    if ((rc = carve(S_BATCH, [&](Carve &c) {
+             d_soff = c.take<uint64_t>((size_t)nm + 1);
+             bj.fcheck = c.take<uint32_t>(1);
+             d_copy = c.take<uint8_t>(src_dev ? 0 : total);
+         })) != ZB_OK)
+        return rc;
 
     CK(cudaEventRecord(ev0, st));
-    CK(cudaMemcpyAsync(bj.moff, h_moff, (size_t)nm * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(bj.mlen, h_mlen, (size_t)nm * 4, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_soff, h_soff, ((size_t)nm + 1) * 8, cudaMemcpyHostToDevice, st));
-    if (!src_dev) CK(cudaMemcpyAsync(const_cast<uint8_t *>(d_src), static_cast<const uint8_t *>(src) + seg_off[0], total, cudaMemcpyHostToDevice, st));
     // staging: every segment at its offset with zeros behind it, as a batch item (zb_bgzf.h: the bytes behind a segment do not matter)
-    k_batch_stage<<<nm, 256, 0, st>>>(d_src, d_soff, nullptr, nullptr, bj, const_cast<uint8_t *>(jb.in), span);
-    CK(cudaMemsetAsync(const_cast<uint8_t *>(jb.in) + span, 0, kPad + 16, st));
-    launches++;
-    CK(cudaMemsetAsync(bj.minfo, 0, mi_bytes + sizeof(BgzfCtl), st));
+    if ((rc = members_stage(jb, bj, h_moff, h_mlen, h_soff, d_soff, (size_t)nm + 1, src, src_dev, seg_off[0], total, d_copy, nullptr,
+                            nullptr)) != ZB_OK)
+        return rc;
     CK(cudaMemcpyAsync(&bj.ctl->count, h_count, 4, cudaMemcpyHostToDevice, st));
-    CK(cudaMemsetAsync(jb.out, 0, out_cap, st));
     // the segments' checks, joined in order into the whole input's
     if (wrap == 1) {
         CK(launch_adler32_segments(jb.in, bj.moff, bj.mlen, nm, bj.mcheck, st));
@@ -1448,35 +1450,17 @@ int Engine::deflate_flushed(const void *src, const uint64_t *seg_off, size_t n_s
         CK(launch_crc32_join(bj.mcheck, bj.mlen, &bj.ctl->count, bj.fcheck, st));
     } else CK(cudaMemsetAsync(bj.fcheck, 0, 4, st));
     if (wrap) launches += 2;
-    if ((rc = members_launch(jb, bj, level, d_freq)) != ZB_OK) return rc;
-    CK(cudaMemcpyAsync(h_ctl, bj.ctl, sizeof(BgzfCtl), cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(h_mout, bj.mout, (size_t)nm * 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(h_check, bj.fcheck, 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    if (h_ctl->error) { snprintf(g_err, sizeof g_err, "engine error flags 0x%x (flushed)", h_ctl->error); return ZB_E_INTERNAL; }
-    const uint64_t out_bytes = h_ctl->out_bytes;
-    if (out_bytes > dst_cap) {
-        res->out_bytes = out_bytes;
-        return ZB_E_BUF;
-    }
-    CK(cudaMemcpyAsync(dst, jb.out, out_bytes, dst_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
-    CK(cudaEventRecord(ev1, st));
-    CK(cudaStreamSynchronize(st));
-    float ms = 0;
-    CK(cudaEventElapsedTime(&ms, ev0, ev1));
+    members_parse(jb, bj, mc);
+    if ((rc = members_blocks(jb, bj, mc.nslots, d_freq)) != ZB_OK) return rc;
+    if ((rc = members_finish("flushed", jb, bj, h_ctl, {{h_mout, bj.mout, (size_t)nm * 8}, {h_check, bj.fcheck, 4}}, dst, dst_cap,
+                             dst_dev, res)) != ZB_OK)
+        return rc;
     restart[0] = stream_header_len(wrap);
     for (uint32_t i = 1; i < nm; i++) restart[i] = h_mout[i];
-    restart[nm] = out_bytes - stream_trailer_len(wrap);
-    res->out_bytes = out_bytes;
+    restart[nm] = res->out_bytes - stream_trailer_len(wrap);
     res->check = *h_check;
-    res->data_type = (int32_t)h_ctl->data_type;
     res->iterations = level > 0 ? 1 : 0;
-    res->n_symbols = h_ctl->n_syms;
-    res->n_blocks = h_ctl->n_blocks + nm - 1; // with the empty stored block of every full flush
-    res->gpu_launches = launches;
-    res->exact_parity = 1;
-    res->gpu_ms = ms;
-    res->bits_used = 8;
+    res->n_blocks += nm - 1; // with the empty stored block of every full flush
     return ZB_OK;
 }
 

@@ -3,6 +3,8 @@
 #include <cuda_runtime.h>
 #include <stddef.h>
 #include <stdint.h>
+#include <functional>
+#include <initializer_list>
 #include <vector>
 #include "../../include/zb_engine.h"
 #include "zb_index.h"
@@ -62,6 +64,36 @@ struct IdxWrite {
     zb_index *out = nullptr;
 };
 
+// One bump allocation of 64-byte aligned tables, each taken by type and count (Engine::carve).  Without a base it only counts.
+struct Carve {
+    uint8_t *base = nullptr;
+    size_t used = 0;
+    template <class T> T *take(size_t n)
+    {
+        T *p = base ? reinterpret_cast<T *>(base + used) : nullptr;
+        used += (n * sizeof(T) + 63) & ~(size_t)63;
+        return p;
+    }
+};
+
+// The parser classes of a member call (MemberClass, zb_bgzf.h): class c is the staged members [beg[c], beg[c + 1]), staged from
+// byte off[c] on (the link kernels' N for a class behind the last member).  A call whose members share one level (BGZF, batches,
+// flushed writing) has a single class and that level; a batch with parameters per item has level -1 and a record per member.
+struct MemberClasses {
+    int level = -1;
+    uint32_t nslots = 0; // block slots of the call
+    uint32_t beg[kClasses + 1] = {};
+    uint64_t off[kClasses + 1] = {};
+    bool any(uint32_t c0, uint32_t c1) const { return beg[c1] > beg[c0]; } // a member in classes [c0, c1)
+    static MemberClasses uniform(int level, uint32_t nm, uint32_t N);
+};
+// Pinned bytes a member call reads back with its control block (Engine::members_finish); none when `bytes` is 0.
+struct Readback {
+    void *host;
+    const void *dev;
+    size_t bytes;
+};
+
 struct Engine {
     static constexpr int kSlots = 44;
     struct Buf { void *p = nullptr; size_t cap = 0; };
@@ -95,6 +127,19 @@ struct Engine {
     ~Engine();
     int reserve(int slot, size_t bytes, void **out);
     int stage(size_t bytes);
+    // Lays out pinned staging (slot -1) or a device slot with `lay(Carve &)`, which runs twice: once to size the buffer, once on it.
+    // The size reserved and the pointers handed out come from the same code.
+    template <class F> int carve(int slot, F &&lay)
+    {
+        Carve c;
+        lay(c);
+        void *p = nullptr;
+        const int rc = slot < 0 ? stage(c.used) : reserve(slot, c.used, &p);
+        if (rc != ZB_OK) return rc;
+        c = Carve{static_cast<uint8_t *>(slot < 0 ? h_stage : p)};
+        lay(c);
+        return ZB_OK;
+    }
     int deflate(const void *src, size_t n, bool src_dev, void *dst, size_t dst_cap, bool dst_dev, int level, int strategy,
                 int window_bits, uint32_t flags, zb_deflate_result *res, const void *dict = nullptr, size_t dict_len = 0,
                 IdxWrite *iw = nullptr);
@@ -117,12 +162,16 @@ struct Engine {
                         int level, int strategy, int window_bits, uint32_t flags, uint64_t *restart, zb_deflate_result *res);
     int inflate_flushed(const void *src, size_t src_len, bool src_dev, const uint64_t *restart, size_t n_segs, const uint32_t *which,
                         size_t n_which, void *dst, const uint64_t *dst_off, bool dst_dev, int window_bits, zb_inflate_result *items);
-    int members_reserve(JobBufs &jb, BgzfJob &bj, uint32_t nm, uint32_t S, size_t span, int level, size_t out_cap, uint32_t wrap,
-                        uint32_t **d_freq);
-    int members_launch(JobBufs &jb, BgzfJob &bj, int level, uint32_t *d_freq, bool ghost = false);
-    int members_alloc(JobBufs &jb, BgzfJob &bj, uint32_t nm, uint32_t S, size_t span, size_t out_cap, uint32_t wrap, uint32_t nslots,
-                      bool parse, bool links, bool slow, uint32_t **d_freq);
-    int members_blocks(JobBufs &jb, BgzfJob &bj, bool blocks, uint32_t nslots, uint32_t *d_freq);
+    int members_alloc(JobBufs &jb, BgzfJob &bj, const MemberClasses &mc, uint32_t nm, uint32_t S, size_t span, size_t out_cap,
+                      uint32_t wrap, uint32_t **d_freq);
+    int members_stage(const JobBufs &jb, const BgzfJob &bj, const uint64_t *h_moff, const uint32_t *h_mlen, const uint64_t *h_soff,
+                      uint64_t *d_soff, size_t n_soff, const void *src, bool src_dev, uint64_t base, uint64_t total, uint8_t *d_copy,
+                      const uint8_t *d_dict, const uint64_t *d_mdsrc);
+    void members_parse(const JobBufs &jb, const BgzfJob &bj, const MemberClasses &mc, bool ghost = false);
+    int members_blocks(JobBufs &jb, BgzfJob &bj, uint32_t nslots, uint32_t *d_freq);
+    int members_finish(const char *name, const JobBufs &jb, const BgzfJob &bj, BgzfCtl *h_ctl, std::initializer_list<Readback> back,
+                       void *dst, size_t dst_cap, bool dst_dev, zb_deflate_result *res,
+                       const std::function<int(uint64_t)> &before_copy = nullptr);
     int deflate_batch_params(const void *src, const uint64_t *src_off, size_t n_items, bool src_dev, const zb_batch_params *params,
                              size_t n_params, void *dst, size_t dst_cap, bool dst_dev, uint64_t *dst_off, uint32_t *checks,
                              zb_deflate_result *res);
