@@ -259,6 +259,32 @@ ZB_API int zb_inflate_ex(zb_engine *e, const void *src, size_t src_len, int src_
  * ZB_E_PARAM).  Each item is decoded by one warp: a single large stream decodes faster through zb_inflate_ex. */
 ZB_API int zb_inflate_batch(zb_engine *e, const void *src, const uint64_t *src_off, size_t n_items, int src_on_device, void *dst,
                             const uint64_t *dst_off, int dst_on_device, int window_bits, zb_inflate_result *items);
+
+/* Decoding without a caller-given output size (DESIGN.md §2q), for data that comes without its lengths: a gzip file from elsewhere
+ * (ISIZE is only the last member's length modulo 2^32), a zlib column, HTTP bodies.  The output lies in a buffer the engine owns
+ * and grows: *out is a device pointer into it, valid until the next call on this engine (zb_copy_to_host copies it out).
+ *
+ * zb_inflate_auto: decode src without a caller-given output size.  *out holds res->out_bytes bytes.  The result (return code,
+ * status, msg, out_bytes, in_bytes, check) is what zb_inflate_ex gives with a dst_cap no smaller than the stream's output.  An
+ * output longer than max_out is not decoded: ZB_E_BUF with res->out_bytes = its length (the decompression-bomb limit); with
+ * ZB_INF_MEMBERS, the output up to the end of the member that crosses max_out.  Flags are those of zb_inflate_ex; with
+ * ZB_INF_NO_SERIAL, an output over max_out on the block-parallel path is declined as "capacity".  A stream the block-parallel
+ * decoder takes is sized by its block chain, at no extra launch or sync; any other stream (inputs below 64 KiB, streams the chain
+ * declines) runs a count pass of the one-warp decoder first: one launch and one host sync more than zb_inflate_ex.  With
+ * ZB_INF_MEMBERS, runs of BGZF members are sized by their ISIZE hints (still only hints: a wrong one, or one above 1032 times the
+ * member's length, which no deflate data can reach, sends the member through the single-stream path).  ZB_E_MEM with a
+ * zb_last_error() text, and no decode, when the device cannot hold the output.  Refusing an output over max_out takes a count
+ * pass of the one-warp decoder over the whole stream (the exact length is reported), so it costs time in proportion to the
+ * output, as decoding it serially would, but no output memory. */
+ZB_API int zb_inflate_auto(zb_engine *e, const void *src, size_t src_len, int src_on_device, int window_bits, uint32_t flags,
+                           uint64_t max_out, zb_inflate_result *res, const void **out);
+/* zb_inflate_batch_auto: zb_inflate_batch without slot sizes.  Item i's output is (*out)[dst_off[i], dst_off[i+1]), packed back to
+ * back; dst_off (host, n_items + 1 entries) is filled, and items[i] is what zb_inflate_batch gives for item i with a slot of exactly
+ * that length -- a damaged item's slot is its partial output.  max_out bounds the sum: over it, ZB_E_BUF, nothing decoded, dst_off
+ * filled with the offsets needed.  Limits are those of zb_inflate_batch (2^20 items, ZB_E_PARAM for an item whose output is 4 GiB
+ * or more).  6 launches whatever n_items (k_batch_count, k_batch_slots, then zb_inflate_batch's 4) and 2 host syncs. */
+ZB_API int zb_inflate_batch_auto(zb_engine *e, const void *src, const uint64_t *src_off, size_t n_items, int src_on_device,
+                                 int window_bits, uint64_t max_out, uint64_t *dst_off, zb_inflate_result *items, const void **out);
 /* zb_inflate_batch_dict: zb_inflate_batch with one preset dictionary (DESIGN.md §2j).  items[i] gets what inflateInit2(window_bits),
  * inflateSetDictionary(dict) up front for a raw stream or after inflate() returned Z_NEED_DICT, and inflate(Z_FINISH) give for
  * that item alone: a raw item decodes with the dictionary as its window, a zlib item with FDICT when its DICTID equals

@@ -150,6 +150,10 @@ def lib():
         L.zb_bgzf_bound.argtypes, L.zb_bgzf_bound.restype = [sz], sz
         L.zb_inflate.argtypes = [vp, vp, sz, ci, vp, sz, ci, ci, ctypes.POINTER(InflateResult)]
         L.zb_inflate_ex.argtypes = [vp, vp, sz, ci, vp, sz, ci, ci, u32, ctypes.POINTER(InflateResult)]
+        if hasattr(L, "zb_inflate_auto"):
+            L.zb_inflate_auto.argtypes = [vp, vp, sz, ci, ci, u32, u64, ctypes.POINTER(InflateResult), ctypes.POINTER(vp)]
+            L.zb_inflate_batch_auto.argtypes = [vp, vp, ctypes.POINTER(u64), sz, ci, ci, u64, ctypes.POINTER(u64),
+                                                ctypes.POINTER(InflateResult), ctypes.POINTER(vp)]
         if hasattr(L, "zb_deflate_batch"):  # builds before the batch calls (ZB_LIB_PATH baselines of scripts/gpu_ab.sh) lack them
             u64p = ctypes.POINTER(u64)
             L.zb_deflate_batch.argtypes = [vp, vp, u64p, sz, ci, vp, sz, ci, ci, ci, ci, u32, u64p, ctypes.POINTER(u32),
@@ -215,6 +219,11 @@ def _buf(data):
 def bgzf_bound(n):
     """Largest file Engine.deflate(..., window_bits=31, flags=ZB_FLAG_BGZF) writes for n input bytes: ceil(n / 65280) * 65536 + 28."""
     return lib().zb_bgzf_bound(n)
+
+
+def _max_out(max_out):
+    """max_out of the auto-sized inflate calls: None is no limit."""
+    return (1 << 64) - 1 if max_out is None else max_out
 
 
 def _offsets(lengths):
@@ -634,14 +643,27 @@ class Engine:
             raise e
         return (own.raw[: res.out_bytes] if own is not None else None), res, Index(h.value)
 
-    def inflate(self, src, out_cap, n=None, window_bits=15, src_on_device=False, dst=None, dst_on_device=False, flags=0):
-        """Returns (rc, bytes or None, InflateResult).  flags: ZB_INF_*."""
+    def inflate(self, src, out_cap=None, n=None, window_bits=15, src_on_device=False, dst=None, dst_on_device=False, flags=0,
+                max_out=None):
+        """Returns (rc, bytes or None, InflateResult).  flags: ZB_INF_*.
+        Without out_cap (zb_inflate_auto) the engine finds the output size itself and the bytes are copied back from its buffer;
+        the result is what a large enough out_cap gives.  An output longer than max_out (None: no limit) is not decoded: rc
+        Z_BUF_ERROR, res.out_bytes its length, and no bytes."""
         res = InflateResult()
         keep = None
         if not src_on_device:
             data, keep = _buf(src)
             n = len(data)
             src = ctypes.addressof(keep)
+        if out_cap is None:
+            if dst is not None:
+                raise ValueError("Engine.inflate without out_cap writes to the engine's buffer: no dst")
+            out = ctypes.c_void_p()
+            rc = lib().zb_inflate_auto(self.h, src, n, int(src_on_device), window_bits, flags, _max_out(max_out), ctypes.byref(res),
+                                       ctypes.byref(out))
+            if rc == Z_BUF_ERROR or rc not in (Z_OK, Z_DATA_ERROR, ZB_E_DECLINED):
+                return rc, None, res
+            return rc, (self.to_host(out.value, res.out_bytes) if res.out_bytes else b""), res
         own = None
         if dst is None:
             own = ctypes.create_string_buffer(max(out_cap, 1))
@@ -729,16 +751,32 @@ class Engine:
                               lib().zb_deflate_batch_params(self.h, src, off, n, int(src_on_device), par, len(plist), dst, dst_cap,
                                                             dst_on_device, dst_off, checks, res))
 
-    def inflate_batch(self, items, out_caps, window_bits=15, src_on_device=False, src_off=None, dst=None, dst_off=None,
-                      dst_on_device=False, dictionary=None):
+    def inflate_batch(self, items, out_caps=None, window_bits=15, src_on_device=False, src_off=None, dst=None, dst_off=None,
+                      dst_on_device=False, dictionary=None, max_out=None):
         """Inflate every item into its own slot in one call (zb_inflate_batch).  Host `items`: a list of bytes-like objects and
         `out_caps` the slot length of each; device `items`: a pointer with `src_off`.  A caller's `dst` takes `dst_off` (n + 1
         offsets) instead of out_caps.  Returns (rc, list of bytes or None, list of InflateResult): each result is what
         Engine.inflate gives for that item alone.
         With a `dictionary` (bytes-like, or (device pointer, length) with src_on_device; zb_inflate_batch_dict) raw items decode
-        with it as their window, and zlib items whose FDICT header names its adler32 too."""
+        with it as their window, and zlib items whose FDICT header names its adler32 too.
+        Without out_caps and dst (zb_inflate_batch_auto) the engine finds each item's output size itself: each result is what
+        a slot of exactly that size gives.  Outputs longer than max_out (None: no limit) in all are not decoded: rc Z_BUF_ERROR
+        and no bytes."""
         src, off, keep = _items(items, src_on_device, src_off)
         n = len(off) - 1
+        if out_caps is None and dst is None:
+            if dictionary is not None:
+                raise ValueError("Engine.inflate_batch with a dictionary needs out_caps")
+            doff = (ctypes.c_uint64 * (n + 1))()
+            res = (InflateResult * max(n, 1))()
+            out = ctypes.c_void_p()
+            rc = lib().zb_inflate_batch_auto(self.h, src, off, n, int(src_on_device), window_bits, _max_out(max_out), doff, res,
+                                             ctypes.byref(out))
+            results = list(res)[:n]
+            if rc not in (Z_OK, Z_DATA_ERROR):
+                return rc, None, results
+            raw = self.to_host(out.value, doff[n]) if doff[n] else b""
+            return rc, [raw[doff[i]:doff[i + 1]] for i in range(n)], results
         own = None
         if dst is None:
             doff = _offsets(list(out_caps))

@@ -1715,6 +1715,23 @@ int zb_inflate_ex(zb_engine *z, const void *src, size_t n, int src_dev, void *ds
     return z->e.inflate(src, n, src_dev != 0, dst, cap, dst_dev != 0, window_bits, res, flags);
 }
 
+int zb_inflate_auto(zb_engine *z, const void *src, size_t n, int src_dev, int window_bits, uint32_t flags, uint64_t max_out,
+                    zb_inflate_result *res, const void **out)
+{
+    if (!z) return ZB_E_NODEVICE;
+    z->e.shard.phase = 0; // a range job in progress is gone (its buffers are reused)
+    return z->e.inflate_auto(src, n, src_dev != 0, window_bits, flags, max_out, res, out);
+}
+
+int zb_inflate_batch_auto(zb_engine *z, const void *src, const uint64_t *src_off, size_t n_items, int src_dev, int window_bits,
+                          uint64_t max_out, uint64_t *dst_off, zb_inflate_result *items, const void **out)
+{
+    if (!z) return ZB_E_NODEVICE;
+    z->e.shard.phase = 0; // a range job in progress is gone (its buffers are reused)
+    const zb::Engine::BatchAuto ba{max_out, dst_off, out};
+    return z->e.inflate_batch(zb::Engine::DictTable{}, src, src_off, n_items, src_dev != 0, nullptr, nullptr, true, window_bits, items, &ba);
+}
+
 int zb_inflate_blocks(zb_engine *z, const void *src, size_t n, uint64_t start_bit, const void *dict, size_t dict_len, void *dst, size_t cap,
                       int check_kind, uint32_t check_start, zb_inflate_seg *out)
 {

@@ -23,6 +23,7 @@ enum { S_IN, S_L, S_HOLES, S_HOLESN, S_M, S_NXT, S_PEXIT, S_PCNT, S_SYMIDX, S_TE
        S_BATCH,        // batches: the caller's offsets, a host source's bytes (deflate), item tables and results (inflate)
        S_INDEX,        // index build: jobs, hits and points; extract: pieces, decoder states, windows and staged input
        S_INDEXW,       // index build: the windows of the points
+       S_AUTO,         // zb_inflate_auto / zb_inflate_batch_auto: the output, sized to what the stream or batch decodes to
        S_COUNT };
 
 // A range job of chunk-sharded deflate (zb_shard_*, zb_shard.cu) between its four calls.
@@ -95,7 +96,7 @@ struct Readback {
 };
 
 struct Engine {
-    static constexpr int kSlots = 44;
+    static constexpr int kSlots = 45;
     struct Buf { void *p = nullptr; size_t cap = 0; };
     int device = -1;
     cudaStream_t st = nullptr, st2 = nullptr; // st2: the serial tail runs beside k_emit
@@ -177,18 +178,28 @@ struct Engine {
                              zb_deflate_result *res);
     int inflate(const void *src, size_t n, bool src_dev, void *dst, size_t dst_cap, bool dst_dev, int window_bits,
                 zb_inflate_result *res, uint32_t flags = 0, IdxBuild *ib = nullptr);
+    // auto_base (zb_inflate_auto): the output goes to S_AUTO from that byte on, sized to the stream; dst_cap is the most accepted
     int inflate_stream(const uint8_t *d_src, size_t n, uint8_t *d_dst, size_t dst_cap, int window_bits, uint32_t flags,
-                       zb_inflate_result *res, InfTrace *tr = nullptr);
+                       zb_inflate_result *res, InfTrace *tr = nullptr, const uint64_t *auto_base = nullptr);
     int inflate_members(const uint8_t *d_src, size_t n, uint8_t *d_dst, size_t dst_cap, int window_bits, zb_inflate_result *res,
-                        InfTrace *tr = nullptr);
+                        InfTrace *tr = nullptr, bool automatic = false);
+    int inflate_auto(const void *src, size_t n, bool src_dev, int window_bits, uint32_t flags, uint64_t max_out, zb_inflate_result *res,
+                     const void **out);
+    int grow_auto(size_t bytes, size_t keep, uint8_t **out);
     int index_points(const uint8_t *d_src, const uint8_t *d_dst, const zb_inflate_result *res, int window_bits, IdxBuild *ib);
     int index_fill(zb_index &x, std::vector<IdxMember> &&M, std::vector<IdxPoint> &&pts, const IdxHeader &h, const uint8_t *d_src,
                    uint64_t shift);
     int index_bgzf(const void *src, size_t n, bool src_dev, zb_inflate_result *res, zb_index *x);
     int index_extract(const zb_index *x, const void *src, size_t src_len, bool src_dev, const uint64_t *offsets, size_t n_ranges,
                       void *dst, const uint64_t *dst_off, bool dst_dev, zb_inflate_result *items);
+    // zb_inflate_batch_auto: no slots from the caller; the batch's output goes to S_AUTO, its offsets to dst_off
+    struct BatchAuto {
+        uint64_t max_out;
+        uint64_t *dst_off;
+        const void **out;
+    };
     int inflate_batch(const DictTable &dt, const void *src, const uint64_t *src_off, size_t n_items, bool src_dev, void *dst,
-                      const uint64_t *dst_off, bool dst_dev, int window_bits, zb_inflate_result *items);
+                      const uint64_t *dst_off, bool dst_dev, int window_bits, zb_inflate_result *items, const BatchAuto *ba = nullptr);
     int inflate_blocks(const void *src, size_t n, uint64_t start_bit, const void *dict, size_t dict_len, void *dst, size_t dst_cap,
                        int check_kind, uint32_t check_start, zb_inflate_seg *out);
     int checksum(bool crc, uint32_t start, const void *buf, size_t len, bool on_dev, uint32_t *out, float *ms);

@@ -164,7 +164,11 @@ struct InfRange {
 // The one-warp decoder: a whole stream (header, blocks, trailer) or, in segment mode, raw blocks from a bit position.  Output goes to
 // dst[0, cap) only.  k_inflate runs it on one stream, k_members on one gzip member per warp, k_index_extract (kRange) on one piece
 // of a range; the kRange additions compile away in the others.
-template <bool kRange = false>
+// kCount (k_inflate_count, k_batch_count): the same decode with unlimited output that writes nothing -- neither S.out nor dst --
+// and ignores dst and cap.  opos still counts, so res gets what a decode with a large enough cap gives, except no check value is
+// made here.  Flushes and warp copies are replaced by their effect on lane 0 (oflush moves on, a long copy ends the symbol loop),
+// so the symbols are taken in the same rounds and a truncated stream stops at the same output position as in a real decode.
+template <bool kRange = false, bool kCount = false>
 __device__ __forceinline__ void inflate_warp(InfShared &S, const uint8_t *__restrict__ src, uint64_t n, uint8_t *__restrict__ dst,
                                              uint64_t cap, int window_bits, InfState *res, InfSeg seg, InfDict pd = InfDict{nullptr, nullptr, 0, 0},
                                              InfRange rg = InfRange{})
@@ -194,7 +198,7 @@ __device__ __forceinline__ void inflate_warp(InfShared &S, const uint8_t *__rest
     uint64_t blk_bit = seg.start_bit, blk_out = D0;
     uint32_t final_done = 0, stored_wait = 0;
     if (seg.on) {
-        for (uint32_t i = lane; i < seg.dict_len; i += 32) S.out[i] = seg.dict[i];
+        if constexpr (!kCount) { for (uint32_t i = lane; i < seg.dict_len; i += 32) S.out[i] = seg.dict[i]; } // kCount: D0 is enough
         ifill = seg.start_bit >> 3;
         oflush = D0;
         ipos = seg.start_bit >> 3;
@@ -204,7 +208,7 @@ __device__ __forceinline__ void inflate_warp(InfShared &S, const uint8_t *__rest
         kind = 0;
     }
     if (pd.on) {
-        for (uint32_t i = lane; i < pd.len; i += 32) S.out[i] = pd.win[i];
+        if constexpr (!kCount) { for (uint32_t i = lane; i < pd.len; i += 32) S.out[i] = pd.win[i]; }
         if (window_bits < 0) { D0 = pd.len; oflush = opos = blk_out = D0; }
     }
     const uint32_t dict_id = pd.on ? *pd.id : 0u;
@@ -256,7 +260,10 @@ __device__ __forceinline__ void inflate_warp(InfShared &S, const uint8_t *__rest
                 if (mode == 5) { cmd = C_DONE; break; }
                 if constexpr (kRange) { if (opos >= rlim) { if (rg.to_end) FAIL(IE_LENGTH_CHECK); else mode = 5; continue; } }
                 if (ifill < n && ifill - ipos < 1024) { cmd = C_REFILL; break; }
-                if (opos - oflush >= kOutRing / 2 + 2048) { cmd = C_FLUSH; break; }
+                if (opos - oflush >= kOutRing / 2 + 2048) {
+                    if constexpr (kCount) { oflush += kOutRing / 2; continue; } // what C_FLUSH does to lane 0
+                    cmd = C_FLUSH; break;
+                }
                 if (consumed_bits > 8 * n) { FAIL(IE_TRUNCATED); continue; }
                 if (mode == 0) {
                     if (window_bits < 0) { mode = 1; continue; }
@@ -388,9 +395,9 @@ __device__ __forceinline__ void inflate_warp(InfShared &S, const uint8_t *__rest
                     while (stored_left && k < 4096) {
                         if constexpr (kRange) { if (opos >= rlim) break; }
                         if (ifill < n && ifill - ipos < 16) break;
-                        if (opos - D0 >= cap) { FAIL(IE_OUTPUT_FULL); break; }
+                        if (!kCount && opos - D0 >= cap) { FAIL(IE_OUTPUT_FULL); break; }
                         NEED(8);
-                        S.out[opos & (kOutRing - 1)] = (uint8_t)BITS(8);
+                        if constexpr (!kCount) S.out[opos & (kOutRing - 1)] = (uint8_t)BITS(8);
                         DROP(8);
                         opos++; stored_left--; k++;
                         if (consumed_bits > 8 * n) { FAIL(IE_TRUNCATED); break; }
@@ -413,8 +420,8 @@ __device__ __forceinline__ void inflate_warp(InfShared &S, const uint8_t *__rest
                         }
                         DROP(here.bits);
                         if (here.op == 0) {
-                            if (opos - D0 >= cap) { FAIL(IE_OUTPUT_FULL); break; }
-                            S.out[opos & (kOutRing - 1)] = (uint8_t)here.val;
+                            if (!kCount && opos - D0 >= cap) { FAIL(IE_OUTPUT_FULL); break; }
+                            if constexpr (!kCount) S.out[opos & (kOutRing - 1)] = (uint8_t)here.val;
                             opos++;
                             continue;
                         }
@@ -435,8 +442,9 @@ __device__ __forceinline__ void inflate_warp(InfShared &S, const uint8_t *__rest
                         ex = here.op & 15;
                         if (ex) { dist += BITS(ex); DROP(ex); }
                         if (dist > opos) { FAIL(IE_TOO_FAR); break; }
-                        if (opos - D0 + len > cap) { FAIL(IE_OUTPUT_FULL); break; }
+                        if (!kCount && opos - D0 + len > cap) { FAIL(IE_OUTPUT_FULL); break; }
                         if (consumed_bits > 8 * n) { FAIL(IE_TRUNCATED); break; }
+                        if constexpr (kCount) { opos += len; if (len >= 24) break; continue; } // a C_COPY ends the round too
                         if (len >= 24) { copy_len = len; copy_dist = dist; cmd = C_COPY; break; }
                         for (uint32_t j = 0; j < len; j++) S.out[(opos + j) & (kOutRing - 1)] = S.out[(opos + j - dist) & (kOutRing - 1)];
                         opos += len;
@@ -472,7 +480,9 @@ __device__ __forceinline__ void inflate_warp(InfShared &S, const uint8_t *__rest
             for (uint64_t i = lane; i < cnt; i += 32) S.in[(ifill + i) & (kInRing - 1)] = src[ifill + i];
             ifill += cnt;
             __syncwarp();
-        } else if (cmd == C_FLUSH || cmd == C_DONE) {
+        } else if (kCount && cmd == C_DONE) {
+            break;
+        } else if (!kCount && (cmd == C_FLUSH || cmd == C_DONE)) {
             const uint64_t opos0 = __shfl_sync(0xffffffffu, opos, 0);
             const uint64_t upto = cmd == C_DONE ? opos0 : oflush + kOutRing / 2; // the trigger guarantees opos0 >= upto
             const uint64_t end = upto - D0 > cap ? cap + D0 : upto;
@@ -485,7 +495,7 @@ __device__ __forceinline__ void inflate_warp(InfShared &S, const uint8_t *__rest
             if (end > oflush) oflush = end;
             __syncwarp();
             if (cmd == C_DONE) break;
-        } else if (cmd == C_COPY) {
+        } else if (!kCount && cmd == C_COPY) {
             const uint32_t len = __shfl_sync(0xffffffffu, copy_len, 0);
             const uint32_t dist = __shfl_sync(0xffffffffu, copy_dist, 0);
             const uint64_t o = __shfl_sync(0xffffffffu, opos, 0);
@@ -532,6 +542,13 @@ __global__ void __launch_bounds__(32) k_inflate(const uint8_t *__restrict__ src,
 {
     extern __shared__ __align__(16) uint8_t smem_raw[];
     inflate_warp(*reinterpret_cast<InfShared *>(smem_raw), src, n, dst, cap, window_bits, res, seg);
+}
+
+// zb_inflate_auto's serial path: the output length of a stream, ahead of the k_inflate that decodes it into a buffer of that length.
+__global__ void __launch_bounds__(32) k_inflate_count(const uint8_t *__restrict__ src, uint64_t n, int window_bits, InfState *res)
+{
+    extern __shared__ __align__(16) uint8_t smem_raw[];
+    inflate_warp<false, true>(*reinterpret_cast<InfShared *>(smem_raw), src, n, nullptr, 0, window_bits, res, InfSeg{0, nullptr, 0, 0});
 }
 
 // ================================================================================================
@@ -1237,7 +1254,9 @@ __global__ void __launch_bounds__(32) k_inf_tiles(const uint8_t *src, InfPar *pa
                 const uint32_t i = __ffs(m) - 1;
                 const uint32_t ee = sm_e[i], L = ee >> 16, D = ee & 0xffffu;
                 const uint64_t G = b.out_off + sm_c[i]; // where the copy starts in the output
-                if ((uint64_t)D > G) bad = true;         // "invalid distance too far back"
+                // "invalid distance too far back": the replay is discarded (decode_err); the copy is skipped, its source
+                // G + j - D would lie in front of the output
+                if ((uint64_t)D > G) { bad = true; continue; }
                 for (uint32_t j = lane; j < L; j += 32) {
                     const uint64_t g = G + j;
                     if (g < pos || g >= upto) continue;
@@ -1541,6 +1560,31 @@ __global__ void __launch_bounds__(32) k_batch_members(const uint8_t *__restrict_
     }
 }
 
+// zb_inflate_batch_auto: each item's output length (one warp per item), as its slot length out_cap.
+__global__ void __launch_bounds__(32) k_batch_count(const uint8_t *__restrict__ src, BatchItem *items, int window_bits, InfState *ist)
+{
+    extern __shared__ __align__(16) uint8_t smem_raw[];
+    const uint32_t i = blockIdx.x;
+    const BatchItem it = items[i];
+    inflate_warp<false, true>(*reinterpret_cast<InfShared *>(smem_raw), src + it.in_off, it.in_len, nullptr, 0, window_bits, ist + i,
+                              InfSeg{0, nullptr, 0, 0});
+    __syncwarp();
+    if (threadIdx.x == 0) items[i].out_cap = ist[i].out_bytes;
+}
+
+// ... and the slots packed back to back: out_off the exclusive prefix sum of out_cap, *total the sum (one CTA).
+__global__ void __launch_bounds__(1024) k_batch_slots(BatchItem *items, uint32_t n, uint64_t *total)
+{
+    __shared__ uint64_t ws[32];
+    const uint32_t per = (n + 1023) / 1024, beg = min(n, threadIdx.x * per), end = min(n, beg + per);
+    uint64_t sum = 0;
+    for (uint32_t i = beg; i < end; i++) sum += items[i].out_cap;
+    uint64_t all;
+    uint64_t run = cta_exclusive_scan(sum, ws, all);
+    for (uint32_t i = beg; i < end; i++) { items[i].out_off = run; run += items[i].out_cap; }
+    if (threadIdx.x == 0) *total = all;
+}
+
 // One thread per item: the status inflate_stream gives for it alone (the decoder's error, else the trailer checks) and its check.
 __global__ void __launch_bounds__(256) k_batch_verdict(const InfState *ist, const uint32_t *crc, const uint32_t *adler, uint32_t n,
                                                        BatchResult *out)
@@ -1656,6 +1700,10 @@ int Engine::inflate_init()
     if (e != cudaSuccess) { snprintf(g_err, sizeof g_err, "k_flushed_members attr: %s", cudaGetErrorString(e)); return ZB_E_CUDA; }
     e = cudaFuncSetAttribute(k_index_extract, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(InfShared));
     if (e != cudaSuccess) { snprintf(g_err, sizeof g_err, "k_index_extract attr: %s", cudaGetErrorString(e)); return ZB_E_CUDA; }
+    e = cudaFuncSetAttribute(k_inflate_count, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(InfShared));
+    if (e != cudaSuccess) { snprintf(g_err, sizeof g_err, "k_inflate_count attr: %s", cudaGetErrorString(e)); return ZB_E_CUDA; }
+    e = cudaFuncSetAttribute(k_batch_count, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(InfShared));
+    if (e != cudaSuccess) { snprintf(g_err, sizeof g_err, "k_batch_count attr: %s", cudaGetErrorString(e)); return ZB_E_CUDA; }
     if (cudaMalloc(&d_inf_state, sizeof(InfState)) != cudaSuccess) return ZB_E_MEM;
     if (cudaMallocHost(&h_inf_state, sizeof(InfState)) != cudaSuccess) return ZB_E_MEM;
     return ZB_OK;
@@ -1667,15 +1715,22 @@ int Engine::inflate_init()
         if (e_ != cudaSuccess) { snprintf(g_err, sizeof g_err, "%s: %s", #call, cudaGetErrorString(e_)); return ZB_E_CUDA; } \
     } while (0)
 
+// window_bits and flags that zb_inflate_ex (and zb_inflate_auto) accept
+static bool inflate_args_ok(int window_bits, uint32_t flags)
+{
+    if (window_bits < 0) { if (window_bits < -15 || window_bits > -8) return false; }
+    else if (window_bits != 0 && ((window_bits & 15) < 8) ) return false;
+    if (window_bits > 47) return false;
+    if ((flags & ZB_INF_MEMBERS) && (window_bits < 24 || window_bits > 31 || (flags & ZB_INF_NO_SERIAL))) return false;
+    return true;
+}
+
 int Engine::inflate(const void *src, size_t n, bool src_dev, void *dst, size_t dst_cap, bool dst_dev, int window_bits,
                     zb_inflate_result *res, uint32_t flags, IdxBuild *ib)
 {
     if (!res || (!src && n) || (!dst && dst_cap)) return ZB_E_PARAM;
     memset(res, 0, sizeof *res);
-    if (window_bits < 0) { if (window_bits < -15 || window_bits > -8) return ZB_E_PARAM; }
-    else if (window_bits != 0 && ((window_bits & 15) < 8) ) return ZB_E_PARAM;
-    if (window_bits > 47) return ZB_E_PARAM;
-    if ((flags & ZB_INF_MEMBERS) && (window_bits < 24 || window_bits > 31 || (flags & ZB_INF_NO_SERIAL))) return ZB_E_PARAM;
+    if (!inflate_args_ok(window_bits, flags)) return ZB_E_PARAM;
     CKI(cudaSetDevice(device));
     int rc;
     void *p;
@@ -1709,12 +1764,75 @@ int Engine::inflate(const void *src, size_t n, bool src_dev, void *dst, size_t d
     return status;
 }
 
+// The most a deflate stream can expand: a 258-byte copy in 2 bits (a 1-bit length code and a 1-bit distance code).
+constexpr uint64_t kMaxRatio = 1032;
+
+// The output buffer of zb_inflate_auto / zb_inflate_batch_auto (S_AUTO), grown to hold `bytes` with its first `keep` bytes kept.
+int Engine::grow_auto(size_t bytes, size_t keep, uint8_t **out)
+{
+    Buf &b = bufs[S_AUTO];
+    if (b.cap < bytes + 64) {
+        void *p = nullptr;
+        size_t want = bytes + 64 + (bytes >> 3) + 4096;
+        cudaError_t e = cudaMalloc(&p, want);
+        if (e != cudaSuccess) { cudaGetLastError(); want = bytes + 64; e = cudaMalloc(&p, want); } // no room for the slack
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            snprintf(g_err, sizeof g_err, "inflate auto: no device memory for %llu output bytes (%s)", (unsigned long long)bytes,
+                     cudaGetErrorString(e));
+            return ZB_E_MEM;
+        }
+        if (keep) {
+            CKI(cudaMemcpyAsync(p, b.p, keep, cudaMemcpyDeviceToDevice, st));
+            CKI(cudaStreamSynchronize(st));
+        }
+        if (b.p) cudaFree(b.p);
+        b.p = p;
+        b.cap = want;
+    }
+    *out = static_cast<uint8_t *>(b.p);
+    return ZB_OK;
+}
+
+// zb_inflate_auto: Engine::inflate with the output in S_AUTO, sized by the block chain or by a count pass (inflate_stream).
+int Engine::inflate_auto(const void *src, size_t n, bool src_dev, int window_bits, uint32_t flags, uint64_t max_out, zb_inflate_result *res,
+                         const void **out)
+{
+    if (!res || !out || (!src && n)) return ZB_E_PARAM;
+    memset(res, 0, sizeof *res);
+    *out = nullptr;
+    if (!inflate_args_ok(window_bits, flags)) return ZB_E_PARAM;
+    CKI(cudaSetDevice(device));
+    void *p;
+    int rc;
+    const uint8_t *d_src = static_cast<const uint8_t *>(src);
+    CKI(cudaEventRecord(ev0, st));
+    if (!src_dev) {
+        if ((rc = reserve(S_INF0, n + 64, &p)) != ZB_OK) return rc;
+        if (n) CKI(cudaMemcpyAsync(p, src, n, cudaMemcpyHostToDevice, st));
+        d_src = static_cast<const uint8_t *>(p);
+    }
+    launches = 0;
+    const uint64_t base = 0;
+    const int status = (flags & ZB_INF_MEMBERS) ? inflate_members(d_src, n, nullptr, max_out, window_bits, res, nullptr, true)
+                                                : inflate_stream(d_src, n, nullptr, max_out, window_bits, flags, res, nullptr, &base);
+    if (status != ZB_OK && status != ZB_E_BUF && status != ZB_E_DATA && status != ZB_E_DECLINED) return status;
+    CKI(cudaEventRecord(ev1, st));
+    CKI(cudaStreamSynchronize(st));
+    CKI(cudaEventElapsedTime(&res->gpu_ms, ev0, ev1));
+    res->status = status;
+    res->gpu_launches = launches;
+    *out = bufs[S_AUTO].p;
+    return status;
+}
+
 // ZB_INF_MEMBERS: every member of a gzip file, from offset 0 on, while the next two bytes are 1f 8b (gz_look, libz-rs-sys gz.rs).
 // Runs of BGZF members go through the batch (k_mem_* / k_members); a member the batch hands back, and any other member, through
 // inflate_stream at the current offset.  The error of a member is the one inflate_stream gives for it alone; out_bytes / in_bytes
 // and check cover the members in front of it.
+// automatic (zb_inflate_auto): the output goes to S_AUTO, grown member by member; dst_cap is the most accepted.
 int Engine::inflate_members(const uint8_t *d_src, size_t n, uint8_t *d_dst, size_t dst_cap, int window_bits, zb_inflate_result *res,
-                            InfTrace *tr)
+                            InfTrace *tr, bool automatic)
 {
     int rc;
     void *p;
@@ -1782,9 +1900,28 @@ int Engine::inflate_members(const uint8_t *d_src, size_t n, uint8_t *d_dst, size
             launches += 1;
             CKI(cudaMemcpyAsync(&h_ctl, d_ctl, sizeof h_ctl, cudaMemcpyDeviceToHost, st));
             CKI(cudaStreamSynchronize(st));
+            uint8_t *d_run = d_dst + out;
+            if (automatic && h_ctl.fit) {
+                // The run's slots come from its ISIZE hints, which nothing checks before the decode: a member's hint above
+                // what its bytes can inflate to (kMaxRatio : 1) is wrong, and the run stops in front of it, so that member
+                // takes inflate_stream's count path and the buffer never grows beyond what the input can produce.
+                std::vector<uint32_t> ml(h_ctl.fit), mi(h_ctl.fit);
+                CKI(cudaMemcpyAsync(ml.data(), d_mlen, 4 * (size_t)h_ctl.fit, cudaMemcpyDeviceToHost, st));
+                CKI(cudaMemcpyAsync(mi.data(), d_misz, 4 * (size_t)h_ctl.fit, cudaMemcpyDeviceToHost, st));
+                CKI(cudaStreamSynchronize(st));
+                uint32_t f = 0;
+                uint64_t run_out = 0;
+                while (f < h_ctl.fit && mi[f] <= kMaxRatio * ml[f]) run_out += mi[f++];
+                if (f < h_ctl.fit) {
+                    h_ctl.fit = f;
+                    CKI(cudaMemcpyAsync(&d_ctl->fit, &h_ctl.fit, 4, cudaMemcpyHostToDevice, st)); // k_mem_verdict reads it
+                }
+                if (f && (rc = grow_auto(out + run_out, out, &d_run)) != ZB_OK) return rc;
+                d_run += out;
+            }
             if (h_ctl.fit) {
-                k_members<<<h_ctl.fit, 32, sizeof(InfShared), st>>>(d_src, d_moff, d_mlen, d_misz, d_mout, d_dst + out, window_bits, d_mst);
-                CKI(launch_crc32_segments(d_dst + out, d_mout, d_misz, h_ctl.fit, d_mcrc, st));
+                k_members<<<h_ctl.fit, 32, sizeof(InfShared), st>>>(d_src, d_moff, d_mlen, d_misz, d_mout, d_run, window_bits, d_mst);
+                CKI(launch_crc32_segments(d_run, d_mout, d_misz, h_ctl.fit, d_mcrc, st));
                 k_mem_verdict<<<1, 1024, 0, st>>>(d_mst, d_mcrc, d_moff, d_mlen, d_misz, d_mout, d_ctl);
                 CKI(launch_crc32_join(d_mcrc, d_misz, &d_ctl->good, &d_ctl->good_crc, st));
                 launches += 4;
@@ -1811,9 +1948,11 @@ int Engine::inflate_members(const uint8_t *d_src, size_t n, uint8_t *d_dst, size
         }
         zb_inflate_result r;
         memset(&r, 0, sizeof r);
-        const int st1 = inflate_stream(d_src + in, n - in, d_dst + out, dst_cap - out, window_bits, 0, &r, tr);
+        const int st1 = automatic ? inflate_stream(d_src + in, n - in, nullptr, dst_cap - out, window_bits, 0, &r, tr, &out)
+                                  : inflate_stream(d_src + in, n - in, d_dst + out, dst_cap - out, window_bits, 0, &r, tr);
         if (st1 != ZB_OK) {
             if (st1 != ZB_E_BUF && st1 != ZB_E_DATA) return st1;
+            if (automatic && st1 == ZB_E_BUF) out += r.out_bytes; // over max_out: the length up to the end of this member
             status = st1;
             memcpy(res->msg, r.msg, sizeof res->msg);
             break;
@@ -1830,8 +1969,10 @@ int Engine::inflate_members(const uint8_t *d_src, size_t n, uint8_t *d_dst, size
 }
 
 // One stream at d_src[0, n) into d_dst[0, dst_cap): the block-parallel path, or k_inflate; then the check value and the trailer.
+// With auto_base (zb_inflate_auto) the block chain's total_out, or else a count pass (k_inflate_count), sizes S_AUTO before the
+// decode writes to it; an output longer than dst_cap is not decoded (ZB_E_BUF, res->out_bytes its length).
 int Engine::inflate_stream(const uint8_t *d_src, size_t n, uint8_t *d_dst, size_t dst_cap, int window_bits, uint32_t flags,
-                           zb_inflate_result *res, InfTrace *tr)
+                           zb_inflate_result *res, InfTrace *tr, const uint64_t *auto_base)
 {
     int rc;
     void *p;
@@ -1888,6 +2029,10 @@ int Engine::inflate_stream(const uint8_t *d_src, size_t n, uint8_t *d_dst, size_
             declined = hpar.status != PS_OK || hpar.nblocks == 0 ? "chain" : "capacity";
             if (hpar.status == PS_OK && hpar.nblocks > 0 && hpar.total_out <= dst_cap) {
                 declined = "decode";
+                if (auto_base) {
+                    if ((rc = grow_auto(*auto_base + hpar.total_out, *auto_base, &d_dst)) != ZB_OK) return rc;
+                    d_dst += *auto_base;
+                }
                 uint16_t *dtmp;
                 if ((rc = reserve(4 /*S_M*/, (hpar.total_out + 64) * 2, &p)) != ZB_OK) return rc;
                 dtmp = static_cast<uint16_t *>(p);
@@ -1935,6 +2080,17 @@ int Engine::inflate_stream(const uint8_t *d_src, size_t n, uint8_t *d_dst, size_
         snprintf(res->msg, sizeof res->msg, "%s", declined);
         return ZB_E_DECLINED;
     }
+    if (!done && auto_base) { // the exact length first, then the decode into a buffer of that length
+        k_inflate_count<<<1, 32, sizeof(InfShared), st>>>(d_src, n, window_bits, dis);
+        launches += 1;
+        CKI(cudaMemcpyAsync(his, dis, sizeof(InfState), cudaMemcpyDeviceToHost, st));
+        CKI(cudaStreamSynchronize(st));
+        CKI(cudaGetLastError());
+        if (his->out_bytes > dst_cap) { res->out_bytes = his->out_bytes; return ZB_E_BUF; }
+        dst_cap = his->out_bytes;
+        if ((rc = grow_auto(*auto_base + dst_cap, *auto_base, &d_dst)) != ZB_OK) return rc;
+        d_dst += *auto_base;
+    }
     if (!done) {
         k_inflate<<<1, 32, sizeof(InfShared), st>>>(d_src, n, d_dst, dst_cap, window_bits, dis, InfSeg{0, nullptr, 0, 0});
         launches += 1;
@@ -1976,12 +2132,19 @@ int Engine::inflate_stream(const uint8_t *d_src, size_t n, uint8_t *d_dst, size_
 // (zb_inflate_batch_dict: one that every item names; zb_inflate_batch_dicts: a table named item by item, DESIGN.md §2p) one more
 // launch gives the adler32 of every dictionary, the ids an FDICT header must name; the decoder preloads the last 32 KiB of the
 // item's dictionary as the window of a raw item and of a zlib item that names it.
+// zb_inflate_batch_auto (ba): before the decode, k_batch_count gives each item's output length as its slot length and k_batch_slots
+// packs the slots; one more host sync reads them, and the batch's output goes to S_AUTO.
 int Engine::inflate_batch(const DictTable &dt, const void *src, const uint64_t *src_off, size_t n_items, bool src_dev, void *dst,
-                          const uint64_t *dst_off, bool dst_dev, int window_bits, zb_inflate_result *items)
+                          const uint64_t *dst_off, bool dst_dev, int window_bits, zb_inflate_result *items, const BatchAuto *ba)
 {
     const bool per_item = dt.kind == DictTable::kPerItem;
-    const char *gn = per_item ? "inflate_batch_dicts" : "inflate_batch";
-    if (n_items && (!src_off || !dst_off || !items)) { snprintf(g_err, sizeof g_err, "%s: null argument", gn); return ZB_E_PARAM; }
+    const char *gn = ba ? "inflate_batch_auto" : per_item ? "inflate_batch_dicts" : "inflate_batch";
+    if (ba) {
+        if (!ba->dst_off || !ba->out) { snprintf(g_err, sizeof g_err, "%s: null argument", gn); return ZB_E_PARAM; }
+        *ba->out = nullptr;
+        ba->dst_off[0] = 0;
+    }
+    if (n_items && (!src_off || (!dst_off && !ba) || !items)) { snprintf(g_err, sizeof g_err, "%s: null argument", gn); return ZB_E_PARAM; }
     const uint32_t nd = (uint32_t)dt.n;
     uint64_t dict_bytes = 0;
     if (dt.kind == DictTable::kShared) {
@@ -2010,10 +2173,11 @@ int Engine::inflate_batch(const DictTable &dt, const void *src, const uint64_t *
     }
     const uint32_t nm = (uint32_t)n_items;
     for (uint32_t i = 0; i < nm; i++) {
-        if (src_off[i + 1] < src_off[i] || dst_off[i + 1] < dst_off[i]) { snprintf(g_err, sizeof g_err, "inflate_batch: offsets of item %u decrease", i); return ZB_E_PARAM; }
-        if (dst_off[i + 1] - dst_off[i] > 0xffffffffull) { snprintf(g_err, sizeof g_err, "inflate_batch: slot of item %u is 4 GiB or more", i); return ZB_E_PARAM; }
+        if (src_off[i + 1] < src_off[i] || (!ba && dst_off[i + 1] < dst_off[i])) { snprintf(g_err, sizeof g_err, "%s: offsets of item %u decrease", gn, i); return ZB_E_PARAM; }
+        if (!ba && dst_off[i + 1] - dst_off[i] > 0xffffffffull) { snprintf(g_err, sizeof g_err, "inflate_batch: slot of item %u is 4 GiB or more", i); return ZB_E_PARAM; }
     }
-    const uint64_t in_total = nm ? src_off[nm] - src_off[0] : 0, out_total = nm ? dst_off[nm] - dst_off[0] : 0;
+    const uint64_t in_total = nm ? src_off[nm] - src_off[0] : 0;
+    uint64_t out_total = nm && !ba ? dst_off[nm] - dst_off[0] : 0;
     if ((in_total && !src) || (out_total && !dst)) { snprintf(g_err, sizeof g_err, "inflate_batch: null buffer"); return ZB_E_PARAM; }
     for (uint32_t i = 0; i < nm; i++) memset(&items[i], 0, sizeof items[i]);
     if (nm == 0) return ZB_OK;
@@ -2053,10 +2217,12 @@ int Engine::inflate_batch(const DictTable &dt, const void *src, const uint64_t *
         if (item_which) memcpy(h_which, dt.which, (size_t)nm * 4);
     }
     for (uint32_t i = 0; i < nm; i++)
-        h_items[i] = BatchItem{src_off[i] - src_off[0], src_off[i + 1] - src_off[i], dst_off[i] - dst_off[0], dst_off[i + 1] - dst_off[i]};
+        h_items[i] = ba ? BatchItem{src_off[i] - src_off[0], src_off[i + 1] - src_off[i], 0, 0}
+                        : BatchItem{src_off[i] - src_off[0], src_off[i + 1] - src_off[i], dst_off[i] - dst_off[0], dst_off[i + 1] - dst_off[i]};
     // the item offsets index the caller's buffers: a host buffer is copied (or staged) as one range
     const uint8_t *d_src = static_cast<const uint8_t *>(src) + (nm ? src_off[0] : 0);
-    uint8_t *d_dst = static_cast<uint8_t *>(dst) + dst_off[0];
+    uint8_t *d_dst = ba ? nullptr : static_cast<uint8_t *>(dst) + dst_off[0];
+    if (ba) dst_dev = true; // S_AUTO
     CKI(cudaEventRecord(ev0, st));
     if (!src_dev) {
         if ((rc = reserve(S_INF0, in_total + 64, &p)) != ZB_OK) return rc;
@@ -2080,6 +2246,24 @@ int Engine::inflate_batch(const DictTable &dt, const void *src, const uint64_t *
         CKI(launch_adler32_segments(d_dict, d_doff, d_dlen, nd, d_dictid, st));
         launches++;
         idt = InfDicts{d_dict, d_doff, d_dictid, item_which ? d_which : nullptr, nd, per_item ? kDictById : 0u};
+    }
+    if (ba) {
+        uint64_t *d_total = static_cast<uint64_t *>(d_inf_state), *h_total = static_cast<uint64_t *>(h_inf_state);
+        k_batch_count<<<nm, 32, sizeof(InfShared), st>>>(d_src, d_items, window_bits, d_ist);
+        k_batch_slots<<<1, 1024, 0, st>>>(d_items, nm, d_total);
+        launches += 2;
+        CKI(cudaMemcpyAsync(h_items, d_items, (size_t)nm * sizeof(BatchItem), cudaMemcpyDeviceToHost, st));
+        CKI(cudaMemcpyAsync(h_total, d_total, 8, cudaMemcpyDeviceToHost, st));
+        CKI(cudaStreamSynchronize(st));
+        CKI(cudaGetLastError());
+        out_total = *h_total;
+        for (uint32_t i = 0; i < nm; i++) ba->dst_off[i] = h_items[i].out_off;
+        ba->dst_off[nm] = out_total;
+        if (out_total > ba->max_out) return ZB_E_BUF;
+        for (uint32_t i = 0; i < nm; i++)
+            if (h_items[i].out_cap > 0xffffffffull) { snprintf(g_err, sizeof g_err, "%s: item %u decodes to 4 GiB or more", gn, i); return ZB_E_PARAM; }
+        if ((rc = grow_auto(out_total, 0, &d_dst)) != ZB_OK) return rc;
+        *ba->out = d_dst;
     }
     k_batch_members<<<nm, 32, sizeof(InfShared), st>>>(d_src, d_items, d_dst, window_bits, d_ist, d_ooff, d_clen, d_alen, idt);
     CKI(launch_crc32_segments(d_dst, d_ooff, d_clen, nm, d_crc, st));
