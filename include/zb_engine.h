@@ -437,6 +437,79 @@ ZB_API int zb_index_get_info(const zb_index *idx, zb_index_info *info);
 ZB_API int zb_index_get_point(const zb_index *idx, size_t i, zb_index_point *p);
 ZB_API void zb_index_free(zb_index *idx);
 
+/* ZIP archives (DESIGN.md §2r; PKWARE APPNOTE.TXT: .zip, .jar, wheels, Office documents, numpy.savez_compressed files).  An entry
+ * is a raw deflate (method 8) or stored (method 0) payload whose crc32 and sizes the central directory holds.
+ *
+ * zb_zip_open: the archive src[0, src_len) (host, or device with src_on_device) read into *out.  The end of central directory
+ *   record is the last "PK\5\6" in the final 65557 bytes whose comment reaches exactly to the end; a ZIP64 locator in front of it
+ *   gives the ZIP64 record, whose values replace the fields at 0xFFFF / 0xFFFFFFFF, and an entry's ZIP64 extra field replaces its
+ *   sizes and offset at 0xFFFFFFFF (APPNOTE 4.5.3 order).  Every local header must have "PK\3\4", the directory's method and name
+ *   bytes, and data (at local offset + 30 + its name and extra lengths) inside the input in front of the central directory; no two
+ *   entries may overlap.  A malformed archive gives ZB_E_DATA, a multi-disk one ZB_E_PARAM, both with *out = NULL and a message
+ *   naming the offset in res->msg and zb_last_error().  Encrypted entries, methods other than 0 and 8, and data descriptors (bit 3)
+ *   do not fail the open.  A host source is walked on the host (0 launches, nothing uploaded: an archive larger than device memory
+ *   opens).  A device source copies back only its tail (65577 bytes at most: the longest EOCD and a ZIP64 locator), the ZIP64 record and the central directory, and
+ *   checks the local headers on the device: 1 launch (k_zip_local, none for an empty archive) and at most 4 host syncs.
+ * zb_zip_extract: decode entries which[i] (host, n_which entries; NULL: entry i for i < n_which) of an archive opened from the same
+ *   src_len bytes into slots dst[dst_off[i], dst_off[i+1]) (dst_off host, n_which + 1 entries), as zb_inflate_flushed does; a host dst
+ *   is written whole, zeros behind each output.  items[i]:
+ *     ZB_OK      the output is exactly the directory's uncompressed size, its crc32 is the directory's, and a deflated entry's final
+ *                block ends exactly at its compressed size;
+ *     ZB_E_DATA  the decoder's message, "incorrect data check", "incorrect length check" or "entry data does not end at its
+ *                compressed size";
+ *     ZB_E_BUF   the slot is smaller than the uncompressed size (nothing decoded);
+ *     ZB_E_PARAM "unsupported compression method" or "encrypted entry" (flag bit 0).
+ *   out_bytes, in_bytes (compressed bytes consumed) and check (crc32 of the output) are filled.  One bad entry never changes another's
+ *   result; returns ZB_OK or the status of the first entry that failed.  which[i] out of range, more than 2^20 items, or src_len not
+ *   the opened archive's length give ZB_E_PARAM.  A host source is not uploaded whole: only the selected entries' payloads go up --
+ *   those below ZB_ZIP_WARP_MAX compressed bytes packed through the engine's pinned staging in one copy (so the staging grows to
+ *   their sum, not to the archive's size), larger ones one copy each straight from src.  Paths: stored entries below
+ *   ZB_ZIP_WARP_MAX bytes are copied by k_zip_stored, deflated entries below ZB_ZIP_WARP_MAX bytes of output decode one warp each
+ *   (k_zip_members), crc32s come from k_crc_segments and statuses from k_zip_verdict -- at most 4 launches and 1 host sync
+ *   whatever their number.  A larger stored entry is a device copy and a crc32 (2 launches).  A larger deflated entry takes the
+ *   block-parallel decoder alone, as zb_inflate_ex(-15, ZB_INF_CHECK_CRC | ZB_INF_NO_SERIAL) would; when that declines (stored or
+ *   fixed-code blocks, damage) the entry joins the one-warp group, or, with 4 GiB of output or more, takes the serial decoder.
+ * zb_zip_write: an archive of n_items entries: entry i is src[src_off[i], src_off[i+1]) (src_off host, n_items + 1 offsets; src host
+ *   or device) named names[name_off[i], name_off[i+1]) (host, 1..65535 bytes, written as given; duplicates are allowed).  Level 0
+ *   stores (method 0); levels -1 and 1..9 deflate (method 8) each entry alone, byte for byte the reference's deflateInit2(level,
+ *   Z_DEFLATED, -15, 8, Z_DEFAULT_STRATEGY) + deflate(Z_FINISH) -- the payload zipfile writes at compresslevel=level.  Headers:
+ *   version needed 20 (45 with ZIP64), flags 0 (| 0x800 when the name has a byte >= 0x80), DOS time 0 and date 0x0021, crc32 and
+ *   sizes in the local header, no data descriptors, version made by 0x0314, external attributes 0o100644 << 16.  The central
+ *   directory follows in input order, then the end records; a ZIP64 EOCD and locator are written exactly when the entry count is
+ *   0xFFFF or more or the directory's size or offset 0xFFFFFFFF or more, and an entry carries the ZIP64 extra field exactly when
+ *   one of its fields reaches 0xFFFFFFFF (zb_zip.h has the bytes).  entry_off (host, n_items + 1) gets each local header offset and,
+ *   last, the central directory's.  res: out_bytes (the archive's length), n_blocks, n_symbols, gpu_launches, gpu_ms,
+ *   exact_parity = 1.  An empty name, more than 2^32 entries, a level outside -1..9: ZB_E_PARAM with a zb_last_error() text.
+ *   dst_cap below the archive's length: ZB_E_BUF with res->out_bytes the length needed; zb_zip_bound is always enough.
+ *   Entries of at most 65536 bytes are compressed side by side through zb_deflate_batch's kernels, in runs of consecutive such
+ *   entries (at most 65535 entries and 2^31 bytes a run); a larger entry takes zb_deflate_ex(-15, ZB_FLAG_CHECK_CRC) alone, which
+ *   takes at most 0xF0000000 bytes: a longer entry at a level other than 0 gives ZB_E_PARAM before anything runs (level 0 stores
+ *   entries of any size).  Then
+ *   k_crc_segments gives the small entries' crc32s and k_zip_frame writes every header, the directory and the end records in one
+ *   launch.  A host source is uploaded once. */
+#define ZB_ZIP_WARP_MAX (1u << 20) /* zb_zip_extract: stored entries below this many bytes, and deflated entries below this many
+                                      output bytes, are decoded side by side in one group */
+typedef struct zb_zip zb_zip;
+typedef struct zb_zip_info {
+    uint64_t n_entries, cd_offset, cd_size, src_len;
+} zb_zip_info;
+typedef struct zb_zip_entry {
+    const uint8_t *name; /* name_len bytes as stored (UTF-8 when flags has bit 11), valid as long as the archive object */
+    uint32_t name_len, method, flags, crc32;
+    uint64_t compressed_size, uncompressed_size, local_offset, data_offset;
+    uint32_t dos_time, dos_date, external_attr, reserved;
+} zb_zip_entry;
+ZB_API int zb_zip_open(zb_engine *e, const void *src, size_t src_len, int src_on_device, zb_inflate_result *res, zb_zip **out);
+ZB_API int zb_zip_get_info(const zb_zip *z, zb_zip_info *info);
+ZB_API int zb_zip_get_entry(const zb_zip *z, size_t i, zb_zip_entry *entry);
+ZB_API int zb_zip_extract(zb_engine *e, const zb_zip *z, const void *src, size_t src_len, int src_on_device, const uint64_t *which,
+                          size_t n_which, void *dst, const uint64_t *dst_off, int dst_on_device, zb_inflate_result *items);
+ZB_API void zb_zip_free(zb_zip *z);
+ZB_API int zb_zip_write(zb_engine *e, const void *src, const uint64_t *src_off, size_t n_items, int src_on_device, const void *names,
+                        const uint64_t *name_off, int level, void *dst, size_t dst_cap, int dst_on_device, uint64_t *entry_off,
+                        zb_deflate_result *res);
+ZB_API size_t zb_zip_bound(const uint64_t *src_off, const uint64_t *name_off, size_t n_items);
+
 /* Chunk-sharded deflate with the one-stream bytes (levels 7..9; see DESIGN.md §5).  One input of total_len bytes is cut into
  * contiguous ranges [S_r, E_r), one per rank (every range but the last >= 64 KiB); each rank runs the four calls below on its
  * own engine, and the caller moves the small records between them (the library has no transport):

@@ -11,6 +11,7 @@ The names and argument meaning follow the reference's own API for this path:
 
 There is NO CPU fallback: if the shared library is missing, or no CUDA device is usable, the calls raise.
 """
+import collections
 import ctypes
 import os
 
@@ -33,6 +34,7 @@ ZB_INF_CHECK_CRC = 2
 ZB_INF_NO_SERIAL = 4  # Engine.inflate: only the block-parallel decoder; ZB_E_DECLINED with the stage in res.msg when it gives up
 ZB_INF_MEMBERS = 8  # Engine.inflate with gzip framing: every member of the file; runs of BGZF members decoded side by side
 ZB_E_DECLINED = -103
+ZIP_WARP_MAX = 1 << 20  # ZB_ZIP_WARP_MAX: Engine.zip_extract decodes deflated entries below this many output bytes one warp each
 
 
 class ZStream(ctypes.Structure):
@@ -89,6 +91,23 @@ class BatchParams(ctypes.Structure):
     """deflateInit2 parameters of one item of Engine.deflate_batch_params (zb_batch_params)."""
     _fields_ = [("level", ctypes.c_int32), ("strategy", ctypes.c_int32), ("window_bits", ctypes.c_int32),
                 ("mem_level", ctypes.c_int32)]
+
+
+class ZipInfoC(ctypes.Structure):
+    _fields_ = [("n_entries", ctypes.c_uint64), ("cd_offset", ctypes.c_uint64), ("cd_size", ctypes.c_uint64),
+                ("src_len", ctypes.c_uint64)]
+
+
+class ZipEntryC(ctypes.Structure):
+    _fields_ = [("name", ctypes.c_void_p), ("name_len", ctypes.c_uint32), ("method", ctypes.c_uint32), ("flags", ctypes.c_uint32),
+                ("crc32", ctypes.c_uint32), ("compressed_size", ctypes.c_uint64), ("uncompressed_size", ctypes.c_uint64),
+                ("local_offset", ctypes.c_uint64), ("data_offset", ctypes.c_uint64), ("dos_time", ctypes.c_uint32),
+                ("dos_date", ctypes.c_uint32), ("external_attr", ctypes.c_uint32), ("reserved", ctypes.c_uint32)]
+
+
+ZipEntry = collections.namedtuple("ZipEntry", "name method flags crc32 compressed_size uncompressed_size local_offset data_offset "
+                                              "dos_time dos_date external_attr")
+ZipEntry.__doc__ = "One central directory entry of a ZipArchive: name (bytes as stored), ZIP64 fields resolved, data_offset from its local header."
 
 
 class ZlibError(Exception):
@@ -192,6 +211,15 @@ def lib():
             u64p = ctypes.POINTER(u64)
             L.zb_deflate_batch_dicts.argtypes = [vp, vp, u64p, sz, ctypes.POINTER(u32)] + L.zb_deflate_batch.argtypes[1:]
             L.zb_inflate_batch_dicts.argtypes = [vp, vp, u64p, sz, ctypes.POINTER(u32)] + L.zb_inflate_batch.argtypes[1:]
+        if hasattr(L, "zb_zip_open"):
+            u64p = ctypes.POINTER(u64)
+            L.zb_zip_open.argtypes = [vp, vp, sz, ci, ctypes.POINTER(InflateResult), ctypes.POINTER(vp)]
+            L.zb_zip_get_info.argtypes = [vp, ctypes.POINTER(ZipInfoC)]
+            L.zb_zip_get_entry.argtypes = [vp, sz, ctypes.POINTER(ZipEntryC)]
+            L.zb_zip_extract.argtypes = [vp, vp, vp, sz, ci, u64p, sz, vp, u64p, ci, ctypes.POINTER(InflateResult)]
+            L.zb_zip_free.argtypes, L.zb_zip_free.restype = [vp], None
+            L.zb_zip_write.argtypes = [vp, vp, u64p, sz, ci, vp, u64p, ci, vp, sz, ci, u64p, ctypes.POINTER(DeflateResult)]
+            L.zb_zip_bound.argtypes, L.zb_zip_bound.restype = [u64p, u64p, sz], sz
         L.zb_adler32.argtypes = [vp, u32, vp, sz, ci, ctypes.POINTER(u32), ctypes.POINTER(ctypes.c_float)]
         L.zb_crc32.argtypes = [vp, u32, vp, sz, ci, ctypes.POINTER(u32), ctypes.POINTER(ctypes.c_float)]
         L.zb_engine_set_profile.argtypes = [vp, ci]
@@ -552,6 +580,35 @@ class Index:
             pass
 
 
+class ZipArchive:
+    """An opened ZIP archive (zb_zip_open): its entries, read from the central directory and checked against their local headers.
+    Host memory; Engine.zip_extract decodes entries of it from the same source bytes."""
+
+    def __init__(self, handle):
+        self.h = handle
+        info = ZipInfoC()
+        lib().zb_zip_get_info(self.h, ctypes.byref(info))
+        self.cd_offset, self.cd_size, self.src_len = info.cd_offset, info.cd_size, info.src_len
+        self.entries = []
+        e = ZipEntryC()
+        for i in range(info.n_entries):
+            lib().zb_zip_get_entry(self.h, i, ctypes.byref(e))
+            self.entries.append(ZipEntry(ctypes.string_at(e.name, e.name_len) if e.name_len else b"", e.method, e.flags, e.crc32,
+                                         e.compressed_size, e.uncompressed_size, e.local_offset, e.data_offset, e.dos_time,
+                                         e.dos_date, e.external_attr))
+
+    def close(self):
+        if self.h:
+            lib().zb_zip_free(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 # ---------------------------------------------------------------- low-level engine (device-resident buffers)
 class Engine:
     def __init__(self, device=0):
@@ -902,6 +959,87 @@ class Engine:
                 p = e
             res.append(b"".join(parts))
         return res
+
+    def zip_open(self, src, n=None, src_on_device=False):
+        """Open a ZIP archive (zb_zip_open): host bytes or a writable buffer (not copied), or a device pointer with `n` (or a
+        (pointer, n) pair).  Returns a ZipArchive; a malformed archive raises ZlibError (Z_DATA_ERROR, or Z_STREAM_ERROR for a
+        multi-disk one) with the message naming the offset."""
+        if src_on_device:
+            if isinstance(src, tuple):
+                src, n = src
+            addr, keep = src, None
+        else:
+            addr, n, keep = _host_view(src)
+        res = InflateResult()
+        h = ctypes.c_void_p()
+        rc = lib().zb_zip_open(self.h, addr, n, int(src_on_device), ctypes.byref(res), ctypes.byref(h))
+        if rc != 0:
+            raise ZlibError(rc, lib().zb_last_error().decode())
+        return ZipArchive(h.value)
+
+    def zip_extract(self, src, archive, which=None, n=None, src_on_device=False, dst=None, dst_off=None, dst_on_device=False):
+        """Decode entries `which` (indices; None: all) of `archive` from `src`, the bytes it was opened from (zb_zip_extract), each
+        into a slot of its uncompressed size; a caller's `dst` (host or, with dst_on_device, device) takes `dst_off` (len(which) + 1
+        offsets) instead.  Returns (rc, [bytes] or None, [InflateResult]): rc is Z_OK or the status of the first entry that failed,
+        and every entry carries its own status and message."""
+        if src_on_device:
+            if isinstance(src, tuple):
+                src, n = src
+            addr, keep = src, None
+        else:
+            addr, n, keep = _host_view(src)
+        which = list(range(len(archive.entries))) if which is None else list(which)
+        k = len(which)
+        own = None
+        if dst is None:
+            doff = _offsets([archive.entries[i].uncompressed_size if 0 <= i < len(archive.entries) else 0 for i in which])
+            own = ctypes.create_string_buffer(max(doff[k], 1))
+            dst = ctypes.addressof(own)
+            dst_on_device = False
+        else:
+            doff = (ctypes.c_uint64 * len(dst_off))(*dst_off)
+        w = (ctypes.c_uint64 * max(k, 1))(*which)
+        res = (InflateResult * max(k, 1))()
+        rc = lib().zb_zip_extract(self.h, archive.h, addr, n, int(src_on_device), w, k, dst, doff, int(dst_on_device), res)
+        results = list(res)[:k]
+        if rc != 0 and not any(r.status == rc for r in results):
+            raise ZlibError(rc, lib().zb_last_error().decode())
+        if own is None:
+            return rc, None, results
+        raw = own.raw
+        return rc, [raw[doff[i]:doff[i] + results[i].out_bytes] for i in range(k)], results
+
+    def zip_write(self, entries, level=6, src_on_device=False, src_off=None, dst=None, dst_cap=0, dst_on_device=False):
+        """Write a ZIP archive of [(name, data), ...] (zb_zip_write): names are str (UTF-8) or bytes, level 0 stores and -1, 1..9
+        deflate each entry as zipfile does at that compresslevel.  With src_on_device, `entries` is (names, device pointer) and
+        `src_off` the n + 1 offsets.  Returns (bytes or None, DeflateResult, entry_off): entry_off holds each local header's offset
+        and, last, the central directory's.  Raises ZlibError (.needed: the size a too small dst_cap would have to be)."""
+        if src_on_device:
+            names, ptr = entries
+            off = (ctypes.c_uint64 * len(src_off))(*src_off)
+            keep = None
+        else:
+            names = [e[0] for e in entries]
+            keep, off = _gather([e[1] for e in entries])
+            ptr = ctypes.addressof(keep)
+        names = [x.encode() if isinstance(x, str) else bytes(x) for x in names]
+        nkeep, noff = _gather(names)
+        nn = len(names)
+        own = None
+        if dst is None:
+            dst_cap = lib().zb_zip_bound(off, noff, nn) + 64
+            own = ctypes.create_string_buffer(dst_cap)
+            dst = ctypes.addressof(own)
+            dst_on_device = False
+        res = DeflateResult()
+        eoff = (ctypes.c_uint64 * (nn + 1))()
+        rc = lib().zb_zip_write(self.h, ptr, off, nn, int(src_on_device), nkeep, noff, level, dst, dst_cap, int(dst_on_device), eoff,
+                                ctypes.byref(res))
+        if rc != 0:
+            e = ZlibError(rc, lib().zb_last_error().decode())
+            e.needed = res.out_bytes
+            raise e
+        return (own.raw[: res.out_bytes] if own is not None else None), res, list(eoff)
 
     def build_index(self, src, out_cap, span=1 << 20, window_bits=15, flags=0, n=None, src_on_device=False, dst=None,
                     dst_on_device=False):

@@ -8,6 +8,7 @@
 #include <vector>
 #include "../../include/zb_engine.h"
 #include "zb_index.h"
+#include "zb_zip.h"
 #include "zb_kernels.cuh"
 
 namespace zb {
@@ -24,6 +25,10 @@ enum { S_IN, S_L, S_HOLES, S_HOLESN, S_M, S_NXT, S_PEXIT, S_PCNT, S_SYMIDX, S_TE
        S_INDEX,        // index build: jobs, hits and points; extract: pieces, decoder states, windows and staged input
        S_INDEXW,       // index build: the windows of the points
        S_AUTO,         // zb_inflate_auto / zb_inflate_batch_auto: the output, sized to what the stream or batch decodes to
+       S_ZIPIN,        // zb_zip_*: a host source's bytes (the selected entries' payloads on extract, the input on write)
+       S_ZIPPAY,       // zb_zip_write: the compressed payloads
+       S_ZIPOUT,       // zb_zip_write: the archive for a host dst; zb_zip_extract: the slots for a host dst
+       S_ZIPTAB,       // zb_zip_*: entry tables, names and results
        S_COUNT };
 
 // A range job of chunk-sharded deflate (zb_shard_*, zb_shard.cu) between its four calls.
@@ -96,7 +101,7 @@ struct Readback {
 };
 
 struct Engine {
-    static constexpr int kSlots = 45;
+    static constexpr int kSlots = 49;
     struct Buf { void *p = nullptr; size_t cap = 0; };
     int device = -1;
     cudaStream_t st = nullptr, st2 = nullptr; // st2: the serial tail runs beside k_emit
@@ -203,6 +208,11 @@ struct Engine {
     int inflate_blocks(const void *src, size_t n, uint64_t start_bit, const void *dict, size_t dict_len, void *dst, size_t dst_cap,
                        int check_kind, uint32_t check_start, zb_inflate_seg *out);
     int checksum(bool crc, uint32_t start, const void *buf, size_t len, bool on_dev, uint32_t *out, float *ms);
+    int zip_open(const void *src, size_t n, bool src_dev, zb_inflate_result *res, zb_zip **out);
+    int zip_extract(const zb_zip *z, const void *src, size_t src_len, bool src_dev, const uint64_t *which, size_t n_which, void *dst,
+                    const uint64_t *dst_off, bool dst_dev, zb_inflate_result *items);
+    int zip_write(const void *src, const uint64_t *src_off, size_t n, bool src_dev, const void *names, const uint64_t *name_off, int level,
+                  void *dst, size_t dst_cap, bool dst_dev, uint64_t *entry_off, zb_deflate_result *res);
     ShardState shard;
     int shard_parse(const void *src, size_t total, bool src_dev, size_t S, size_t E, int level, int strategy, uint32_t flags,
                     zb_shard_entry *table, uint32_t *adler);
@@ -223,4 +233,12 @@ struct zb_index {
     std::vector<zb::IdxPoint> p;
     std::vector<uint64_t> woff;
     std::vector<uint8_t> win;
+};
+
+// An opened ZIP archive (zb_zip_* in zb_engine.h): host memory, read-only.  Entry i's name is names[name_off[i], name_off[i+1]).
+struct zb_zip {
+    std::vector<zb::zip::Entry> e;
+    std::vector<uint8_t> names;
+    std::vector<uint64_t> name_off;
+    uint64_t src_len = 0, cd_off = 0, cd_size = 0;
 };

@@ -1660,6 +1660,9 @@ __global__ void __launch_bounds__(256) k_flushed_verdict(const uint8_t *__restri
 
 struct IdxPiece;
 __global__ void __launch_bounds__(32) k_index_extract(const IdxPiece *pieces, InfState *st);
+struct ZipItem;
+__global__ void __launch_bounds__(32) k_zip_members(const uint8_t *__restrict__ src, const ZipItem *items, uint8_t *__restrict__ dst,
+                                                    InfState *ist, uint64_t *out_off, uint32_t *crc_len);
 
 static const char *inf_msg(uint32_t e)
 {
@@ -1698,6 +1701,8 @@ int Engine::inflate_init()
     if (e != cudaSuccess) { snprintf(g_err, sizeof g_err, "k_batch_members attr: %s", cudaGetErrorString(e)); return ZB_E_CUDA; }
     e = cudaFuncSetAttribute(k_flushed_members, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(InfShared));
     if (e != cudaSuccess) { snprintf(g_err, sizeof g_err, "k_flushed_members attr: %s", cudaGetErrorString(e)); return ZB_E_CUDA; }
+    e = cudaFuncSetAttribute(k_zip_members, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(InfShared));
+    if (e != cudaSuccess) { snprintf(g_err, sizeof g_err, "k_zip_members attr: %s", cudaGetErrorString(e)); return ZB_E_CUDA; }
     e = cudaFuncSetAttribute(k_index_extract, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(InfShared));
     if (e != cudaSuccess) { snprintf(g_err, sizeof g_err, "k_index_extract attr: %s", cudaGetErrorString(e)); return ZB_E_CUDA; }
     e = cudaFuncSetAttribute(k_inflate_count, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(InfShared));
@@ -2387,6 +2392,275 @@ int Engine::inflate_flushed(const void *src, size_t src_len, bool src_dev, const
         r.gpu_launches = launches;
         r.gpu_ms = ms;
         if (status == ZB_OK) status = r.status;
+    }
+    return status;
+}
+
+// ================================================================================================
+// ZIP entries (zb_zip_extract, DESIGN.md §2r).  Stored entries below ZB_ZIP_WARP_MAX bytes, deflated entries below ZB_ZIP_WARP_MAX
+// bytes of output, and the deflated entries the block-parallel decoder declines, form one group whatever their number:
+//   k_zip_stored     one CTA per stored entry: its bytes, min(compressed, uncompressed size) of them, into its slot;
+//   k_zip_members    one warp per deflated entry: inflate_warp in raw mode, the output capped at the directory's size;
+//   k_crc_segments   the crc32 of each output;
+//   k_zip_verdict    one status per entry against the directory's crc32 and sizes.
+// Larger entries go one by one: a device copy for a stored one, inflate_stream for a deflated one.
+// ================================================================================================
+struct ZipItem {
+    uint64_t in_off, in_len, out_off, usize;
+    uint32_t crc, stored;
+};
+constexpr uint32_t kZipBadEnd = 0xfffeu; // BatchResult::err of a deflated entry whose final block does not end at its compressed size
+
+__global__ void __launch_bounds__(256) k_zip_stored(const uint8_t *__restrict__ src, const ZipItem *items, uint8_t *__restrict__ dst,
+                                                    InfState *ist, uint64_t *out_off, uint32_t *crc_len)
+{
+    const ZipItem it = items[blockIdx.x];
+    const uint64_t n = it.in_len < it.usize ? it.in_len : it.usize;
+    const uint8_t *s = src + it.in_off;
+    uint8_t *d = dst + it.out_off;
+    for (uint64_t k = threadIdx.x; k < n; k += 256) d[k] = s[k];
+    if (threadIdx.x == 0) {
+        InfState &r = ist[blockIdx.x];
+        r.out_bytes = n;
+        r.in_bytes = n;
+        r.err = it.in_len > it.usize ? IE_OUTPUT_FULL : IE_OK;
+        out_off[blockIdx.x] = it.out_off;
+        crc_len[blockIdx.x] = (uint32_t)n; // stored entries in the group are below ZB_ZIP_WARP_MAX bytes
+    }
+}
+
+__global__ void __launch_bounds__(32) k_zip_members(const uint8_t *__restrict__ src, const ZipItem *items, uint8_t *__restrict__ dst,
+                                                    InfState *ist, uint64_t *out_off, uint32_t *crc_len)
+{
+    extern __shared__ __align__(16) uint8_t smem_raw[];
+    const uint32_t i = blockIdx.x;
+    const ZipItem it = items[i];
+    inflate_warp(*reinterpret_cast<InfShared *>(smem_raw), src + it.in_off, it.in_len, dst + it.out_off, it.usize, -15, ist + i,
+                 InfSeg{0, nullptr, 0, 0});
+    __syncwarp();
+    if (threadIdx.x == 0) {
+        const InfState &r = ist[i];
+        out_off[i] = it.out_off;
+        crc_len[i] = r.err == IE_OUTPUT_FULL ? 0u : (uint32_t)r.out_bytes; // the group's outputs are below 4 GiB (host check)
+    }
+}
+
+__global__ void __launch_bounds__(256) k_zip_verdict(const ZipItem *items, const InfState *ist, const uint32_t *crc, uint32_t n,
+                                                     BatchResult *out)
+{
+    const uint32_t i = blockIdx.x * 256 + threadIdx.x;
+    if (i >= n) return;
+    const InfState &r = ist[i];
+    const ZipItem it = items[i];
+    uint32_t err = r.err;
+    if (err == IE_OUTPUT_FULL) err = IE_LENGTH_CHECK; // the data holds more than the directory's uncompressed size
+    else if (err == IE_OK) {
+        if (r.in_bytes != it.in_len) err = it.stored ? (uint32_t)IE_LENGTH_CHECK : kZipBadEnd;
+        else if (r.out_bytes != it.usize) err = IE_LENGTH_CHECK;
+        else if (crc[i] != it.crc) err = IE_DATA_CHECK;
+    }
+    out[i] = BatchResult{r.out_bytes, r.in_bytes, crc[i], err};
+}
+
+static const char *zip_msg(uint32_t e) { return e == kZipBadEnd ? "entry data does not end at its compressed size" : inf_msg(e); }
+
+// zb_zip_extract: see zb_engine.h.
+int Engine::zip_extract(const zb_zip *z, const void *src, size_t src_len, bool src_dev, const uint64_t *which, size_t n_which, void *dst,
+                        const uint64_t *dst_off, bool dst_dev, zb_inflate_result *items)
+{
+    if (!z || (n_which && (!dst_off || !items))) { snprintf(g_err, sizeof g_err, "zip_extract: null argument"); return ZB_E_PARAM; }
+    if (src_len != z->src_len) {
+        snprintf(g_err, sizeof g_err, "zip_extract: %zu source bytes, the archive was opened from %llu", src_len, (unsigned long long)z->src_len);
+        return ZB_E_PARAM;
+    }
+    if (n_which > kBatchMaxInflateItems) {
+        snprintf(g_err, sizeof g_err, "zip_extract: %zu items (at most %llu)", n_which, (unsigned long long)kBatchMaxInflateItems);
+        return ZB_E_PARAM;
+    }
+    const uint32_t nw = (uint32_t)n_which;
+    for (uint32_t i = 0; i < nw; i++) {
+        if (which && which[i] >= z->e.size()) {
+            snprintf(g_err, sizeof g_err, "zip_extract: item %u names entry %llu of %zu", i, (unsigned long long)which[i], z->e.size());
+            return ZB_E_PARAM;
+        }
+        if (!which && i >= z->e.size()) { snprintf(g_err, sizeof g_err, "zip_extract: %u items, %zu entries", nw, z->e.size()); return ZB_E_PARAM; }
+        if (dst_off[i + 1] < dst_off[i]) { snprintf(g_err, sizeof g_err, "zip_extract: offsets of item %u decrease", i); return ZB_E_PARAM; }
+    }
+    const uint64_t out_total = nw ? dst_off[nw] - dst_off[0] : 0;
+    if ((out_total && !dst) || (!src && src_len)) { snprintf(g_err, sizeof g_err, "zip_extract: null buffer"); return ZB_E_PARAM; }
+    for (uint32_t i = 0; i < nw; i++) memset(&items[i], 0, sizeof items[i]);
+    if (nw == 0) return ZB_OK;
+    // the host decides what it can: refused entries, slots that are too small, and which path each of the others takes
+    enum : uint8_t { kRefused, kGroup, kStoredBig, kStream };
+    std::vector<uint8_t> cls(nw);
+    uint64_t small_total = 0, big_total = 0;
+    for (uint32_t i = 0; i < nw; i++) {
+        const zip::Entry &e = z->e[which ? which[i] : i];
+        zb_inflate_result &r = items[i];
+        cls[i] = kRefused;
+        if (e.flags & zip::kFlagEncrypted) { r.status = ZB_E_PARAM; snprintf(r.msg, sizeof r.msg, "encrypted entry"); }
+        else if (e.method != 0 && e.method != 8) { r.status = ZB_E_PARAM; snprintf(r.msg, sizeof r.msg, "unsupported compression method"); }
+        else if (dst_off[i + 1] - dst_off[i] < e.usize) { r.status = ZB_E_BUF; r.out_bytes = e.usize; }
+        else {
+            cls[i] = e.method == 0 ? (e.csize < ZB_ZIP_WARP_MAX ? kGroup : kStoredBig) : (e.usize < ZB_ZIP_WARP_MAX ? kGroup : kStream);
+            (cls[i] == kGroup ? small_total : big_total) += e.csize;
+        }
+    }
+    CKI(cudaSetDevice(device));
+    cudaEvent_t z0 = nullptr, z1 = nullptr;
+    CKI(cudaEventCreate(&z0));
+    if (cudaEventCreate(&z1) != cudaSuccess) { cudaEventDestroy(z0); snprintf(g_err, sizeof g_err, "zip_extract: cudaEventCreate"); return ZB_E_CUDA; }
+    struct Ev { cudaEvent_t a, b; ~Ev() { cudaEventDestroy(a); cudaEventDestroy(b); } } ev_guard{z0, z1};
+    int rc;
+    void *p;
+    uint32_t nl = 0;
+    // pinned staging: the group's table and results, then a host source's group payloads packed back to back (each below
+    // ZB_ZIP_WARP_MAX compressed bytes); larger payloads go up straight from the caller's memory
+    ZipItem *h_items = nullptr;
+    BatchResult *h_res = nullptr;
+    uint8_t *h_pack = nullptr;
+    if ((rc = carve(-1, [&](Carve &c) {
+             h_items = c.take<ZipItem>(nw);
+             h_res = c.take<BatchResult>(nw);
+             h_pack = c.take<uint8_t>(src_dev ? 0 : small_total + 1);
+         })) != ZB_OK)
+        return rc;
+    CKI(cudaEventRecord(z0, st));
+    std::vector<uint64_t> in_at(nw); // where entry i's payload lies in d_src
+    const uint8_t *d_src = static_cast<const uint8_t *>(src);
+    if (!src_dev) {
+        if ((rc = reserve(S_ZIPIN, small_total + big_total + 64, &p)) != ZB_OK) return rc;
+        d_src = static_cast<const uint8_t *>(p);
+        uint64_t at = 0, big_at = small_total;
+        for (uint32_t i = 0; i < nw; i++) {
+            const zip::Entry &e = z->e[which ? which[i] : i];
+            const uint8_t *h = static_cast<const uint8_t *>(src) + e.data_off;
+            if (cls[i] == kGroup) {
+                memcpy(h_pack + at, h, e.csize);
+                in_at[i] = at;
+                at += e.csize;
+            } else if (cls[i] != kRefused) {
+                CKI(cudaMemcpyAsync(static_cast<uint8_t *>(p) + big_at, h, e.csize, cudaMemcpyHostToDevice, st));
+                in_at[i] = big_at;
+                big_at += e.csize;
+            }
+        }
+        if (small_total) CKI(cudaMemcpyAsync(p, h_pack, small_total, cudaMemcpyHostToDevice, st));
+    } else {
+        for (uint32_t i = 0; i < nw; i++) in_at[i] = z->e[which ? which[i] : i].data_off;
+    }
+    uint8_t *d_dst = static_cast<uint8_t *>(dst) + dst_off[0];
+    if (!dst_dev) {
+        if ((rc = reserve(S_ZIPOUT, out_total + 64, &p)) != ZB_OK) return rc;
+        d_dst = static_cast<uint8_t *>(p);
+        CKI(cudaMemsetAsync(d_dst, 0, out_total, st)); // the slots go back whole: what lies behind an entry's output is zeros
+    }
+    // large entries one by one: a stored one is a device copy and a crc32; a deflated one takes the block-parallel decoder, and
+    // when that declines (stored or fixed-code blocks, damage) it joins the group, or below 4 GiB of output takes the serial decoder
+    for (uint32_t i = 0; i < nw; i++) {
+        if (cls[i] != kStoredBig && cls[i] != kStream) continue;
+        const zip::Entry &e = z->e[which ? which[i] : i];
+        zb_inflate_result &r = items[i];
+        uint8_t *o = d_dst + (dst_off[i] - dst_off[0]);
+        if (cls[i] == kStoredBig) {
+            const uint64_t nb = e.csize < e.usize ? e.csize : e.usize;
+            if (nb) CKI(cudaMemcpyAsync(o, d_src + in_at[i], nb, cudaMemcpyDeviceToDevice, st));
+            if ((rc = checksum(true, 0, o, nb, true, &r.check, nullptr)) != ZB_OK) return rc;
+            nl += launches;
+            r.out_bytes = r.in_bytes = nb;
+            const bool len_bad = nb != e.usize || e.csize != e.usize;
+            r.status = len_bad || r.check != e.crc ? ZB_E_DATA : ZB_OK;
+            if (r.status) snprintf(r.msg, sizeof r.msg, "%s", inf_msg(len_bad ? IE_LENGTH_CHECK : IE_DATA_CHECK));
+            continue;
+        }
+        zb_inflate_result s;
+        int st_ = ZB_E_DECLINED;
+        for (int pass = 0; pass < 2 && st_ == ZB_E_DECLINED; pass++) {
+            launches = 0;
+            memset(&s, 0, sizeof s);
+            st_ = inflate_stream(d_src + in_at[i], e.csize, o, e.usize, -15, ZB_INF_CHECK_CRC | (pass ? 0u : ZB_INF_NO_SERIAL), &s);
+            nl += launches;
+            if (st_ == ZB_E_DECLINED && e.usize < (1ull << 32)) break;
+        }
+        if (st_ == ZB_E_DECLINED) {
+            if (!dst_dev) CKI(cudaMemsetAsync(o, 0, dst_off[i + 1] - dst_off[i], st)); // what a declined replay left behind
+            cls[i] = kGroup;
+            continue;
+        }
+        if (st_ != ZB_OK && st_ != ZB_E_BUF && st_ != ZB_E_DATA) return st_;
+        r.out_bytes = s.out_bytes;
+        r.in_bytes = s.in_bytes;
+        r.check = s.check;
+        uint32_t err = IE_OK;
+        if (st_ == ZB_E_BUF) err = IE_LENGTH_CHECK;
+        else if (st_ == ZB_E_DATA) { r.status = ZB_E_DATA; snprintf(r.msg, sizeof r.msg, "%s", s.msg); continue; }
+        else if (s.in_bytes != e.csize) err = kZipBadEnd;
+        else if (s.out_bytes != e.usize) err = IE_LENGTH_CHECK;
+        else if (s.check != e.crc) err = IE_DATA_CHECK;
+        if (err != IE_OK) { r.status = ZB_E_DATA; snprintf(r.msg, sizeof r.msg, "%s", zip_msg(err)); }
+        if (err == IE_LENGTH_CHECK && st_ == ZB_E_BUF) r.out_bytes = e.usize;
+    }
+    // the group, side by side: stored entries first, then the deflated ones
+    uint32_t ng = 0, nstored = 0;
+    for (uint32_t i = 0; i < nw; i++)
+        if (cls[i] == kGroup) { ng++; nstored += z->e[which ? which[i] : i].method == 0; }
+    std::vector<uint32_t> gi(ng);
+    if (ng) {
+        ZipItem *d_items = nullptr;
+        BatchResult *d_res = nullptr;
+        uint64_t *d_ooff = nullptr;
+        uint32_t *d_clen = nullptr, *d_crc = nullptr;
+        InfState *d_ist = nullptr;
+        if ((rc = carve(S_ZIPTAB, [&](Carve &c) {
+                 d_items = c.take<ZipItem>(ng);
+                 d_res = c.take<BatchResult>(ng);
+                 d_ooff = c.take<uint64_t>(ng);
+                 d_clen = c.take<uint32_t>(ng);
+                 d_crc = c.take<uint32_t>(ng);
+                 d_ist = c.take<InfState>(ng);
+             })) != ZB_OK)
+            return rc;
+        uint32_t ks = 0, kd = nstored;
+        for (uint32_t i = 0; i < nw; i++) {
+            if (cls[i] != kGroup) continue;
+            const zip::Entry &e = z->e[which ? which[i] : i];
+            const uint32_t k = e.method == 0 ? ks++ : kd++;
+            gi[k] = i;
+            h_items[k] = ZipItem{in_at[i], e.csize, dst_off[i] - dst_off[0], e.usize, e.crc, e.method == 0 ? 1u : 0u};
+        }
+        CKI(cudaMemcpyAsync(d_items, h_items, ng * sizeof(ZipItem), cudaMemcpyHostToDevice, st));
+        if (nstored) { k_zip_stored<<<nstored, 256, 0, st>>>(d_src, d_items, d_dst, d_ist, d_ooff, d_clen); nl++; }
+        if (ng > nstored) {
+            k_zip_members<<<ng - nstored, 32, sizeof(InfShared), st>>>(d_src, d_items + nstored, d_dst, d_ist + nstored, d_ooff + nstored,
+                                                                     d_clen + nstored);
+            nl++;
+        }
+        CKI(launch_crc32_segments(d_dst, d_ooff, d_clen, ng, d_crc, st));
+        k_zip_verdict<<<(ng + 255) / 256, 256, 0, st>>>(d_items, d_ist, d_crc, ng, d_res);
+        nl += 2;
+        CKI(cudaMemcpyAsync(h_res, d_res, ng * sizeof(BatchResult), cudaMemcpyDeviceToHost, st));
+    }
+    if (!dst_dev && out_total) CKI(cudaMemcpyAsync(static_cast<uint8_t *>(dst) + dst_off[0], d_dst, out_total, cudaMemcpyDeviceToHost, st));
+    CKI(cudaEventRecord(z1, st));
+    CKI(cudaStreamSynchronize(st));
+    CKI(cudaGetLastError());
+    float ms = 0;
+    CKI(cudaEventElapsedTime(&ms, z0, z1));
+    for (uint32_t k = 0; k < ng; k++) {
+        zb_inflate_result &r = items[gi[k]];
+        const BatchResult &b = h_res[k];
+        r.out_bytes = b.out_bytes;
+        r.in_bytes = b.in_bytes;
+        r.check = b.check;
+        r.status = b.err == IE_OK ? ZB_OK : ZB_E_DATA;
+        if (r.status) snprintf(r.msg, sizeof r.msg, "%s", zip_msg(b.err));
+    }
+    launches = nl;
+    int status = ZB_OK;
+    for (uint32_t i = 0; i < nw; i++) {
+        items[i].gpu_launches = nl;
+        items[i].gpu_ms = ms;
+        if (status == ZB_OK) status = items[i].status;
     }
     return status;
 }
