@@ -459,8 +459,12 @@ ZB_API void zb_index_free(zb_index *idx);
  *                compressed size";
  *     ZB_E_BUF   the slot is smaller than the uncompressed size (nothing decoded);
  *     ZB_E_PARAM "unsupported compression method" or "encrypted entry" (flag bit 0).
- *   out_bytes, in_bytes (compressed bytes consumed) and check (crc32 of the output) are filled.  One bad entry never changes another's
- *   result; returns ZB_OK or the status of the first entry that failed.  which[i] out of range, more than 2^20 items, or src_len not
+ *   out_bytes, in_bytes (compressed bytes consumed) and check (crc32 of the output) are filled.  An entry that fails with ZB_E_DATA
+ *   keeps out_bytes <= the uncompressed size, its slot's first out_bytes bytes are output of the data (a stored entry's first
+ *   min(compressed, uncompressed size) bytes), check is their crc32 and in_bytes is at most the compressed size; where a deflated
+ *   entry's decode stops inside bad data is not promised.  No byte past the uncompressed size of a slot is written; behind
+ *   out_bytes a device slot holds its earlier bytes, or zeros where a declined block-parallel attempt was cleared.  One bad entry
+ *   never changes another's result; returns ZB_OK or the status of the first entry that failed.  which[i] out of range, more than 2^20 items, or src_len not
  *   the opened archive's length give ZB_E_PARAM.  A host source is not uploaded whole: only the selected entries' payloads go up --
  *   those below ZB_ZIP_WARP_MAX compressed bytes packed through the engine's pinned staging in one copy (so the staging grows to
  *   their sum, not to the archive's size), larger ones one copy each straight from src.  Paths: stored entries below

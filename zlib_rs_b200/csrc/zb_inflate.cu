@@ -2441,7 +2441,7 @@ __global__ void __launch_bounds__(32) k_zip_members(const uint8_t *__restrict__ 
     if (threadIdx.x == 0) {
         const InfState &r = ist[i];
         out_off[i] = it.out_off;
-        crc_len[i] = r.err == IE_OUTPUT_FULL ? 0u : (uint32_t)r.out_bytes; // the group's outputs are below 4 GiB (host check)
+        crc_len[i] = (uint32_t)r.out_bytes; // what was flushed to the slot, an output that stopped at the cap too; below 4 GiB (host check)
     }
 }
 
@@ -2459,7 +2459,8 @@ __global__ void __launch_bounds__(256) k_zip_verdict(const ZipItem *items, const
         else if (r.out_bytes != it.usize) err = IE_LENGTH_CHECK;
         else if (crc[i] != it.crc) err = IE_DATA_CHECK;
     }
-    out[i] = BatchResult{r.out_bytes, r.in_bytes, crc[i], err};
+    // the decoder reads zeros past the end of the input to find a truncation: what it consumed is never more than the payload
+    out[i] = BatchResult{r.out_bytes, r.in_bytes < it.in_len ? r.in_bytes : it.in_len, crc[i], err};
 }
 
 static const char *zip_msg(uint32_t e) { return e == kZipBadEnd ? "entry data does not end at its compressed size" : inf_msg(e); }
@@ -2583,14 +2584,20 @@ int Engine::zip_extract(const zb_zip *z, const void *src, size_t src_len, bool s
             if (st_ == ZB_E_DECLINED && e.usize < (1ull << 32)) break;
         }
         if (st_ == ZB_E_DECLINED) {
-            if (!dst_dev) CKI(cudaMemsetAsync(o, 0, dst_off[i + 1] - dst_off[i], st)); // what a declined replay left behind
+            // what a declined attempt left behind (at most usize bytes): the group's decode may stop short of it
+            if (e.usize) CKI(cudaMemsetAsync(o, 0, e.usize, st));
             cls[i] = kGroup;
             continue;
         }
         if (st_ != ZB_OK && st_ != ZB_E_BUF && st_ != ZB_E_DATA) return st_;
         r.out_bytes = s.out_bytes;
-        r.in_bytes = s.in_bytes;
+        r.in_bytes = s.in_bytes < e.csize ? s.in_bytes : e.csize;
         r.check = s.check;
+        // an output that stopped at the cap gets no check value from inflate_stream: the crc32 of what is in the slot
+        if (st_ == ZB_E_BUF) {
+            if ((rc = checksum(true, 0, o, s.out_bytes, true, &r.check, nullptr)) != ZB_OK) return rc;
+            nl += launches;
+        }
         uint32_t err = IE_OK;
         if (st_ == ZB_E_BUF) err = IE_LENGTH_CHECK;
         else if (st_ == ZB_E_DATA) { r.status = ZB_E_DATA; snprintf(r.msg, sizeof r.msg, "%s", s.msg); continue; }
@@ -2598,7 +2605,6 @@ int Engine::zip_extract(const zb_zip *z, const void *src, size_t src_len, bool s
         else if (s.out_bytes != e.usize) err = IE_LENGTH_CHECK;
         else if (s.check != e.crc) err = IE_DATA_CHECK;
         if (err != IE_OK) { r.status = ZB_E_DATA; snprintf(r.msg, sizeof r.msg, "%s", zip_msg(err)); }
-        if (err == IE_LENGTH_CHECK && st_ == ZB_E_BUF) r.out_bytes = e.usize;
     }
     // the group, side by side: stored entries first, then the deflated ones
     uint32_t ng = 0, nstored = 0;
